@@ -2,7 +2,7 @@
 """Benchmark of the PLAID search hot path (BASELINE.json metric: queries/sec @ top_k=100 on a
 1M-doc x 300-tok x 128-dim index; MaxSim HBM GB/s vs roofline).
 
-    python bench.py --gpus 1 --steps 5 --warmup 3                # B200 engine (default)
+    python bench.py --gpus 1 --steps 5 --warmup 3                # the engine (default)
     python bench.py --impl reference --gpus 1 --steps 5 --warmup 3   # the reference's CPU path
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...   # document-sharded
 
@@ -10,7 +10,8 @@ A "step" is one batch of 64 queries x 32 tokens through the whole hot path.  `va
 queries/sec with the queries already resident in HBM (stage by stage through the C ABI, CUDA
 events between the stages); `e2e` is the same through the user-facing call
 `FastPlaid.search(fp32 host queries, top_k=...)` -> `list[list[(doc_id, score)]]`, host<->device
-copies inside the timed region.  One JSON line on stdout.
+copies inside the timed region.  One JSON line on stdout.  `--dump-outputs DIR` writes what the
+timed path returned in its last step (ids, scores, counts per query) as DIR/<name>.npy.
 
 Parity is part of the line: `parity_sample` runs the CPU oracle on the first queries of a batch, at
 any number of GPUs, and classifies every difference between the engine's id lists and the oracle's.
@@ -59,15 +60,7 @@ PARITY_QUERIES = 16  # queries cross-checked against the oracle (and classified)
 
 
 # ----------------------------------------------------------------------------------------
-def measured_peak_hbm() -> tuple[float, str]:
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        try:
-            with open(p) as f:
-                return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet: 3.35 TB/s of HBM3 (a data-sheet figure, not a measured one)
 
 
 class ClockSampler:
@@ -230,27 +223,15 @@ def approx_algorithmic_bytes(didx, views, lay) -> tuple[int, int]:
     return hbm, tokens
 
 
-def traffic_for(config: str, world: int):
-    """ncu dram__bytes_read+write of the MaxSim kernel per launch, from the capture committed for exactly this
-    (config, world size); None when there is none."""
-    tp = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        with open(tp) as f:
-            entry = json.load(f).get(f"{config}@{world}")
-        return (entry or {}).get("k5_maxsim_dram_bytes_per_launch"), (entry or {}).get("source")
-    except Exception:
-        return None, None
-
-
-HBM_INDEX_BUDGET = 60e9  # bytes of one GPU's 180 GB given to index data; the rest is score table, workspace, headroom
+HBM_INDEX_BUDGET = 48e9  # bytes of one H100's 80 GB given to index data; the rest is score table, workspace, headroom
 
 
 def default_query_groups(world: int, cfg: dict) -> int:
     """Grid policy: the FEWEST document shards whose slice fits the per-GPU budget, every other rank a query group.
     Splitting the queries costs nothing (they are independent; each rank runs K1 / the probe on its own B / groups
     queries), splitting the documents repeats those stages on every shard and adds the pruning exchange -- measured
-    on cfg3: 2 x 1 beats 1 x 2 by 11 %, 4 x 1 beats 2 x 2 by 6 % (profiles/r02_summary.md).  Documents are sharded
-    when the index needs it (or on request: --query-groups)."""
+    on cfg3 (2 x 1 against 1 x 2, 4 x 1 against 2 x 2).  Documents are sharded when the index needs it (or on
+    request: --query-groups)."""
     tokens = cfg["n_docs"] * cfg["doc_len"]
     index_bytes = tokens * (DIM * NBITS // 8 + 4 + 2 + 4)  # residuals, int32 code, fp16 norm, inverted-file entry
     for n_shards in range(1, world + 1):
@@ -377,11 +358,12 @@ def run_b200(args) -> dict:
                 e0 = torch.cuda.Event(enable_timing=True)
                 e0.record()
                 events.append(e0)
-            didx.search_sharded(comm, n_groups, qb, params)
+            out = didx.search_sharded(comm, n_groups, qb, params)
             if events is not None:
                 e1 = torch.cuda.Event(enable_timing=True)
                 e1.record()
                 events.append(e1)
+            return out
 
     for w in range(args.warmup):
         one_step(q_dev16[w % N_QUERY_BATCHES], None)
@@ -396,10 +378,12 @@ def run_b200(args) -> dict:
     t_wall0 = time.time()
     for s in range(args.steps):
         ev: list = []
-        one_step(q_dev16[s % N_QUERY_BATCHES], ev)
+        last = one_step(q_dev16[s % N_QUERY_BATCHES], ev)
         all_events.append(ev)
     barrier()
     t_wall = time.time() - t_wall0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *(last if world > 1 else (ids, scores, counts)))
     total_ms = all_events[0][0].elapsed_time(all_events[-1][-1])
     stage_ms = [0.0] * len(stage_names)
     for ev in all_events:
@@ -442,7 +426,7 @@ def run_b200(args) -> dict:
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
     total_ms, e2e_ms = float(tt[0]), float(tt[1])
 
-    peak, peak_src = measured_peak_hbm()
+    peak, peak_src = HBM_PEAK_GBS, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
     if world > 1:
         # stage breakdown of the sharded step: the same sequence once more through the step-wise entry points, the two
         # all-gathers issued through torch.distributed here (the timed product path issues them below the C ABI)
@@ -526,7 +510,6 @@ def run_b200(args) -> dict:
     i_ap = stage_names.index("approx")
     ms_time = stage_ms[i_ms] / 1000.0
     achieved = ms_bytes / ms_time / 1e9 if ms_time > 0 else 0.0
-    traffic, traffic_src = traffic_for(args.config, world)
     h2d = B * Q * DIM * 2
     d2h = B * k * 12 + B * 4
     n_launch = count_launches(world, args.approx)
@@ -565,7 +548,7 @@ def run_b200(args) -> dict:
         "roofline": {"kernel": ("k5_maxsim_v4_kernel" if Q <= 32 else "k5_maxsim_v5_kernel") +
                                " (fused residual decompression + MaxSim)", "bound": "hbm",
                      "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak if peak else None,
-                     "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                     "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": ms_bytes, "launch_ms": stage_ms[i_ms]},
         "stages_ms": dict(zip(stage_names, [round(x, 4) for x in stage_ms])),
         "approx_stage": {"mode": args.approx,
@@ -611,6 +594,18 @@ def run_b200(args) -> dict:
         dist.barrier()
         dist.destroy_process_group()
     return out if rank == 0 else {}
+
+
+def dump_outputs(out_dir: str, ids: torch.Tensor, scores: torch.Tensor, counts: torch.Tensor) -> None:
+    """The last timed step's results as DIR/<name>.npy: ids (float64, exact below 2**53; -1 past a query's count),
+    scores (float32) and counts (float64), [B, top_k] / [B]."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "ids.npy"), ids.cpu().numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "scores.npy"), scores.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "counts.npy"), counts.cpu().numpy().astype(np.float64))
 
 
 def count_launches(world: int, approx: str) -> int:
@@ -998,6 +993,8 @@ def main() -> None:
                          "shards that fit the per-GPU budget)")
     ap.add_argument("--approx", choices=["two-pass", "direct"], default="two-pass",
                     help="approximate stage: exact two-pass pruning (default) or the one-pass A/B alternative")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's ids / scores / counts as DIR/<name>.npy")
     args = ap.parse_args()
     # keep stdout clean for the ONE JSON line: NCCL / libraries may print to fd 1
     sys.stdout.flush()

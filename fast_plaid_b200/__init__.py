@@ -1,4 +1,4 @@
-"""fast_plaid_b200 -- a B200-native (sm_100a) PLAID search engine behind the FastPlaid surface.
+"""fast_plaid_b200 -- an H100-native (sm_90a) PLAID search engine behind the FastPlaid surface.
 
     from fast_plaid_b200 import search
     index = search.FastPlaid(index="my_index", device="cuda:0")

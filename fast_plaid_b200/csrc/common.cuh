@@ -1,4 +1,4 @@
-// Shared definitions for the sm_100a PLAID search kernels.
+// Shared definitions for the sm_90a PLAID search kernels.
 #pragma once
 
 #include <cuda_fp16.h>

@@ -5,8 +5,7 @@
 // The reference gathers S rows into a [tokens, Q] tensor, pads it to [2000, maxlen, Q], masks, maxes and
 // sums, 128 times per query with two host syncs each.  A one-pass GPU formulation (one warp walks one
 // candidate, every token gathers its Qp*2-byte S row) is bound by the L1 data pipe: one wavefront per
-// gathered row, 4.87 G rows per batch on cfg-3 = 16.8 ms at one wavefront per clock per SM, and the kernel
-// sat at 97 % of that (profiles/r01c_k3_approx_nsh_raw.csv).  Going faster needs FEWER ROWS, exactly:
+// gathered row, 4.87 G rows per batch on cfg-3.  Going faster needs FEWER ROWS, exactly:
 //
 //   1. tau[b,q]   = a quantile of the per-128-centroid-tile column maxima K1 already produces
 //                   (any value is correct; it only moves work between the two passes)
@@ -340,7 +339,7 @@ k3_tau_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __r
           const int t = base + lane;
           const int code = (t < len) ? __ldg(codes + o0 + t) : -1;
           // all LPR row gathers of the window go out before the first histogram update (the kernel is a chain of
-          // dependent latencies otherwise: 0.33 ms with the loads issued one per update round)
+          // dependent latencies otherwise)
           constexpr int JB = LPR < 8 ? LPR : 8;  // gathers in flight per lane
 #pragma unroll 1
           for (int j0 = 0; j0 < LPR; j0 += JB) {
@@ -450,9 +449,9 @@ k3_hibits_kernel(const __half* __restrict__ S, int64_t K, const __half* __restri
 // lengths of the chunk's documents (staged by the first K3A_DOCS_PER_CHUNK threads so that the dependent
 // candidate -> offset loads are paid once per chunk, not once per document).  A warp walks its documents as a stream
 // of W-window groups and always has the NEXT group's code loads in flight while it tests, queues and gathers the
-// current one.  The first version of this kernel was ISSUE-bound (profiles/r02_k3_bound_v1_raw.csv: 15.3 G warp
-// instructions, 91 per 32-token window, issue slots 81 % busy; a third of them branches and generic-address
-// arithmetic around the shared-memory accesses), so the per-window path is written branch-free with explicit 32-bit
+// current one.  A straightforward version of this kernel is ISSUE-bound (about 90 warp instructions per 32-token
+// window, a third of them branches and generic-address arithmetic around the shared-memory accesses), so the
+// per-window path is written branch-free with explicit 32-bit
 // shared addresses: predicated code load, one LDS of the bitmap word, a wrap-around funnel shift for the bit, ballot,
 // predicated STS into the ring.  Tokens outside the document carry the code K3_INV whose bit is a spare zero word.
 __device__ __forceinline__ uint32_t k3_lds(uint32_t addr) {
@@ -1174,7 +1173,7 @@ int launch_k3_exact(const fpb_index* ix, const Ws& ws, const int32_t* list, cons
   const int blocks = ix->sm_count * 8;
   if constexpr (LPR <= 4) {
     // shuffle-free up to Qp = 32 (the vector code loads need a 16-byte aligned code array; any torch allocation
-    // is); at Qp = 64 the shuffle kernel is faster (cfg-5: 10.55 vs 11.31 ms)
+    // is); at Qp = 64 the shuffle kernel is used
     if ((reinterpret_cast<uintptr_t>(ix->doc_codes) & 15u) == 0) {
       k3_approx_nsh_kernel<LPR, 2, 6><<<blocks, K3_THREADS, 0, st>>>(
           ws.S(), ix->K, L.Q, ix->doc_offsets, ix->doc_codes, ix->E, ws.cand(), L.cand_cap, ws.n_cand(), list, n_list,
@@ -1192,7 +1191,7 @@ int launch_k3_exact(const fpb_index* ix, const Ws& ws, const int32_t* list, cons
 
 // LAMBDA of k3_tau_kernel: the expected number of tokens per candidate and column at or above tau.  A document is
 // resolved when all of its Q columns are, so the useful level grows with log Q: LAMBDA = ln(Q) - 1.45 (2.0 at
-// Q = 32, 2.7 at Q = 64; measured optimum on cfg-3, within 10 % of it on cfg-5).  FPB_K3_LAMBDA overrides it
+// Q = 32, 2.7 at Q = 64).  FPB_K3_LAMBDA overrides it
 // (tuning only: every value gives the same results).
 float k3_tau_lambda(int Q) {
   static const float pinned = [] {
@@ -1230,9 +1229,7 @@ int launch_k3_t(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st) {
   {
     // resident CTAs per SM: limited by the bitmap (228 KB of shared memory per SM, 1 KB reserved per CTA)
     // shape of the walk: 6 32-token windows per group (all their code loads in flight at once, the next group's
-    // prefetched), 4 gathers per lane and batch, 4 CTAs per SM at 64 registers, paired epilogues.  Measured
-    // alternatives (profiles/r02_summary.md): 4 / 8 / 11 / 12 windows, 2 / 8 gathers, 5-6 CTAs at 48 / 40 registers,
-    // one document per epilogue -- all within 3 % or slower.
+    // prefetched), 4 gathers per lane and batch, 4 CTAs per SM at 64 registers, paired epilogues.
     constexpr int TPI = 32 / LPR;
     constexpr int W = 6, U = 4, MINB = 4;
     const bool fullq = L.Q == L.Qp;

@@ -34,7 +34,7 @@ struct Ws {
 
 int launch_pad_queries(const fpb_index* ix, const Ws& ws, const __half* d_queries, cudaStream_t st);
 int launch_centroid_scores(const fpb_index* ix, const Ws& ws, cudaStream_t st);   // K1 (dispatch)
-int launch_centroid_scores_v2(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K1 on tcgen05
+int launch_centroid_scores_v2(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K1 on wgmma
 int launch_probe(const fpb_index* ix, const Ws& ws, bool subset, cudaStream_t st);       // K1b
 int launch_candidates(const fpb_index* ix, const Ws& ws, bool subset, cudaStream_t st);  // K2
 int launch_subset_mark(const fpb_index* ix, const Ws& ws, const int32_t* d_ids, const int64_t* d_offsets,
@@ -50,7 +50,7 @@ int launch_select(const fpb_index* ix, const Ws& ws, cudaStream_t st);          
 int launch_maxsim(const fpb_index* ix, const Ws& ws, cudaStream_t st);            // K5 (dispatch)
 int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st);      // per-token fp16 norms (index load)
 int launch_maxsim_v4(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K5 v4 (register operands)
-int launch_maxsim_v5(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K5 v5 (tcgen05, 20 decode warps)
+int launch_maxsim_v5(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K5 v5 (wgmma, 16 decode warps)
 int launch_rank(const fpb_index* ix, const Ws& ws, int top_k, int64_t* d_out_ids, float* d_out_scores,
                 int32_t* d_out_counts, cudaStream_t st);                          // K6
 int launch_emit_keys(const fpb_index* ix, const Ws& ws, uint64_t* d_keys, cudaStream_t st);

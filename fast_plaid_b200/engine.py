@@ -249,16 +249,16 @@ def _check(rc: int) -> None:
 def _require_cuda() -> None:
     if not torch.cuda.is_available():
         raise EngineUnavailableError(
-            "fast_plaid_b200 needs a CUDA device (B200, sm_100a); there is no CPU search path."
+            "fast_plaid_b200 needs a CUDA device (H100, sm_90a); there is no CPU search path."
         )
 
 
 def check_supported(dim: int, nbits: int) -> None:
     """The engine's compiled limits (csrc/index.cu fpb_index_create): raise before an index is written."""
     if int(nbits) not in (2, 4):
-        raise ValueError(f"unsupported nbits={nbits}: the B200 engine supports nbits 2 and 4")
+        raise ValueError(f"unsupported nbits={nbits}: the engine supports nbits 2 and 4")
     if int(dim) not in (64, 128):
-        raise ValueError(f"unsupported embedding dim={dim}: the B200 engine supports dim 64 and 128")
+        raise ValueError(f"unsupported embedding dim={dim}: the engine supports dim 64 and 128")
 
 
 def _ptr(t: torch.Tensor | None) -> int | None:
@@ -490,7 +490,7 @@ class DeviceIndex:
         self._lib = load_library()
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise ValueError(f"Unsupported device string: '{device}' (the B200 engine runs on CUDA only)")
+            raise ValueError(f"Unsupported device string: '{device}' (the engine runs on CUDA only)")
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
         dev = self.device

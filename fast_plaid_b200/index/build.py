@@ -9,8 +9,8 @@ Same algorithm and on-disk result as the reference's ``compute_kmeans`` + ``crea
   4. inverted file: per centroid, sorted unique doc ids
 
 This module is not on the search hot path; it runs on whichever torch device it is given
-(CUDA on the B200 box, CPU in the container's tests) with dense torch ops.  The encode step
-(argmax GEMM + bucketize + pack) runs in the sm_100a kernels behind `fpb_encode`
+(CUDA on the GPU, CPU in the non-GPU tests) with dense torch ops.  The encode step
+(argmax GEMM + bucketize + pack) runs in the sm_90a kernels behind `fpb_encode`
 (csrc/encode.cu) when the tokens are on CUDA with dim=128; elsewhere it is dense torch ops.
 """
 
@@ -89,7 +89,7 @@ def lloyd_kmeans(data: torch.Tensor, k: int, niters: int, seed: int, device: tor
 
 def _lloyd_kmeans_b200(data: torch.Tensor, centroids: torch.Tensor, niters: int, n: int,
                        device: torch.device, chunk: int = 4_000_000) -> torch.Tensor:
-    """The same Lloyd iterations on the sm_100a kernels (csrc/encode.cu): the assignment is the tcgen05 argmax
+    """The same Lloyd iterations on the sm_90a kernels (csrc/encode.cu): the assignment is the wgmma argmax
     GEMM with a -|c|^2/2 bias in the epilogue (fpb_kmeans_assign), the update a deterministic segmented mean
     (fpb_kmeans_update); empty clusters are re-seeded from random points and the loop stops on a zero shift, as
     kmeans.py:196-218 does.  The points are staged to the GPU in `chunk`-row pieces when they live on the host."""
@@ -207,7 +207,7 @@ def train_codec(docs: list[torch.Tensor], centroids: torch.Tensor, nbits: int, s
 def encode(batch: torch.Tensor, centroids: torch.Tensor, centroids_t: torch.Tensor, cutoffs: torch.Tensor,
            nbits: int) -> tuple[torch.Tensor, torch.Tensor]:
     """One batch of fp16 token rows -> (codes int64, packed residual bytes) (create.rs:404-428).
-    On a CUDA device with dim = 128 this is the sm_100a encode kernel pair (tcgen05 argmax GEMM +
+    On a CUDA device with dim = 128 this is the sm_90a encode kernel pair (wgmma argmax GEMM +
     bucketize/pack, csrc/encode.cu); otherwise dense torch ops."""
     if batch.is_cuda and batch.shape[1] == 128 and nbits in (2, 4):
         from ..engine import encode_tokens

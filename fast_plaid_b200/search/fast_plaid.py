@@ -1,9 +1,9 @@
-"""The FastPlaid Python surface on top of the B200 engine.
+"""The FastPlaid Python surface on top of the H100 engine.
 
 Same class, method names, argument meaning and error behaviour as the reference's
 ``fast_plaid.search.FastPlaid`` (python/fast_plaid/search/fast_plaid.py:325-1186), same index
 directory on disk, PyTorch tensors in and ``list[list[(doc_id, score)]]`` out.  What differs
-is underneath: the whole query batch goes through one C-ABI call into hand-written sm_100a
+is underneath: the whole query batch goes through one C-ABI call into hand-written sm_90a
 kernels (``fast_plaid_b200/csrc``) instead of a per-query loop of ATen ops, and with several
 GPUs the index is sharded by document (one process per GPU, NCCL all-gather of per-shard
 records) instead of replicated.
@@ -96,7 +96,7 @@ class FastPlaid:
     ) -> None:
         """``index``/``device``/``low_memory`` as in the reference (fast_plaid.py:328-385).
 
-        ``low_memory`` is accepted and ignored: a B200 holds the whole index in HBM.
+        ``low_memory`` is accepted and ignored: the GPU holds the whole index in HBM.
         ``shard``: ``(rank, world)`` makes this process one rank of the document-sharded search (one
         process per GPU; both exchanges are NCCL all-gathers issued below the C ABI, csrc/comm.cu);
         ``"auto"`` takes rank/world from an initialised process group.  ``query_groups`` (a divisor of

@@ -1,5 +1,5 @@
 /*
- * fastplaid_b200.h -- C ABI of the B200-native PLAID search engine.
+ * fastplaid_b200.h -- C ABI of the H100-native PLAID search engine.
  *
  * This is the drop-in boundary for the search hot path of lightonai/fast-plaid
  * (v1.4.6 @ 87f96f6).  In the reference that path sits behind the PyO3 module

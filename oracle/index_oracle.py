@@ -4,8 +4,8 @@ TEST INFRASTRUCTURE ONLY -- see the header of ``plaid_oracle.py`` for the import
 Restates, op for op in PyTorch-CPU, ``create_index`` (rust/index/create.rs:206-585) for a
 given centroid table, plus the K heuristic and normalisation of ``compute_kmeans``
 (python/fast_plaid/search/fast_plaid.py:71-185) with a plain Lloyd k-means standing in
-for the third-party ``fastkmeans==0.5.0`` dependency (pyproject.toml:30; absent from
-/root/reference and from this image).  The in-tree chunked Lloyd loop that the reference
+for the third-party ``fastkmeans==0.5.0`` dependency (pyproject.toml:30; not part of the
+fast-plaid source tree).  The in-tree chunked Lloyd loop that the reference
 layers on it (python/fast_plaid/search/kmeans.py:60-223) is what ``kmeans`` follows.
 
 Two things cannot be reproduced bit-for-bit and are documented instead:

@@ -1,6 +1,6 @@
 """CPU oracle for the fast-plaid search hot path.  TEST INFRASTRUCTURE ONLY.
 
-This module is the parity checker for the B200 engine.  Only ``tests/``,
+This module is the parity checker for the H100 engine.  Only ``tests/``,
 ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` / ``--impl reference``
 legs may import it.  Nothing under ``fast_plaid_b200/`` imports it, and the product
 path never falls back to it.

@@ -1,13 +1,15 @@
 """Mint tests/golden/kmeans_ref.pt by running the REFERENCE's own k-means code.
 
 The Lloyd loop the reference layers on the (absent) third-party `fastkmeans` package lives in
-/root/reference/python/fast_plaid/search/kmeans.py:60-223 and is plain PyTorch.  This script
+python/fast_plaid/search/kmeans.py:60-223 of a lightonai/fast-plaid checkout and is plain PyTorch.  This script
 imports that file unmodified -- only `fastkmeans` itself is stubbed with an empty base class --
 seeds the RNG exactly as `FastKMeans.train` does (kmeans.py:236-238) and records inputs and
 outputs.  tests/test_oracle.py then requires oracle/index_oracle.py::kmeans to reproduce the
-recorded centroids, which pins that part of the oracle on reference outputs.
+recorded centroids, which pins that part of the oracle on reference outputs.  A second file,
+kmeans_ref_seed99.pt, holds the reference's centroids for one more problem that the test
+regenerates from its seed.
 
-Run in the build container (needs /root/reference):  python tests/golden/make_kmeans_golden.py
+    python tests/golden/make_kmeans_golden.py <path to a fast-plaid checkout>
 """
 
 import importlib.util
@@ -18,11 +20,18 @@ import types
 import numpy as np
 import torch
 
-REF = "/root/reference/python/fast_plaid/search/kmeans.py"
-OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "kmeans_ref.pt")
+HERE = os.path.dirname(os.path.abspath(__file__))
+OUT = os.path.join(HERE, "kmeans_ref.pt")
+OUT_SEED99 = os.path.join(HERE, "kmeans_ref_seed99.pt")
 
 
-def load_reference_kmeans():
+def seed99_problem() -> torch.Tensor:
+    """The extra problem of kmeans_ref_seed99.pt (k=32, niters=3, seed=5, max_points_per_centroid=256)."""
+    g = torch.Generator().manual_seed(99)
+    return torch.nn.functional.normalize(torch.randn(1500, 24, generator=g), dim=-1).half()
+
+
+def load_reference_kmeans(checkout: str):
     stub = types.ModuleType("fastkmeans")
 
     class FastKMeans:  # the third-party base class; never instantiated here
@@ -30,7 +39,8 @@ def load_reference_kmeans():
 
     stub.FastKMeans = FastKMeans
     sys.modules.setdefault("fastkmeans", stub)
-    spec = importlib.util.spec_from_file_location("ref_kmeans", REF)
+    ref = os.path.join(checkout, "python", "fast_plaid", "search", "kmeans.py")
+    spec = importlib.util.spec_from_file_location("ref_kmeans", ref)
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
     return mod
@@ -49,7 +59,7 @@ def run_case(mod, data_f16: torch.Tensor, k: int, niters: int, seed: int, mppc: 
 
 def main():
     torch.set_num_threads(1)  # the fixture must not depend on the blocking of a threaded GEMM
-    mod = load_reference_kmeans()
+    mod = load_reference_kmeans(sys.argv[1])
     g = torch.Generator().manual_seed(2024)
     cases = []
     # (n, dim, k, niters, seed, max_points_per_centroid)
@@ -67,6 +77,10 @@ def main():
                           "torch " + torch.__version__ + ", CPU, 1 thread",
                 "cases": cases}, OUT)
     print("wrote", OUT, os.path.getsize(OUT), "bytes")
+    c, _ = run_case(mod, seed99_problem(), 32, 3, 5, 256)
+    torch.save({"source": "reference python/fast_plaid/search/kmeans.py::_kmeans_torch_double_chunked, "
+                          "torch " + torch.__version__ + ", CPU, 1 thread", "centroids": c}, OUT_SEED99)
+    print("wrote", OUT_SEED99, os.path.getsize(OUT_SEED99), "bytes")
 
 
 if __name__ == "__main__":

@@ -54,8 +54,8 @@ def test_grid_policy_uses_the_fewest_document_shards_that_fit():
 
     for world in (1, 2, 4, 8):
         assert bench.default_query_groups(world, bench.CONFIGS["cfg3"]) == world
-    big = dict(n_docs=10_000_000, doc_len=300)  # ~220 GB of index data
-    assert bench.default_query_groups(8, big) == 2  # 4 shards of 55 GB, two query groups
+    big = dict(n_docs=6_000_000, doc_len=300)  # ~133 GB of index data
+    assert bench.default_query_groups(8, big) == 2  # 4 shards of 33 GB, two query groups
     assert bench.default_query_groups(4, big) == 1
     assert bench.default_query_groups(2, big) == 1  # does not fit at all: as many shards as there are ranks
     for world in (2, 4, 8):

@@ -61,7 +61,7 @@ def test_create_on_gpu_uses_the_kernels_and_matches_the_cpu_builder(tmp_path, cu
 
 
 def test_kmeans_kernels_match_torch(cuda_device):
-    """fpb_kmeans_assign (tcgen05 argmax of <x,c> - |c|^2/2) against the fp32 nearest-centroid search, and
+    """fpb_kmeans_assign (wgmma argmax of <x,c> - |c|^2/2) against the fp32 nearest-centroid search, and
     fpb_kmeans_update (deterministic segmented mean) against index_add_; un-normalised centroids, K not a
     multiple of 128, a cluster left empty."""
     from fast_plaid_b200.engine import kmeans_assign, kmeans_update
@@ -101,7 +101,7 @@ def test_kmeans_kernels_match_torch(cuda_device):
 
 
 def test_gpu_lloyd_kmeans_reaches_the_quality_of_the_cpu_loop(cuda_device):
-    """The sm_100a Lloyd loop and the oracle's CPU loop start from the same seeded initial centroids and must end
+    """The sm_90a Lloyd loop and the oracle's CPU loop start from the same seeded initial centroids and must end
     at the same clustering quality (inertia within 2 %): the reference's own CUDA path differs from its CPU path
     in exactly this way (fp16 tensor-core distances, kmeans.py:113-114)."""
     from fast_plaid_b200.index import build

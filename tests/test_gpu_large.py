@@ -121,7 +121,7 @@ def test_sharded_equals_unsharded_at_size(big, cuda_device):
 
 def test_cfg2_built_by_create_searches_like_the_oracle(tmp_path, cuda_device):
     """BASELINE config 2 end to end through the public surface: 100k documents x 300 tokens built by
-    FastPlaid.create() on the GPU (k-means on the sm_100a assign/update kernels, streaming chunk encode, K = 65536),
+    FastPlaid.create() on the GPU (k-means on the sm_90a assign/update kernels, streaming chunk encode, K = 65536),
     loaded by the direct-to-device loader, searched with B = 64, Q = 32, top_k = 100.  For 8 queries every integer
     stage must equal the canonical oracle given the GPU's own S -- probed cells, candidates, approximate scores
     (or the pruned list from the GPU's approximate scores when a fp32 sum rounds differently), pruned list -- and

@@ -1,12 +1,12 @@
-"""Index directory layout: the product's builder/reader against the oracle's builder and --
-when /root/reference is mounted -- against the reference's own Python loader."""
+"""Index directory layout: the product's builder/reader against the oracle's builder and against what
+the reference's own Python loader read from a directory this builder wrote."""
 
 from __future__ import annotations
 
 import json
 import os
+import shutil
 import sys
-import types
 
 import numpy as np
 import pytest
@@ -75,32 +75,24 @@ def test_ivf_lists_are_sorted_unique_and_consistent(built):
         assert set(lst.tolist()) == set(tok2doc[data.doc_codes == c].tolist())
 
 
-REF_PY = "/root/reference/python"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_PY), reason="reference tree not mounted (GPU box)")
-def test_reference_loader_reads_our_directory_identically(built, monkeypatch):
-    """Pin the on-disk format against the reference's OWN loader
-    (python/fast_plaid/search/load.py:220-322).  Its module imports the Rust extension and the
-    third-party fastkmeans at import time; both are stubbed -- the loader code that runs is the
-    reference's, unmodified, read from /root/reference."""
-    path, _ = built
-    stub = types.ModuleType("fast_plaid.fast_plaid_rust")
-    pkg = types.ModuleType("fast_plaid")
-    pkg.__path__ = [os.path.join(REF_PY, "fast_plaid")]
-    pkg.fast_plaid_rust = stub
-    srch = types.ModuleType("fast_plaid.search")
-    srch.__path__ = [os.path.join(REF_PY, "fast_plaid", "search")]
-    monkeypatch.setitem(sys.modules, "fast_plaid", pkg)
-    monkeypatch.setitem(sys.modules, "fast_plaid.fast_plaid_rust", stub)
-    monkeypatch.setitem(sys.modules, "fast_plaid.search", srch)
-    import importlib.util
+def test_reference_loader_reads_our_directory_identically(tmp_path):
+    """Pin the on-disk format against the reference's OWN loader (python/fast_plaid/search/load.py:220-322).
+    tests/golden/ref_loader_index/ was written by this builder and read by the reference's loader, unmodified;
+    tests/golden/ref_loader.pt holds what that loader returned (tests/golden/make_loader_golden.py).  Our reader
+    must return the same tensors, and a fresh build of the same documents must still write that directory's
+    files with the same dtypes and shapes."""
+    sys.path.insert(0, GOLDEN)
+    import make_loader_golden as mk
 
-    spec = importlib.util.spec_from_file_location("fast_plaid.search.load",
-                                                  os.path.join(REF_PY, "fast_plaid", "search", "load.py"))
-    ref_load = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref_load)
-    ref = ref_load._load_index_tensors_cpu(index_path=path)
+    path = str(tmp_path / "golden_copy")
+    shutil.copytree(os.path.join(GOLDEN, "ref_loader_index"), path)
+    ref = torch.load(os.path.join(GOLDEN, "ref_loader.pt"), weights_only=False)
+    assert "reference" in ref["source"]
+    # the merged mmap cache the reference wrote is in the directory and does not confuse our reader
+    assert os.path.exists(os.path.join(path, "merged_codes.npy"))
     ours = store.read_index(path)
     n_tok = int(ours.doc_lengths.sum())
     assert ref["nbits"] == ours.nbits
@@ -113,11 +105,17 @@ def test_reference_loader_reads_our_directory_identically(built, monkeypatch):
     assert torch.equal(ref["doc_codes"][:n_tok], ours.doc_codes)
     assert torch.equal(ref["doc_residuals"][:n_tok], ours.doc_residuals)
     assert ref["doc_codes"].shape[0] - n_tok == int(ours.doc_lengths.max() - ours.doc_lengths[-1])
-    # the merged mmap cache the reference wrote does not confuse our reader
-    again = store.read_index(path)
-    assert torch.equal(again.doc_codes, ours.doc_codes)
-    for f in ("merged_codes.npy", "merged_residuals.npy", "merged_codes.manifest.json", "merged_residuals.manifest.json"):
-        os.remove(os.path.join(path, f))
+
+    fresh = str(tmp_path / "fresh")
+    mk.build_index(fresh)
+    for f in sorted(os.listdir(path)):
+        if f.startswith("merged_"):
+            continue
+        if f.endswith(".npy"):
+            a, b = np.load(os.path.join(path, f)), np.load(os.path.join(fresh, f))
+            assert (a.dtype, a.shape) == (b.dtype, b.shape), f
+        else:
+            assert os.path.exists(os.path.join(fresh, f)), f
 
 
 def test_pack_buckets_is_the_reference_bit_order():
