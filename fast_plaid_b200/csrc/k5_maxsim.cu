@@ -15,6 +15,7 @@
 // v1 data path: mma.sync m16n8k16 (legacy tensor path) with a CTA of 4 warps per document.
 #include <stdlib.h>
 
+#include "decode.cuh"
 #include "kernels.h"
 
 namespace {
@@ -27,72 +28,6 @@ struct K5Smem {
   static constexpr int LDS = D + 8;
   static constexpr int bytes = (K5_TILE * LDS + QP * LDS) * 2 + 4 * QP * 2 + 256 * 8;
 };
-
-// Decode `NB` packed bytes of one token slice and add the centroid slice.
-// nbits=4: byte -> elements (2i, 2i+1) = (w_perm[b>>4], w_perm[b&15])      (Appendix B of SURVEY.md)
-// nbits=2: byte -> elements 4i..4i+3  = w_perm[(b>>6)&3], [(b>>4)&3], [(b>>2)&3], [b&3]
-template <int NBITS>
-struct Decoder;
-
-template <>
-struct Decoder<4> {
-  static constexpr int EL_PER_BYTE = 2;
-  // lut: 256 x half2
-  __device__ static void build(uint32_t* lut, const WPerm& wp, int tid, int nthreads) {
-    for (int v = tid; v < 256; v += nthreads) lut[v] = uint32_t(wp.v[v >> 4]) | (uint32_t(wp.v[v & 15]) << 16);
-  }
-  // 16 bytes -> 16 half2
-  __device__ __forceinline__ static void decode16(const uint32_t* lut, const uint4& rv, const uint4* cent,
-                                                  __half2 (&e)[16]) {
-    const uint32_t w[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-    for (int wi = 0; wi < 4; ++wi) {
-      const uint4 c = __ldg(cent + wi);  // 8 halves = 4 half2 = 4 bytes of residual
-      const uint32_t cw[4] = {c.x, c.y, c.z, c.w};
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const uint32_t byte = (w[wi] >> (8 * k)) & 0xffu;
-        e[wi * 4 + k] = __hadd2(u32_as_half2(lut[byte]), u32_as_half2(cw[k]));
-      }
-    }
-  }
-};
-
-template <>
-struct Decoder<2> {
-  static constexpr int EL_PER_BYTE = 4;
-  // lut: 256 x (half2, half2) stored as uint2
-  __device__ static void build(uint32_t* lut, const WPerm& wp, int tid, int nthreads) {
-    for (int v = tid; v < 256; v += nthreads) {
-      lut[2 * v] = uint32_t(wp.v[(v >> 6) & 3]) | (uint32_t(wp.v[(v >> 4) & 3]) << 16);
-      lut[2 * v + 1] = uint32_t(wp.v[(v >> 2) & 3]) | (uint32_t(wp.v[v & 3]) << 16);
-    }
-  }
-  // 16 bytes -> 32 half2
-  __device__ __forceinline__ static void decode16(const uint32_t* lut, const uint4& rv, const uint4* cent,
-                                                  __half2 (&e)[32]) {
-    const uint32_t w[4] = {rv.x, rv.y, rv.z, rv.w};
-#pragma unroll
-    for (int wi = 0; wi < 4; ++wi) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const uint32_t byte = (w[wi] >> (8 * k)) & 0xffu;
-        const uint2 c = __ldg(reinterpret_cast<const uint2*>(cent) + wi * 4 + k);  // 4 halves
-        const uint2 l = *reinterpret_cast<const uint2*>(lut + 2 * byte);
-        e[(wi * 4 + k) * 2] = __hadd2(u32_as_half2(l.x), u32_as_half2(c.x));
-        e[(wi * 4 + k) * 2 + 1] = __hadd2(u32_as_half2(l.y), u32_as_half2(c.y));
-      }
-    }
-  }
-};
-
-// fp16( fp32(e) / fp32(n) ) with IEEE fp32 division: q = e*r, one Newton correction with the
-// exact remainder (Markstein); r = RN(1/n).
-__device__ __forceinline__ float div_rn(float e, float n, float r) {
-  const float q = __fmul_rn(e, r);
-  const float rem = __fmaf_rn(-q, n, e);
-  return __fmaf_rn(rem, r, q);
-}
 
 // Decompress + normalise one token slice (the lane's 16 residual bytes) into `dst`
 // (shared or global), returning nothing.  LPT lanes cooperate on one token.

@@ -1,0 +1,445 @@
+// K7 : exhaustive exact MaxSim -- every local document against every query of a batch (fpb_exhaustive_scores).
+//
+//   scores[b, d] = RN_fp32( sum_{q<Q} fp16( max_t e_hat[d, t] . q[b, q] ) )
+//
+// K5's formula and rounding points up to the last one: the fp16 maxima are the same, their sum is exact and rounded
+// once to fp32 where K5 keeps an fp32 running sum (see the last point below).
+//
+// The approximate pipeline exact-scores n_full_scores/4 documents per query; here every document meets every
+// query, a GEMM-shaped problem of 2 * dim * E * B * Q FLOP, and the cost to avoid is decoding a token more than
+// once.  Each CTA takes chunks of consecutive documents, decodes 256 of their tokens at a time into a resident
+// shared-memory tile (the B operand) and streams every query row of the batch past it (the A operand):
+//
+//   * query rows: query b owns rows [b*Qs, b*Qs + Q) of a dense row array (Qs = Q rounded up to 16, so the 16
+//     rows of an MMA warp belong to one query); rows q >= Q are zero and are left out of the sum;
+//   * 256 threads = two warpgroups.  Both decode the tile with the shared decoder (decode.cuh) in v5's 8-token
+//     passes: pass p of a document is its tokens 8p..8p+7, a partial pass repeats the last token (a duplicate
+//     cannot change a maximum), passes of consecutive documents follow each other, and a document is split only
+//     where it crosses a tile boundary.  Then the 128-row A stages are cp.async-loaded one stage ahead, and
+//     warpgroup c multiplies its 64 rows against the tile with wgmma.m64n128k16 (two 128-token blocks issued
+//     back to back; the epilogue starts once both have completed);
+//   * the per-document maxima come straight out of the accumulator registers (column group j = one pass, as in
+//     v5).  A document whose passes cross a tile boundary keeps its running row maxima in a per-CTA carry array
+//     (global memory, L2-resident) until its last tile;
+//   * the sum over q: every fp16 maximum is an integer multiple of 2^-24 below 2^16 in magnitude, so the fp32
+//     sum is computed as the exact 64-bit integer sum of m * 2^24 (a warp adds its 16 rows, then one integer
+//     atomicAdd per warp and document) and rounded once to fp32 by k7_finalize.  Integer addition is
+//     associative: the result does not depend on the order of the atomics, on the grid or on how a batch is
+//     split into calls.  Where the fp32 running sum of K5 / the reference is exact (every partial sum fits 24
+//     significant bits, the usual case) the two are bit-identical; elsewhere they can differ in the last bit.
+#include <stdlib.h>
+#include <string.h>
+
+#include "decode.cuh"
+#include "kernels.h"
+#include "wgmma.cuh"
+
+namespace {
+
+constexpr int K7_THREADS = 256;          // two warpgroups: both decode, both run MMAs
+constexpr int K7_TILE = 256;             // decoded token rows resident per tile
+constexpr int K7_PASSES = K7_TILE / 8;   // 32 passes of 8 tokens
+constexpr int K7_RB = 128;               // query rows per A stage (64 per warpgroup)
+constexpr int K7_MAX_DOCS = 32;          // documents per chunk (one warp scans their pass counts)
+static_assert(K7_TILE == 2 * 128, "the MMA loop keeps two 128-column accumulator blocks");
+
+template <int D>
+struct K7Smem {
+  static constexpr int b_kblock = K7_TILE * 128;  // B: tile rows x 128 B per 64-element K block
+  static constexpr int a_kblock = K7_RB * 128;
+  static constexpr int a_stage = (D / 64) * a_kblock;
+  static constexpr int b_off = 0;
+  static constexpr int a_off = b_off + (D / 64) * b_kblock;
+  static constexpr int lut_off = a_off + 2 * a_stage;
+  static constexpr int do0_off = lut_off + 512 * 4;           // int64 first token row of every chunk document
+  static constexpr int trow_off = do0_off + K7_MAX_DOCS * 8;  // int64 first token row of every tile pass
+  static constexpr int dlen_off = trow_off + K7_PASSES * 8;   // int tokens of every chunk document
+  static constexpr int dnp_off = dlen_off + K7_MAX_DOCS * 4;  // int passes of every chunk document
+  static constexpr int dpfx_off = dnp_off + K7_MAX_DOCS * 4;  // int passes of the chunk before the document
+  static constexpr int tnv_off = dpfx_off + K7_MAX_DOCS * 4;  // int valid tokens of every tile pass
+  static constexpr int tdoc_off = tnv_off + K7_PASSES * 4;    // int document (chunk slot) of every tile pass
+  static constexpr int tseg_off = tdoc_off + K7_PASSES * 4;    // int first tile pass of every segment (+ end)
+  static constexpr int tsegd_off = tseg_off + (K7_PASSES + 4) * 4;  // int document of every segment
+  static constexpr int misc_off = tsegd_off + K7_PASSES * 4;
+  static constexpr int bytes = misc_off + 64 + 1024;          // + slack for the 1024-byte alignment
+};
+static_assert(K7Smem<128>::bytes <= 227 * 1024, "K7 shared memory");
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// fp16(m) * 2^24 as an integer: exact for every fp16 value (the smallest subnormal is 2^-24, |m| <= 65504)
+__device__ __forceinline__ long long k7_fixed(float m) {
+  return __float2ll_rn(__half2float(__float2half_rn(m)) * 16777216.0f);
+}
+
+// The work of a launch.  K7_ALL is the product; the other two are timing variants that time one part of the loop
+// alone (tools/bench_exhaustive.py, FPB_K7=mma|decode).  Their scores are meaningless.
+enum K7Part { K7_ALL = 0, K7_MMA_ONLY = 1, K7_DECODE_ONLY = 2 };
+
+template <int D, int NBITS, int PART>
+__global__ void __launch_bounds__(K7_THREADS, 1)
+k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ doc_offsets,
+                     const int32_t* __restrict__ codes, const uint8_t* __restrict__ residuals,
+                     const __half* __restrict__ norms, WPerm wp, const __half* __restrict__ rows, int B, int Q,
+                     int Qs, int n_rows, int64_t N, int docs_per_chunk, unsigned long long* __restrict__ acc,
+                     float* __restrict__ carry_all, int* __restrict__ counter) {
+  using S = K7Smem<D>;
+  constexpr int PD = D * NBITS / 8;
+  constexpr int LPT = PD / 16;           // lanes per token, 16 packed bytes each
+  constexpr int EPL = D / LPT;           // elements per lane
+  constexpr int NH2 = EPL / 2;
+  constexpr int TPR = K7_THREADS / LPT;  // tokens per decode round
+  constexpr int ROUNDS = K7_TILE / TPR;
+  constexpr int KS = D / 16;             // MMA k steps
+  constexpr int CPR = D / 8;             // 16-byte chunks per row
+  extern __shared__ unsigned char smem_dyn[];
+  const uint32_t dyn_addr = smem_u32(smem_dyn);
+  unsigned char* base = smem_dyn + ((1024u - (dyn_addr & 1023u)) & 1023u);  // SWIZZLE_128B atoms are 1024 B
+  unsigned char* smB = base + S::b_off;
+  unsigned char* smA = base + S::a_off;
+  uint32_t* lut = reinterpret_cast<uint32_t*>(base + S::lut_off);
+  int64_t* doc_o0 = reinterpret_cast<int64_t*>(base + S::do0_off);
+  int64_t* t_row = reinterpret_cast<int64_t*>(base + S::trow_off);
+  int* doc_len = reinterpret_cast<int*>(base + S::dlen_off);
+  int* doc_np = reinterpret_cast<int*>(base + S::dnp_off);
+  int* doc_pfx = reinterpret_cast<int*>(base + S::dpfx_off);
+  int* t_nv = reinterpret_cast<int*>(base + S::tnv_off);
+  int* t_doc = reinterpret_cast<int*>(base + S::tdoc_off);
+  int* t_seg = reinterpret_cast<int*>(base + S::tseg_off);
+  int* t_segdoc = reinterpret_cast<int*>(base + S::tsegd_off);
+  int* misc = reinterpret_cast<int*>(base + S::misc_off);  // [0] chunk, [1] passes of the chunk, [2] tile segments
+
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int c = warp >> 2, w = warp & 3, quad = lane & 3;
+  float* carry = carry_all + int64_t(blockIdx.x) * n_rows;
+  Decoder<NBITS>::build(lut, wp, tid, K7_THREADS);
+  const int64_t n_chunks = (N + docs_per_chunk - 1) / docs_per_chunk;
+  const int n_rb = n_rows / K7_RB;
+
+  // A stage: 128 query rows, K-major SWIZZLE_128B, one cp.async group per stage
+  auto load_a = [&](int rb, int stage) {
+    const __half* src = rows + int64_t(rb) * K7_RB * D;
+    unsigned char* dst = smA + stage * S::a_stage;
+    for (int i = tid; i < K7_RB * CPR; i += K7_THREADS) {
+      const int r = i / CPR, cc = i % CPR;
+      cp_async16(smem_u32(dst + sw128_off(r, cc, S::a_kblock)), src + int64_t(r) * D + cc * 8);
+    }
+    cp_async_commit();
+  };
+
+  for (;;) {
+    __syncthreads();  // every role is done with the previous chunk's tables
+    if (tid == 0) misc[0] = atomicAdd(counter, 1);
+    __syncthreads();
+    const int64_t chunk = misc[0];
+    if (chunk >= n_chunks) break;
+    const int64_t d0 = chunk * docs_per_chunk;
+    const int nd = int(min(int64_t(docs_per_chunk), N - d0));
+
+    // ---- chunk metadata (warp 0): documents and their pass prefix ----
+    if (warp == 0) {
+      int np = 0, len = 0;
+      int64_t o0 = 0;
+      if (lane < nd) {
+        o0 = doc_offsets[d0 + lane];
+        len = int(doc_offsets[d0 + lane + 1] - o0);
+        np = (len + 7) >> 3;
+      }
+      int incl = np;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, off);
+        if (lane >= off) incl += t;
+      }
+      if (lane < nd) {
+        doc_o0[lane] = o0;
+        doc_len[lane] = len;
+        doc_np[lane] = np;
+        doc_pfx[lane] = incl - np;
+      }
+      if (lane == 31) misc[1] = incl;
+    }
+    __syncthreads();
+    const int n_pass = misc[1];
+
+    for (int p0 = 0; p0 < n_pass; p0 += K7_PASSES) {
+      const int tp = min(K7_PASSES, n_pass - p0);
+      // ---- tile table: pass -> (first row, valid tokens, document) ----
+      if (tid < tp) {
+        const int g = p0 + tid;
+        int i = 0;
+        while (doc_pfx[i] + doc_np[i] <= g) ++i;  // documents without tokens own no pass and are skipped
+        const int k = g - doc_pfx[i];
+        t_row[tid] = doc_o0[i] + 8 * k;
+        t_nv[tid] = min(8, doc_len[i] - 8 * k);
+        t_doc[tid] = i;
+      }
+      if (warp == 0) {  // segments: maximal runs of tile passes of one document (the table above is warp 0's)
+        __syncwarp();
+        const bool start = lane < tp && (lane == 0 || t_doc[lane] != t_doc[lane - 1]);
+        const unsigned starts = __ballot_sync(0xffffffffu, start);
+        if (start) {
+          const int sg = __popc(starts & ((1u << lane) - 1u));
+          t_seg[sg] = lane;
+          t_segdoc[sg] = t_doc[lane];
+        }
+        if (lane == 0) {
+          misc[2] = __popc(starts);
+          t_seg[__popc(starts)] = tp;
+        }
+      }
+      load_a(0, 0);  // in flight during the decode
+      __syncthreads();
+
+      // ---- decode the tile once: row r = tile pass r/8, token r%8 ----
+      {
+        const int sub = tid % LPT;
+        const int nrow = tp * 8;
+        int64_t tok[ROUNDS];
+        int code[ROUNDS];
+        uint4 rv[ROUNDS];
+#pragma unroll
+        for (int u = 0; u < ROUNDS; ++u) {  // every load of the tile in flight before the first decode
+          const int r = u * TPR + tid / LPT;
+          tok[u] = 0;
+          code[u] = 0;
+          rv[u] = make_uint4(0u, 0u, 0u, 0u);
+          if (r < nrow) {
+            const int p = r >> 3;
+            tok[u] = t_row[p] + min(r & 7, t_nv[p] - 1);
+            code[u] = __ldg(codes + tok[u]);
+            rv[u] = ldg_nc_na(reinterpret_cast<const uint4*>(residuals + tok[u] * PD) + sub);
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < ROUNDS; ++u) {
+          const int r = u * TPR + tid / LPT;
+          if (r < nrow) {
+            __half2 e[NH2];
+            Decoder<NBITS>::decode16(lut, rv[u], reinterpret_cast<const uint4*>(C + int64_t(code[u]) * D + sub * EPL), e);
+            const float nf = __half2float(norms[tok[u]]);
+            const float rc = __frcp_rn(nf);
+#pragma unroll
+            for (int i = 0; i < EPL / 8; ++i) {
+              uint32_t o[4];
+#pragma unroll
+              for (int h = 0; h < 4; ++h) {
+                const float2 f = __half22float2(e[4 * i + h]);
+                o[h] = pack_half2_rn(div_rn(f.x, nf, rc), div_rn(f.y, nf, rc));
+              }
+              *reinterpret_cast<uint4*>(smB + sw128_off(r, sub * (EPL / 8) + i, S::b_kblock)) =
+                  make_uint4(o[0], o[1], o[2], o[3]);
+            }
+          }
+        }
+      }
+
+      // ---- stream every query row past the tile ----
+      const bool two_blocks = tp > 16;
+      for (int rb = 0; rb < (PART == K7_DECODE_ONLY ? 0 : n_rb); ++rb) {
+        if (rb + 1 < n_rb) {
+          load_a(rb + 1, (rb + 1) & 1);
+          cp_async_wait<1>();
+        } else {
+          cp_async_wait<0>();
+        }
+        fence_proxy_async();  // this thread's cp.async rows and decoded rows -> visible to wgmma
+        __syncthreads();
+
+        const uint32_t a_addr = smem_u32(smA + (rb & 1) * S::a_stage) + c * 8 * 1024;  // warpgroup c: rows 64c..
+        const uint32_t b_addr = smem_u32(smB);
+        float acc0[64], acc1[64];
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+          const uint32_t ka = (ks >> 2) * S::a_kblock + (ks & 3) * 32;
+          const uint32_t kb = (ks >> 2) * S::b_kblock + (ks & 3) * 32;
+          wgmma_m64n128k16(acc0, gmma_desc(a_addr + ka), gmma_desc(b_addr + kb), ks > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        if (two_blocks) {
+#pragma unroll
+          for (int ks = 0; ks < KS; ++ks) {
+            const uint32_t ka = (ks >> 2) * S::a_kblock + (ks & 3) * 32;
+            const uint32_t kb = (ks >> 2) * S::b_kblock + (ks & 3) * 32;
+            wgmma_m64n128k16(acc1, gmma_desc(a_addr + ka), gmma_desc(b_addr + 16 * 1024 + kb), ks > 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+        }
+
+        // thread (w, lane) holds rows wrow + lane/4 (+8) of the warp's 16 rows, all of query b
+        const int wrow = rb * K7_RB + c * 64 + 16 * w;
+        const int r0 = wrow + (lane >> 2);
+        const int b = wrow / Qs, q0 = wrow % Qs + (lane >> 2);
+        const bool live = b < B && wrow % Qs < Q;  // warp-uniform: some row of this warp is a real query token
+        int di = 0;
+        float m0 = -INFINITY, m1 = -INFINITY;
+        auto flush = [&]() {
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+          m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
+          m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+          if (!live) return;
+          const int pfx = doc_pfx[di], np = doc_np[di];
+          if (pfx < p0 && quad == 0) {  // the document began in an earlier tile
+            m0 = fmaxf(m0, __ldcg(carry + r0));
+            m1 = fmaxf(m1, __ldcg(carry + r0 + 8));
+          }
+          if (pfx + np > p0 + K7_PASSES) {  // ... or goes on in the next one: keep the running maxima
+            if (quad == 0) {
+              __stcg(carry + r0, m0);
+              __stcg(carry + r0 + 8, m1);
+            }
+            return;
+          }
+          long long v = 0;
+          if (quad == 0) v = (q0 < Q ? k7_fixed(m0) : 0ll) + (q0 + 8 < Q ? k7_fixed(m1) : 0ll);
+          v += __shfl_xor_sync(0xffffffffu, v, 4);
+          v += __shfl_xor_sync(0xffffffffu, v, 8);
+          v += __shfl_xor_sync(0xffffffffu, v, 16);
+          if (lane == 0) atomicAdd(acc + int64_t(b) * N + d0 + di, static_cast<unsigned long long>(v));
+        };
+        // both blocks complete before the epilogue: reading acc0 while acc1 is in flight makes ptxas serialise
+        // every wgmma of the kernel (C7514)
+        wgmma_wait0();
+        if (PART != K7_MMA_ONLY) {
+          // per-pass maxima of rows r0, r0 + 8 (accumulator column group j = pass j of the block), then one masked
+          // maximum and one flush per segment: the same code whatever the documents, no branch per pass
+          float pm0[K7_PASSES], pm1[K7_PASSES];
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            pm0[j] = fmaxf(acc0[4 * j], acc0[4 * j + 1]);
+            pm1[j] = fmaxf(acc0[4 * j + 2], acc0[4 * j + 3]);
+          }
+          if (two_blocks) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              pm0[16 + j] = fmaxf(acc1[4 * j], acc1[4 * j + 1]);
+              pm1[16 + j] = fmaxf(acc1[4 * j + 2], acc1[4 * j + 3]);
+            }
+          } else {
+#pragma unroll
+            for (int j = 16; j < K7_PASSES; ++j) pm0[j] = pm1[j] = -INFINITY;
+          }
+          const int n_seg = misc[2];
+          for (int sg = 0; sg < n_seg; ++sg) {
+            const int j0 = t_seg[sg], j1 = t_seg[sg + 1];
+            di = t_segdoc[sg];
+            m0 = m1 = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < K7_PASSES; ++j) {
+              const bool in = j >= j0 && j < j1;
+              m0 = fmaxf(m0, in ? pm0[j] : -INFINITY);
+              m1 = fmaxf(m1, in ? pm1[j] : -INFINITY);
+            }
+            flush();
+          }
+        } else {
+          // timing variant: keep every accumulator live so that no MMA is dropped as dead code
+          float x = -INFINITY;
+#pragma unroll
+          for (int j = 0; j < 64; ++j) x = fmaxf(x, two_blocks ? fmaxf(acc0[j], acc1[j]) : acc0[j]);
+          if (x == 1234.5f) misc[3] = 1;
+        }
+        __syncthreads();  // both warpgroups are done with this A stage (and, after the last one, with the tile)
+      }
+    }
+  }
+}
+
+// query b, token q -> row b*Qs + q of the dense row array; every other row is zero
+__global__ void k7_pack_rows_kernel(const __half* __restrict__ q, int B, int Q, int Qs, int D, int64_t n_chunks16,
+                                    __half* __restrict__ rows) {
+  const int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
+  if (i >= n_chunks16) return;
+  const int cpr = D / 8;
+  const int64_t r = i / cpr;
+  const int cc = int(i % cpr);
+  const int64_t b = r / Qs;
+  const int qq = int(r % Qs);
+  uint4 v = make_uint4(0u, 0u, 0u, 0u);
+  if (b < B && qq < Q) v = *reinterpret_cast<const uint4*>(q + (b * Q + qq) * D + cc * 8);
+  reinterpret_cast<uint4*>(rows)[i] = v;
+}
+
+// exact fixed-point sums -> fp32 scores; a document without tokens scores Q times the padding sentinel
+__global__ void k7_finalize_kernel(const unsigned long long* __restrict__ acc, const int64_t* __restrict__ doc_offsets,
+                                   int64_t N, int64_t total, int Q, float* __restrict__ scores) {
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
+    const int64_t d = i % N;
+    const bool empty = doc_offsets[d + 1] == doc_offsets[d];
+    scores[i] = empty ? float(Q) * FPB_PAD_SENTINEL
+                      : __ll2float_rn(static_cast<long long>(acc[i])) * (1.0f / 16777216.0f);
+  }
+}
+
+template <int D, int NBITS, int PART>
+int launch_k7_t(const fpb_index* ix, const ExLayout& X, char* ws, cudaStream_t st) {
+  auto kern = k7_exhaustive_kernel<D, NBITS, PART>;
+  constexpr int smem = K7Smem<D>::bytes;
+  // opt in on every launch: the attribute is per device and the call costs about a microsecond
+  FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  WPerm wp;
+  for (int i = 0; i < 16; ++i) wp.v[i] = ix->w_perm_bits[i];
+  // documents per chunk: as many as one warp scans, fewer (down to 4, as in v5) when that leaves too few chunks to
+  // balance the SMs.  FPB_K7_DOCS_PER_CHUNK=n (1..32) pins it: the result does not depend on it, and the tests use
+  // it to run the multi-document chunk walk on small indexes.
+  int dpc = K7_MAX_DOCS;
+  while (dpc > 4 && (ix->N + dpc - 1) / dpc < int64_t(ix->sm_count) * 8) dpc >>= 1;
+  if (const char* pin = getenv("FPB_K7_DOCS_PER_CHUNK")) {
+    const int v = atoi(pin);
+    if (v >= 1 && v <= K7_MAX_DOCS) dpc = v;
+  }
+  const int64_t chunks = (ix->N + dpc - 1) / dpc;
+  const int blocks = int(chunks < X.grid ? chunks : X.grid);
+  kern<<<blocks, K7_THREADS, smem, st>>>(ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals,
+                                         ix->token_norms, wp, reinterpret_cast<const __half*>(ws + X.off_rows), X.B,
+                                         X.Q, X.Qs, X.n_rows, ix->N, dpc,
+                                         reinterpret_cast<unsigned long long*>(ws + X.off_acc),
+                                         reinterpret_cast<float*>(ws + X.off_carry),
+                                         reinterpret_cast<int*>(ws + X.off_counter));
+  FPB_LAUNCH_CHECK("k7_exhaustive");
+  return FPB_OK;
+}
+
+}  // namespace
+
+int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
+                             float* d_scores, cudaStream_t st) {
+  if (ix->N == 0) return FPB_OK;
+  const int64_t n16 = int64_t(X.n_rows) * (ix->dim / 8);
+  k7_pack_rows_kernel<<<int((n16 + 255) / 256), 256, 0, st>>>(d_queries, X.B, X.Q, X.Qs, ix->dim, n16,
+                                                               reinterpret_cast<__half*>(ws + X.off_rows));
+  FPB_LAUNCH_CHECK("k7_pack_rows");
+  FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_acc, 0, size_t(X.B) * ix->N * 8, st));
+  FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_counter, 0, sizeof(int), st));
+  // FPB_K7=mma | decode: timing variants of dim 128 / nbits 4 (their scores are meaningless)
+  const char* part = getenv("FPB_K7");
+  const bool mma_only = part && strcmp(part, "mma") == 0, decode_only = part && strcmp(part, "decode") == 0;
+  int rc;
+  if (ix->dim == 128 && ix->nbits == 4 && mma_only) rc = launch_k7_t<128, 4, K7_MMA_ONLY>(ix, X, ws, st);
+  else if (ix->dim == 128 && ix->nbits == 4 && decode_only) rc = launch_k7_t<128, 4, K7_DECODE_ONLY>(ix, X, ws, st);
+  else if (ix->dim == 128 && ix->nbits == 4) rc = launch_k7_t<128, 4, K7_ALL>(ix, X, ws, st);
+  else if (ix->dim == 128 && ix->nbits == 2) rc = launch_k7_t<128, 2, K7_ALL>(ix, X, ws, st);
+  else if (ix->dim == 64 && ix->nbits == 4) rc = launch_k7_t<64, 4, K7_ALL>(ix, X, ws, st);
+  else if (ix->dim == 64 && ix->nbits == 2) rc = launch_k7_t<64, 2, K7_ALL>(ix, X, ws, st);
+  else {
+    fpb_set_error("exhaustive search: unsupported (dim=%d, nbits=%d)", ix->dim, ix->nbits);
+    return FPB_ERR_UNSUPPORTED;
+  }
+  if (rc != FPB_OK) return rc;
+  const int64_t total = int64_t(X.B) * ix->N;
+  const int64_t want = (total + 255) / 256;
+  const int blocks = int(want < int64_t(ix->sm_count) * 16 ? want : int64_t(ix->sm_count) * 16);
+  k7_finalize_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const unsigned long long*>(ws + X.off_acc),
+                                             ix->doc_offsets, ix->N, total, X.Q, d_scores);
+  FPB_LAUNCH_CHECK("k7_finalize");
+  return FPB_OK;
+}

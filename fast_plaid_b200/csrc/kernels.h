@@ -59,3 +59,17 @@ int launch_apply_threshold(const Ws& ws, const uint64_t* d_all_keys, int n_shard
 int launch_merge(const fpb_record* d_all_records, int n_shards, int b_stride, int n_queries, int R, int top_k,
                  int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t stream);
 int launch_emit_records(const fpb_index* ix, const Ws& ws, fpb_record* d_records, cudaStream_t st);
+
+// Workspace of the exhaustive search (exhaustive.cu).  The selection part (top_k > 0) is laid out so that an
+// fpb_layout can point k3b_select and k6_rank at it: the score array plays off_approx, an iota plays off_cand.
+struct ExLayout {
+  int B, Q, Qs, n_rows, top_k, grid;  // Qs = Q rounded up to 16; n_rows = B*Qs rounded up to 128; grid = K7 CTAs
+  int64_t off_rows;     // f16 [n_rows, dim] dense query rows
+  int64_t off_acc;      // u64 [B, N] fixed-point score sums
+  int64_t off_carry;    // f32 [grid, n_rows] running maxima of documents that cross a tile boundary
+  int64_t off_counter;  // i32 chunk counter
+  int64_t off_scores, off_cand, off_n_cand, off_n_rerank, off_rerank, off_rerank_approx;  // selection (top_k > 0)
+  int64_t total_bytes;
+};
+int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
+                             float* d_scores, cudaStream_t st);  // K7 + finalize

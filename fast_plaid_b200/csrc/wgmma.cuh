@@ -1,5 +1,5 @@
 // Hopper (sm_90a) warpgroup-MMA and mbarrier PTX wrappers shared by the tensor-core kernels
-// (k1_centroid_v2.cu, encode.cu, k5_maxsim_v5.cu).  Operand tiles live in shared memory in the
+// (k1_centroid_v2.cu, encode.cu, k5_maxsim_v5.cu, k7_exhaustive.cu).  Operand tiles live in shared memory in the
 // K-major SWIZZLE_128B layout: a K block of 64 halves is 128 bytes per row, rows come in 8-row
 // atoms of 1024 bytes, and 16-byte chunk c of row r is stored at chunk (c ^ (r % 8)).
 #pragma once
@@ -58,6 +58,7 @@ __device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 // D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, f16 inputs, f32 accumulators, both operands K-major in shared memory.
 // Accumulator fragment of thread t of the warpgroup (warp w = t / 32, lane l = t % 32): d[4j + e] holds row

@@ -128,6 +128,9 @@ EXPORTED_SYMBOLS = [
     "fpb_sharded_scratch_bytes",
     "fpb_search_batch_sharded",
     "fpb_search_batch_sharded_host",
+    "fpb_exhaustive_workspace_bytes",
+    "fpb_exhaustive_scores",
+    "fpb_search_exhaustive",
     "fpb_reconstruct",
     "fpb_token_scores",
     "fpb_encode",
@@ -233,6 +236,12 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_kmeans_update.argtypes = [i32, i32, i64, vp, vp, vp, vp, vp, vp]
         lib.fpb_token_scores.restype = i32
         lib.fpb_token_scores.argtypes = [vp, vp, i32, vp, vp, i32, i64, vp, vp]
+        lib.fpb_exhaustive_workspace_bytes.restype = i32
+        lib.fpb_exhaustive_workspace_bytes.argtypes = [vp, i32, i32, i32, ctypes.POINTER(sz)]
+        lib.fpb_exhaustive_scores.restype = i32
+        lib.fpb_exhaustive_scores.argtypes = [vp, vp, i32, i32, vp, sz, vp, vp]
+        lib.fpb_search_exhaustive.restype = i32
+        lib.fpb_search_exhaustive.argtypes = [vp, vp, i32, i32, i32, vp, sz, vp, vp, vp, vp]
         _lib = lib
         return lib
 
@@ -706,6 +715,88 @@ class DeviceIndex:
                         )
                     )
                     self._keepalive = (sid, soff)  # until the stream has consumed them
+        return ids, scores, counts
+
+    # -- exhaustive exact search ---------------------------------------------------------------
+    def exhaustive_workspace_bytes(self, B: int, Q: int, top_k: int) -> int:
+        """Workspace of fpb_search_exhaustive (top_k >= 1) or of fpb_exhaustive_scores alone (top_k = 0)."""
+        out = ctypes.c_size_t()
+        _check(self._lib.fpb_exhaustive_workspace_bytes(self._handle, B, Q, top_k, ctypes.byref(out)))
+        return int(out.value)
+
+    def _exhaustive_buffer(self, nbytes: int) -> torch.Tensor:
+        """The grow-only workspace `search` uses (both run under _exclusive)."""
+        with self._lock:
+            if self._buf is None or self._buf.numel() < nbytes:
+                self._buf = None
+                self._buf = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            return self._buf
+
+    def _check_queries(self, queries: torch.Tensor) -> torch.Tensor:
+        if queries.dim() != 3:
+            raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
+        if queries.dtype != torch.float16 or queries.device != self.device:
+            raise ValueError("DeviceIndex expects fp16 queries on the index device")
+        if queries.shape[2] != self.dim:
+            raise ValueError(f"query dim {queries.shape[2]} != index dim {self.dim}")
+        return queries.contiguous()
+
+    def _exhaustive_step(self, B: int, Q: int, top_k: int, budget_bytes: int) -> int:
+        """Most queries per call whose workspace fits the budget (at least one).  The size grows with B but not
+        linearly (query rows are padded to blocks of 128), so the largest fitting call is found by bisection."""
+        if self.exhaustive_workspace_bytes(B, Q, top_k) <= budget_bytes:
+            return B
+        lo, hi = 1, B  # ws(lo) may exceed the budget: one query per call is the floor
+        while lo < hi:
+            mid = (lo + hi + 1) // 2
+            if self.exhaustive_workspace_bytes(mid, Q, top_k) <= budget_bytes:
+                lo = mid
+            else:
+                hi = mid - 1
+        return lo
+
+    def exhaustive_scores(self, queries: torch.Tensor) -> torch.Tensor:
+        """Exact MaxSim score of every local document for every query: f32 [B, num_documents]
+        (one fpb_exhaustive_scores call).  Asynchronous."""
+        queries = self._check_queries(queries)
+        B, Q, _ = queries.shape
+        scores = torch.empty((B, self.num_documents), dtype=torch.float32, device=self.device)
+        if B == 0:
+            return scores
+        with self._exclusive(), torch.cuda.device(self.device):
+            buf = self._exhaustive_buffer(self.exhaustive_workspace_bytes(B, Q, 0))
+            _check(
+                self._lib.fpb_exhaustive_scores(
+                    self._handle, queries.data_ptr(), B, Q, buf.data_ptr(), buf.numel(), scores.data_ptr(),
+                    self._stream(),
+                )
+            )
+        return scores
+
+    def search_exhaustive(self, queries: torch.Tensor, top_k: int, budget_bytes: int = 6 << 30
+                          ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Exact top_k over every document: (ids int64 [B, top_k] global, scores f32 [B, top_k], counts int32 [B]),
+        the result contract of `search`.  The batch is split into calls whose workspace fits `budget_bytes`;
+        the result does not depend on the split.  Asynchronous."""
+        queries = self._check_queries(queries)
+        B, Q, _ = queries.shape
+        k = int(top_k)
+        ids = torch.empty((B, k), dtype=torch.int64, device=self.device)
+        scores = torch.empty((B, k), dtype=torch.float32, device=self.device)
+        counts = torch.empty((B,), dtype=torch.int32, device=self.device)
+        if B == 0:
+            return ids, scores, counts
+        step = self._exhaustive_step(B, Q, k, budget_bytes)
+        with self._exclusive(), torch.cuda.device(self.device):
+            for s in range(0, B, step):
+                e = min(B, s + step)
+                buf = self._exhaustive_buffer(self.exhaustive_workspace_bytes(e - s, Q, k))
+                _check(
+                    self._lib.fpb_search_exhaustive(
+                        self._handle, queries[s:e].data_ptr(), e - s, Q, k, buf.data_ptr(), buf.numel(),
+                        ids[s:e].data_ptr(), scores[s:e].data_ptr(), counts[s:e].data_ptr(), self._stream(),
+                    )
+                )
         return ids, scores, counts
 
     def _host_io(self, B: int, Q: int, k: int) -> dict[str, torch.Tensor]:

@@ -588,6 +588,54 @@ class FastPlaid:
             out.extend(f.result())
         return out
 
+    def _search_exhaustive_device(self, idx: DeviceIndex, queries: torch.Tensor,
+                                  top_k: int) -> list[list[tuple[int, float]]]:
+        if queries.dim() != 3:
+            raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
+        q16 = queries.to(device=idx.device, dtype=torch.float16)  # the fp16 cast of `search` (fast_plaid.py:241)
+        ids, scores, counts = idx.search_exhaustive(q16, top_k)
+        return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
+
+    @torch.inference_mode()
+    def search_exhaustive(
+        self,
+        queries_embeddings: torch.Tensor | list[torch.Tensor],
+        top_k: int = 10,
+    ) -> list[list[tuple[int, float]]]:
+        """Exact search: score EVERY document with the exact MaxSim formula of the re-rank stage and return,
+        per query, the ``top_k`` best ``(doc_id, score)`` pairs in rank order (score desc, then id asc).
+
+        No centroid probing and no pruning, so there is no recall loss and no knob to tune; the cost grows
+        with the number of documents (see README for measured times).  Works on ``compress_only`` indexes.
+        Queries take the forms ``search`` accepts.  ``top_k`` <= 4096.
+
+        A score sums the per-query-token fp16 maxima exactly and rounds once to fp32; ``search`` keeps an fp32
+        running sum.  The two agree whenever that running sum is exact (the usual case); otherwise the same
+        document's score can differ in the last bit between ``search`` and ``search_exhaustive``.  In exchange the
+        result is the same bytes however the work is ordered or the batch is split."""
+        if self.shard is not None:
+            raise NotImplementedError(
+                "search_exhaustive on a document-sharded index is not implemented: each rank holds only its "
+                "document range, and the per-shard top-k lists would need a merge across ranks"
+            )
+        search_indices, queries, _ = self._prepare_search(queries_embeddings, None)
+        if len(self.devices) == 1:
+            return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k)
+        # several devices in ONE process hold replicas: the query list is split across them, like `search`
+        n = len(self.devices)
+        chunk = math.ceil(queries.shape[0] / n)
+        chunks = list(torch.split(queries, chunk))
+        with ThreadPoolExecutor(max_workers=n) as ex:
+            futs = [
+                ex.submit(self._search_exhaustive_device, search_indices[d], chunks[i], top_k)
+                for i, d in enumerate(self.devices)
+                if i < len(chunks)
+            ]
+        out: list[list[tuple[int, float]]] = []
+        for f in futs:
+            out.extend(f.result())
+        return out
+
     @torch.inference_mode()
     def search_token_scores(
         self,

@@ -288,6 +288,28 @@ int fpb_search_batch_sharded_host(const fpb_index* index, fpb_comm* comm, int n_
                                   float* d_out_scores, int32_t* d_out_counts, int64_t* h_out_ids, float* h_out_scores,
                                   int32_t* h_out_counts, void* stream);
 
+/* ---- exhaustive exact search (new; the reference has no such mode) ----
+ * Scores EVERY local document against every query with the exact MaxSim formula of the re-rank stage
+ * (search.rs:626-656: same decoder, same fp16 rounding of each token score, an empty document scores
+ * Q * -10000), then ranks them.  No IVF is read, so a compress_only index can be searched this way.
+ * One rounding point differs: the sum over the Q query tokens is the EXACT sum of the fp16 maxima, rounded once
+ * to fp32, where the re-rank stage keeps an fp32 running sum.  The two agree whenever that running sum is exact
+ * (the usual case); otherwise a document's score from fpb_search_batch and from these calls can differ in the
+ * last bit.  The exact sum is what makes the result independent of the order of the work.
+ *   fpb_exhaustive_workspace_bytes : workspace of fpb_search_exhaustive for B queries of Q <= 256 tokens and
+ *                                    1 <= top_k <= 4096 (FPB_ERR_UNSUPPORTED above), or with top_k = 0 of
+ *                                    fpb_exhaustive_scores alone; 256-byte aligned
+ *   fpb_exhaustive_scores  d_queries f16 [B, Q, dim] (16-byte aligned), d_scores f32 [B, n_docs] (local ids)
+ *   fpb_search_exhaustive  outputs as fpb_search_batch: global ids in rank order (score desc, then id asc),
+ *                          d_out_counts[b] = min(top_k, n_docs), unused tail entries id -1 / score -inf
+ * Deterministic: the same inputs give the same bytes, whatever B and however a batch is split into calls. */
+int fpb_exhaustive_workspace_bytes(const fpb_index* index, int B, int Q, int top_k, size_t* out);
+int fpb_exhaustive_scores(const fpb_index* index, const void* d_queries, int B, int Q, void* d_workspace,
+                          size_t workspace_bytes, float* d_scores, void* stream);
+int fpb_search_exhaustive(const fpb_index* index, const void* d_queries, int B, int Q, int top_k, void* d_workspace,
+                          size_t workspace_bytes, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
+                          void* stream);
+
 /* ---- by-products of the MaxSim kernel ("next" rows of SURVEY.md 8f-3) ---- */
 /* reconstruct_embeddings (rust/utils/embeddings.rs:12-69): decompressed, normalised
  * fp16 rows of the given local docs, concatenated.  d_out: f16 [sum(len), dim]. */
