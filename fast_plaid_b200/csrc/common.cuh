@@ -7,6 +7,10 @@
 
 #include "../../include/fastplaid_b200.h"
 
+struct WPerm {
+  uint16_t v[16];
+};
+
 // Immutable index handle (replaces LoadedIndex, rust/search/load.rs:50-56).  Holds only
 // borrowed device pointers plus the small derived codec table.
 struct fpb_index {
@@ -33,15 +37,12 @@ struct fpb_index {
   const int32_t* ivf_pids;
   // w_perm[i] = bucket_weights[bitrev_nbits(i)]  (closed form of the two LUTs of
   // residual_codec.rs:83-140): element j of a byte is w_perm[(byte >> (8-nbits*(j+1))) & mask]
-  uint16_t w_perm_bits[16];
+  // (fp16 bit patterns, passed by value to every decoding kernel)
+  WPerm w_perm;
   // TMA descriptor of the centroid table: 2-D [K, dim] fp16, box 64 x 128, SWIZZLE_128B
   // (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint; has_tmap = 0 if unavailable)
   alignas(64) unsigned char tmap_centroids[128];
   int has_tmap;
-};
-
-struct WPerm {
-  uint16_t v[16];
 };
 
 void fpb_set_error(const char* fmt, ...);

@@ -118,8 +118,8 @@ extern "C" int fpb_index_create(fpb_index** out, int device, int nbits, int dim,
     fpb_set_error("copy of bucket_weights failed: %s", cudaGetErrorString(e));
     return FPB_ERR_CUDA;
   }
-  for (int i = 0; i < 16; ++i) ix->w_perm_bits[i] = 0;
-  for (int i = 0; i < (1 << nbits); ++i) ix->w_perm_bits[i] = w[bitrev(i, nbits)];
+  for (int i = 0; i < 16; ++i) ix->w_perm.v[i] = 0;
+  for (int i = 0; i < (1 << nbits); ++i) ix->w_perm.v[i] = w[bitrev(i, nbits)];
   int64_t n_tokens = 0;
   if (n_docs > 0) {
     e = cudaMemcpy(&n_tokens, d_doc_offsets + n_docs, sizeof(int64_t), cudaMemcpyDeviceToHost);

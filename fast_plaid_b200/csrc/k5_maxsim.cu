@@ -1,8 +1,6 @@
 // K5 : fused residual decompression + exact MaxSim           (search.rs:626-656, :53-107)
 //
-//   e      = fp16( w_perm[idx(byte, j)] + centroid[code][.] )        one fp16 add per element
-//   n      = fp16( sqrt( sum_fp32 e^2 ) )                             norm in fp32, stored fp16
-//   e_hat  = fp16( fp32(e) / fp32(n) )                                 IEEE division, one rounding
+//   e_hat  = the decoded, normalised token (decode.cuh: decompress_slice; n from the token_norm table)
 //   ts     = fp16( sum_fp32 e_hat[t] . q[j] )                          tensor-core MMA, fp32 acc
 //   score  = sum_{j<Q}^{fp32} max_{t<len} ts[t][j]
 //
@@ -28,49 +26,6 @@ struct K5Smem {
   static constexpr int LDS = D + 8;
   static constexpr int bytes = (K5_TILE * LDS + QP * LDS) * 2 + 4 * QP * 2 + 256 * 8;
 };
-
-// Decompress + normalise one token slice (the lane's 16 residual bytes) into `dst`
-// (shared or global), returning nothing.  LPT lanes cooperate on one token.
-// fp16 norm of the token whose slice `e` this lane holds: fp32 sum of squares (per lane in element order, then over
-// the LPT lanes of the token), square root, one rounding to fp16 (norm(...).half(), search.rs:86-93; the
-// clamp_min(1e-12) that follows is a no-op in fp16).  THE definition of the per-token norm table.
-template <int NH2, int LPT>
-__device__ __forceinline__ __half slice_norm(const __half2 (&e)[NH2]) {
-  float ss = 0.f;
-#pragma unroll
-  for (int p = 0; p < NH2; ++p) {
-    const float2 f = __half22float2(e[p]);
-    ss = __fmaf_rn(f.x, f.x, ss);
-    ss = __fmaf_rn(f.y, f.y, ss);
-  }
-#pragma unroll
-  for (int off = 1; off < LPT; off <<= 1) ss += __shfl_xor_sync(0xffffffffu, ss, off);
-  return __float2half_rn(sqrtf(ss));
-}
-
-template <int D, int NBITS, int LPT>
-__device__ __forceinline__ void decompress_slice(const uint32_t* lut, const uint8_t* __restrict__ residuals,
-                                                 const __half* __restrict__ C, const __half* __restrict__ norms,
-                                                 int64_t tok_global, int code, int sub, __half* dst_row) {
-  constexpr int PD = D * NBITS / 8;
-  constexpr int EPL = D / LPT;  // elements per lane
-  constexpr int NH2 = EPL / 2;
-  const uint4 rv = ldg_nc_na(reinterpret_cast<const uint4*>(residuals + tok_global * PD) + sub);
-  const uint4* cent = reinterpret_cast<const uint4*>(C + int64_t(code) * D + sub * EPL);
-  __half2 e[NH2];
-  Decoder<NBITS>::decode16(lut, rv, cent, e);
-  const float nf = __half2float(norms[tok_global]);  // derived once per token at index load (k5_token_norms_kernel)
-  const float r = __frcp_rn(nf);
-  uint32_t out[NH2];
-#pragma unroll
-  for (int p = 0; p < NH2; ++p) {
-    const float2 f = __half22float2(e[p]);
-    out[p] = pack_half2_rn(div_rn(f.x, nf, r), div_rn(f.y, nf, r));
-  }
-  uint4* d4 = reinterpret_cast<uint4*>(dst_row + sub * EPL);
-#pragma unroll
-  for (int i = 0; i < NH2 / 4; ++i) d4[i] = make_uint4(out[4 * i], out[4 * i + 1], out[4 * i + 2], out[4 * i + 3]);
-}
 
 template <int D, int NBITS, int QP>
 __global__ void __launch_bounds__(K5_THREADS)
@@ -258,15 +213,13 @@ k5_token_scores_kernel(const __half* __restrict__ C, const int64_t* __restrict__
   }
 }
 
-// The per-token norm table (fpb_index_create): one token per LPT lanes, same decode as everywhere else.
+// The per-token norm table (fpb_index_create): one token per LPT lanes.
 template <int D, int NBITS>
 __global__ void __launch_bounds__(K5_THREADS)
 k5_token_norms_kernel(const __half* __restrict__ C, const int32_t* __restrict__ codes,
                       const uint8_t* __restrict__ residuals, WPerm wp, int64_t n_tokens, __half* __restrict__ out) {
   constexpr int PD = D * NBITS / 8;
   constexpr int LPT = PD / 16;
-  constexpr int EPL = D / LPT;
-  constexpr int NH2 = EPL / 2;
   __shared__ uint32_t lut[512];
   Decoder<NBITS>::build(lut, wp, threadIdx.x, K5_THREADS);
   __syncthreads();
@@ -275,11 +228,7 @@ k5_token_norms_kernel(const __half* __restrict__ C, const int32_t* __restrict__ 
   const int64_t n_up = (n_tokens + per_cta - 1) / per_cta * per_cta;  // whole LPT groups stay convergent for the shuffles
   for (int64_t t = int64_t(blockIdx.x) * per_cta + threadIdx.x / LPT; t < n_up; t += int64_t(gridDim.x) * per_cta) {
     const int64_t tt = t < n_tokens ? t : n_tokens - 1;
-    const uint4 rv = ldg_nc_na(reinterpret_cast<const uint4*>(residuals + tt * PD) + sub);
-    const uint4* cent = reinterpret_cast<const uint4*>(C + int64_t(__ldg(codes + tt)) * D + sub * EPL);
-    __half2 e[NH2];
-    Decoder<NBITS>::decode16(lut, rv, cent, e);
-    const __half nrm = slice_norm<NH2, LPT>(e);
+    const __half nrm = token_norm<D, NBITS, LPT>(lut, residuals, C, tt, __ldg(codes + tt), sub);
     if (sub == 0 && t < n_tokens) out[t] = nrm;
   }
 }
@@ -291,12 +240,10 @@ int launch_k5_t(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   constexpr int smem = K5Smem<D, QP>::bytes;
   // opt in on every launch: the attribute is per device and the call costs about a microsecond
   FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  WPerm wp;
-  for (int i = 0; i < 16; ++i) wp.v[i] = ix->w_perm_bits[i];
   const int64_t items = int64_t(L.B) * L.R;
   const int blocks = int(items < int64_t(ix->sm_count) * 8 ? items : int64_t(ix->sm_count) * 8);
-  kern<<<blocks, K5_THREADS, smem, st>>>(ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals, ix->token_norms, wp,
-                                         ws.queries(), L.Q, L.B, L.R, ws.n_rerank(), ws.rerank(), ws.exact());
+  kern<<<blocks, K5_THREADS, smem, st>>>(ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals, ix->token_norms,
+                                         ix->w_perm, ws.queries(), L.Q, L.B, L.R, ws.n_rerank(), ws.rerank(), ws.exact());
   FPB_LAUNCH_CHECK("k5_maxsim");
   return FPB_OK;
 }
@@ -328,12 +275,10 @@ int launch_k5_q(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
 }  // namespace
 
 int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st) {
-  WPerm wp;
-  for (int i = 0; i < 16; ++i) wp.v[i] = ix->w_perm_bits[i];
   const int blocks = ix->sm_count * 8;
 #define CALL(DD, NB)                                                                                               \
-  k5_token_norms_kernel<DD, NB><<<blocks, K5_THREADS, 0, st>>>(ix->centroids, ix->doc_codes, ix->doc_residuals, wp, \
-                                                               ix->E, d_out);
+  k5_token_norms_kernel<DD, NB><<<blocks, K5_THREADS, 0, st>>>(ix->centroids, ix->doc_codes, ix->doc_residuals, \
+                                                               ix->w_perm, ix->E, d_out);
   FPB_DISPATCH_D_NBITS(ix, CALL)
 #undef CALL
   FPB_LAUNCH_CHECK("k5_token_norms");
@@ -369,12 +314,10 @@ extern "C" int fpb_reconstruct(const fpb_index* ix, const int32_t* d_doc_ids, in
   }
   if (n == 0) return FPB_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  WPerm wp;
-  for (int i = 0; i < 16; ++i) wp.v[i] = ix->w_perm_bits[i];
   const int blocks = min(n, ix->sm_count * 8);
 #define CALL(DD, NB)                                                                                        \
   k5_reconstruct_kernel<DD, NB><<<blocks, K5_THREADS, 0, st>>>(ix->centroids, ix->doc_offsets, ix->doc_codes, \
-                                                               ix->doc_residuals, ix->token_norms, wp, d_doc_ids, n,          \
+                                                               ix->doc_residuals, ix->token_norms, ix->w_perm, d_doc_ids, n, \
                                                                d_out_offsets, static_cast<__half*>(d_out));
   FPB_DISPATCH_D_NBITS(ix, CALL)
 #undef CALL
@@ -390,13 +333,11 @@ extern "C" int fpb_token_scores(const fpb_index* ix, const void* d_queries, int 
   }
   if (n == 0) return FPB_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  WPerm wp;
-  for (int i = 0; i < 16; ++i) wp.v[i] = ix->w_perm_bits[i];
   const int blocks = min(n, ix->sm_count * 8);
 #define CALL(DD, NB)                                                                                          \
   k5_token_scores_kernel<DD, NB><<<blocks, K5_THREADS, 0, st>>>(                                             \
-      ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals, ix->token_norms, wp, static_cast<const __half*>(d_queries), \
-      Q, d_query_of, d_doc_ids, n, max_len, static_cast<__half*>(d_out));
+      ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals, ix->token_norms, ix->w_perm,               \
+      static_cast<const __half*>(d_queries), Q, d_query_of, d_doc_ids, n, max_len, static_cast<__half*>(d_out));
   FPB_DISPATCH_D_NBITS(ix, CALL)
 #undef CALL
   FPB_LAUNCH_CHECK("k5_token_scores");

@@ -12,10 +12,11 @@
 //
 //   * query rows: query b owns rows [b*Qs, b*Qs + Q) of a dense row array (Qs = Q rounded up to 16, so the 16
 //     rows of an MMA warp belong to one query); rows q >= Q are zero and are left out of the sum;
-//   * 256 threads = two warpgroups.  Both decode the tile with the shared decoder (decode.cuh) in v5's 8-token
-//     passes: pass p of a document is its tokens 8p..8p+7, a partial pass repeats the last token (a duplicate
-//     cannot change a maximum), passes of consecutive documents follow each other, and a document is split only
-//     where it crosses a tile boundary.  Then the 128-row A stages are cp.async-loaded one stage ahead, and
+//   * 256 threads = two warpgroups.  Both decode the tile with the generic path of the shared decoder
+//     (decode.cuh: Decoder, then ehat_chunk per 16-byte SWIZZLE_128B chunk) in v5's 8-token passes: pass p of a
+//     document is its tokens 8p..8p+7, a partial pass repeats the last token (a duplicate cannot change a
+//     maximum), passes of consecutive documents follow each other, and a document is split only where it
+//     crosses a tile boundary.  Then the 128-row A stages are cp.async-loaded one stage ahead, and
 //     warpgroup c multiplies its 64 rows against the tile with wgmma.m64n128k16 (two 128-token blocks issued
 //     back to back; the epilogue starts once both have completed);
 //   * the per-document maxima come straight out of the accumulator registers (column group j = one pass, as in
@@ -227,16 +228,8 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
             const float nf = __half2float(norms[tok[u]]);
             const float rc = __frcp_rn(nf);
 #pragma unroll
-            for (int i = 0; i < EPL / 8; ++i) {
-              uint32_t o[4];
-#pragma unroll
-              for (int h = 0; h < 4; ++h) {
-                const float2 f = __half22float2(e[4 * i + h]);
-                o[h] = pack_half2_rn(div_rn(f.x, nf, rc), div_rn(f.y, nf, rc));
-              }
-              *reinterpret_cast<uint4*>(smB + sw128_off(r, sub * (EPL / 8) + i, S::b_kblock)) =
-                  make_uint4(o[0], o[1], o[2], o[3]);
-            }
+            for (int i = 0; i < EPL / 8; ++i)
+              *reinterpret_cast<uint4*>(smB + sw128_off(r, sub * (EPL / 8) + i, S::b_kblock)) = ehat_chunk(e, i, nf, rc);
           }
         }
       }
@@ -386,8 +379,6 @@ int launch_k7_t(const fpb_index* ix, const ExLayout& X, char* ws, cudaStream_t s
   constexpr int smem = K7Smem<D>::bytes;
   // opt in on every launch: the attribute is per device and the call costs about a microsecond
   FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  WPerm wp;
-  for (int i = 0; i < 16; ++i) wp.v[i] = ix->w_perm_bits[i];
   // documents per chunk: as many as one warp scans, fewer (down to 4, as in v5) when that leaves too few chunks to
   // balance the SMs.  FPB_K7_DOCS_PER_CHUNK=n (1..32) pins it: the result does not depend on it, and the tests use
   // it to run the multi-document chunk walk on small indexes.
@@ -400,7 +391,7 @@ int launch_k7_t(const fpb_index* ix, const ExLayout& X, char* ws, cudaStream_t s
   const int64_t chunks = (ix->N + dpc - 1) / dpc;
   const int blocks = int(chunks < X.grid ? chunks : X.grid);
   kern<<<blocks, K7_THREADS, smem, st>>>(ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals,
-                                         ix->token_norms, wp, reinterpret_cast<const __half*>(ws + X.off_rows), X.B,
+                                         ix->token_norms, ix->w_perm, reinterpret_cast<const __half*>(ws + X.off_rows), X.B,
                                          X.Q, X.Qs, X.n_rows, ix->N, dpc,
                                          reinterpret_cast<unsigned long long*>(ws + X.off_acc),
                                          reinterpret_cast<float*>(ws + X.off_carry),
