@@ -33,6 +33,17 @@ struct fpb_index {
   // It is a property of the token, not of the (query, document) pair: the MaxSim kernels read it (2 B/token)
   // instead of re-deriving it for every pair.  Caller-owned buffer filled by fpb_index_create.
   const __half* token_norms;
+  // derived at load time, owned by the handle: the approximate stage's copy of the codes (k3_approx.cu).  Document
+  // d owns the 32-token windows walk_win[d] .. walk_win[d+1] - 1 (ceil(len/32) of them) of walk_codes; its codes
+  // are dealt over them so that the bitmap words they test in shared memory spread over the 32 banks, and empty
+  // slots hold padding codes >= K (fpb_walk_pad_code).  A max over a document's tokens does not depend on their
+  // order, so every approximate score is unchanged.
+  int32_t* walk_codes;  // [32 * walk_win[N]]
+  int64_t* walk_win;    // [N + 1]
+  // windows per group of the bound pass (4, 5 or 6), chosen at load: the group count of a document is rounded up to
+  // whole groups, and the windows past its end still cost their bit tests, so the width that wastes the fewest
+  // window slots over the index is taken (every 300-token document is 10 windows: 5; 1024 tokens: 4)
+  int walk_group;
   const int64_t* ivf_offsets;  // nullptr => compress_only
   const int32_t* ivf_pids;
   // w_perm[i] = bucket_weights[bitrev_nbits(i)]  (closed form of the two LUTs of
@@ -66,6 +77,15 @@ void fpb_set_error(const char* fmt, ...);
   } while (0)
 
 static inline int64_t fpb_align256(int64_t x) { return (x + 255) & ~int64_t(255); }
+// Words of a query's K-bit map of high centroids (two-pass approximate stage): a multiple of 4, so that the map is
+// uint4-copyable.  The bound pass keeps 32 zero words after it in shared memory, one per bank.
+static inline int fpb_hb_words(int64_t K) { return int(((K + 31) / 32 + 3) / 4 * 4); }
+// The padding code of the walk layout whose bitmap word (hb_words + l' with (hb_words + l') % 32 == bank) is a zero
+// word in `bank`: it never tests high, never adds a bank conflict to a window whose real codes leave `bank` free,
+// and is >= K, so the walkers skip its gather.
+__host__ __device__ inline int32_t fpb_walk_pad_code(int hb_words, int bank) {
+  return int32_t(hb_words + ((bank - hb_words) & 31)) * 32;
+}
 static inline int fpb_next_pow2(int x) {
   int p = 1;
   while (p < x) p <<= 1;

@@ -37,6 +37,46 @@ static int make_centroid_tmap(fpb_index* ix) {
   return 0;
 }
 
+// The approximate stage's walk layout (common.cuh, k3_approx.cu): window starts on the host from the document
+// offsets, then the codes dealt on the device.  Owned by the handle (fpb_index_destroy frees it).
+static int make_walk_layout(fpb_index* ix) {
+  const int64_t N = ix->N;
+  int64_t* offs = new int64_t[N + 1];
+  int64_t* win = new int64_t[N + 1];
+  offs[0] = 0;
+  cudaError_t e = N > 0 ? cudaMemcpy(offs, ix->doc_offsets, sizeof(int64_t) * (N + 1), cudaMemcpyDeviceToHost)
+                        : cudaSuccess;
+  win[0] = 0;
+  int64_t slots[3] = {0, 0, 0};  // window slots the bound pass walks with groups of 4, 5, 6 windows
+  for (int64_t d = 0; d < N; ++d) {
+    const int64_t nw = (offs[d + 1] - offs[d] + 31) / 32;
+    win[d + 1] = win[d] + nw;
+    for (int g = 4; g <= 6; ++g) slots[g - 4] += (nw > g ? (nw + g - 1) / g : 1) * g;
+  }
+  ix->walk_group = 6;  // on a tie the widest group: more code loads in flight
+  for (int g = 5; g >= 4; --g)
+    if (slots[g - 4] < slots[ix->walk_group - 4]) ix->walk_group = g;
+  const int64_t n_win = win[N];
+  if (e == cudaSuccess) e = cudaMalloc(&ix->walk_win, sizeof(int64_t) * (N + 1));
+  if (e == cudaSuccess) e = cudaMemcpy(ix->walk_win, win, sizeof(int64_t) * (N + 1), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMalloc(&ix->walk_codes, sizeof(int32_t) * 32 * (n_win > 0 ? n_win : 1));
+  delete[] offs;
+  delete[] win;
+  if (e != cudaSuccess) {
+    fpb_set_error("walk layout: %s", cudaGetErrorString(e));
+    return FPB_ERR_CUDA;
+  }
+  if (n_win == 0) return FPB_OK;
+  const int rc = launch_walk_layout(ix, nullptr);
+  if (rc != FPB_OK) return rc;
+  e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    fpb_set_error("walk layout kernel failed: %s", cudaGetErrorString(e));
+    return FPB_ERR_CUDA;
+  }
+  return FPB_OK;
+}
+
 static thread_local char g_err[512] = "";
 
 void fpb_set_error(const char* fmt, ...) {
@@ -80,7 +120,8 @@ extern "C" int fpb_index_create(fpb_index** out, int device, int nbits, int dim,
     fpb_set_error("fpb_index_create: bad sizes or NULL codec/offset pointers");
     return FPB_ERR_INVALID;
   }
-  if (n_docs >= (int64_t(1) << 31) || n_centroids >= (int64_t(1) << 31)) {
+  // n_centroids: the walk layout's padding codes (up to 32 * (hb_words + 31)) are int32 too
+  if (n_docs >= (int64_t(1) << 31) || n_centroids >= (int64_t(1) << 31) - 2048) {
     fpb_set_error("fpb_index_create: n_docs and n_centroids must fit in int32 per shard");
     return FPB_ERR_UNSUPPORTED;
   }
@@ -144,12 +185,41 @@ extern "C" int fpb_index_create(fpb_index** out, int device, int nbits, int dim,
       return rc != FPB_OK ? rc : FPB_ERR_CUDA;
     }
   }
+  const int rc = make_walk_layout(ix);
+  if (rc != FPB_OK) {
+    fpb_index_destroy(ix);
+    return rc;
+  }
   make_centroid_tmap(ix);
   *out = ix;
   return FPB_OK;
 }
 
-extern "C" void fpb_index_destroy(fpb_index* index) { delete index; }
+extern "C" void fpb_index_destroy(fpb_index* index) {
+  if (!index) return;
+  if (index->walk_codes || index->walk_win) {
+    int prev = -1;
+    const bool have_prev = cudaGetDevice(&prev) == cudaSuccess;
+    cudaSetDevice(index->device);
+    cudaFree(index->walk_codes);
+    cudaFree(index->walk_win);
+    if (have_prev) cudaSetDevice(prev);
+  }
+  delete index;
+}
+
+extern "C" int fpb_index_walk_layout(const fpb_index* ix, int64_t* n_windows, int32_t* d_codes, int64_t* d_win) {
+  if (!ix || !n_windows) {
+    fpb_set_error("fpb_index_walk_layout: NULL argument");
+    return FPB_ERR_INVALID;
+  }
+  FPB_CUDA_CHECK(cudaSetDevice(ix->device));
+  FPB_CUDA_CHECK(cudaMemcpy(n_windows, ix->walk_win + ix->N, sizeof(int64_t), cudaMemcpyDeviceToHost));
+  if (d_codes && *n_windows > 0)
+    FPB_CUDA_CHECK(cudaMemcpy(d_codes, ix->walk_codes, sizeof(int32_t) * 32 * *n_windows, cudaMemcpyDeviceToDevice));
+  if (d_win) FPB_CUDA_CHECK(cudaMemcpy(d_win, ix->walk_win, sizeof(int64_t) * (ix->N + 1), cudaMemcpyDeviceToDevice));
+  return FPB_OK;
+}
 
 extern "C" int fpb_workspace_layout(const fpb_index* ix, int B, int Q, const fpb_params* p,
                                     fpb_layout* L) {
@@ -217,7 +287,7 @@ extern "C" int fpb_workspace_layout(const fpb_index* ix, int B, int Q, const fpb
   L->off_sbitmap = take(sub ? int64_t(B) * L->bitmap_words * 4 : 0);
   // two-pass approximate stage (k3_approx.cu); hb_words is a multiple of 4 so a query's bitmap is uint4-copyable
   const bool direct = (p->flags & FPB_FLAG_APPROX_DIRECT) != 0;
-  L->hb_words = int(((ix->K + 31) / 32 + 3) / 4 * 4);
+  L->hb_words = fpb_hb_words(ix->K);
   L->off_tau = take(direct ? 0 : int64_t(B) * Qp * 2);
   L->off_hibits = take(direct ? 0 : int64_t(B) * L->hb_words * 4);
   L->off_lb = take(direct ? 0 : int64_t(B) * L->cand_cap * 4);

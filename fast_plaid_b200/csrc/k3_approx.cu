@@ -107,6 +107,86 @@ __device__ __forceinline__ float k3_sum_columns(__half2 m0, __half2 m1, __half2 
 }
 
 // ---------------------------------------------------------------------------------------
+// The walk layout (fpb_index::walk_codes, built once at index load by k3_walk_layout_kernel).  Every K3 walker
+// visits a document as whole 32-token windows of its own: aligned 128-byte code loads and no masks, and a slot
+// whose code is >= K (padding) gathers nothing.  In the bound pass each lane of a window tests the bitmap word
+// code >> 5 in shared memory, whose bank is (code >> 5) & 31, fixed by the code and not by the query.  The 32
+// tests of a window cost as many shared-memory wavefronts as the most crowded bank holds distinct words: ~3.5 for
+// 32 random codes.  So each document's tokens are stable-sorted by bank and dealt round-robin over its
+// ceil(len/32) windows -- a bank with c tokens gets at most ceil(c / windows) slots of any window -- and a window's
+// empty slots take padding codes (fpb_walk_pad_code) in banks its real codes leave free.
+// ---------------------------------------------------------------------------------------
+constexpr int K3_WALK_THREADS = 256;
+
+__global__ void __launch_bounds__(K3_WALK_THREADS)
+k3_walk_layout_kernel(const int64_t* __restrict__ doc_offsets, const int32_t* __restrict__ codes,
+                      const int64_t* __restrict__ walk_win, int64_t N, int hb_words, int32_t* __restrict__ walk_codes) {
+  __shared__ int s_cnt[K3_WALK_THREADS / 32][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned lt_mask;
+  asm("mov.u32 %0, %%lanemask_lt;" : "=r"(lt_mask));
+  int* cnt = s_cnt[warp];
+  for (int64_t d = int64_t(blockIdx.x) * (K3_WALK_THREADS / 32) + warp; d < N;
+       d += int64_t(gridDim.x) * (K3_WALK_THREADS / 32)) {
+    const int64_t o0 = doc_offsets[d];
+    const int len = int(doc_offsets[d + 1] - o0);
+    const int nw = (len + 31) >> 5;
+    int32_t* out = walk_codes + walk_win[d] * 32;
+    // tokens per bank, then each bank's first position in the stable order by bank
+    cnt[lane] = 0;
+    __syncwarp();
+    for (int t0 = 0; t0 < len; t0 += 32) {
+      const bool act = t0 + lane < len;
+      const unsigned am = __ballot_sync(0xffffffffu, act);
+      if (act) {
+        const int bank = (__ldg(codes + o0 + t0 + lane) >> 5) & 31;
+        const unsigned peers = __match_any_sync(am, bank);
+        if ((peers & lt_mask) == 0u) cnt[bank] += __popc(peers);
+      }
+      __syncwarp();
+    }
+    {
+      const int c = cnt[lane];
+      int incl = c;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, incl, off);
+        if (lane >= off) incl += v;
+      }
+      __syncwarp();
+      cnt[lane] = incl - c;
+      __syncwarp();
+    }
+    // sorted position i goes to slot i / nw of window i % nw
+    for (int t0 = 0; t0 < len; t0 += 32) {
+      const bool act = t0 + lane < len;
+      const unsigned am = __ballot_sync(0xffffffffu, act);
+      int code = 0, bank = 0, i = 0;
+      unsigned peers = 0u;
+      if (act) {
+        code = __ldg(codes + o0 + t0 + lane);
+        bank = (code >> 5) & 31;
+        peers = __match_any_sync(am, bank);
+        i = cnt[bank] + __popc(peers & lt_mask);
+      }
+      __syncwarp();
+      if (act && (peers & lt_mask) == 0u) cnt[bank] += __popc(peers);
+      __syncwarp();
+      if (act) out[(i % nw) * 32 + i / nw] = code;
+    }
+    __syncwarp();  // the stores above are read back below
+    // window w holds the positions i < len with i % nw == w; each empty slot takes the next bank no real code of
+    // the window uses (a window of r real codes uses at most r banks, so 32 - r are free)
+    for (int w = 0; w < nw; ++w) {
+      const int r = (len - w + nw - 1) / nw;
+      const unsigned used = __reduce_or_sync(0xffffffffu, lane < r ? 1u << ((out[w * 32 + lane] >> 5) & 31) : 0u);
+      if (lane >= r) out[w * 32 + lane] = fpb_walk_pad_code(hb_words, int(__fns(~used, 0, lane - r + 1)));
+    }
+    __syncwarp();
+  }
+}
+
+// ---------------------------------------------------------------------------------------
 // Exact pass / one-pass scoring.  One warp walks one candidate; each S row (Qp fp16 = LPR x 16 B) is fetched
 // by LPR adjacent lanes, so a warp-wide load touches 32/LPR distinct rows, and the running maxima stay in
 // registers.  `list` (the bound pass's refine list) selects the candidates; NULL = all of them.
@@ -116,7 +196,8 @@ __device__ __forceinline__ float k3_sum_columns(__half2 m0, __half2 m1, __half2 
 template <int LPR, int UNROLL, int MINB>
 __global__ void __launch_bounds__(K3_THREADS, MINB)
 k3_approx_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
-                 const int32_t* __restrict__ codes, const int32_t* __restrict__ cand, int cand_cap,
+                 const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
+                 const int32_t* __restrict__ cand, int cand_cap,
                  const int32_t* __restrict__ n_cand, const int32_t* __restrict__ list,
                  const int32_t* __restrict__ n_list, int32_t* __restrict__ work, int B,
                  float* __restrict__ approx, unsigned long long* __restrict__ stats) {
@@ -125,6 +206,7 @@ k3_approx_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* 
   __shared__ int s_b, s_c;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int sub = lane % LPR, grp = lane / LPR;
+  const int Ki = int(K);
   const __half2 sentinel = __float2half2_rn(FPB_PAD_SENTINEL);
   unsigned long long rows = 0;
 
@@ -146,20 +228,19 @@ k3_approx_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* 
       const int64_t o0 = doc_offsets[d];
       const int len = int(doc_offsets[d + 1] - o0);
       rows += unsigned(len);
+      const int nw = (len + 31) >> 5;
+      const int32_t* cw = walk_codes + walk_win[d] * 32 + lane;
       __half2 m0 = sentinel, m1 = sentinel, m2 = sentinel, m3 = sentinel;
-      for (int base = 0; base < len; base += 32 * UNROLL) {
+      for (int w0 = 0; w0 < nw; w0 += UNROLL) {
         int code[UNROLL];
 #pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-          const int t = base + u * 32 + lane;
-          code[u] = (t < len) ? __ldg(codes + o0 + t) : -1;
-        }
+        for (int u = 0; u < UNROLL; ++u) code[u] = (w0 + u < nw) ? __ldg(cw + (w0 + u) * 32) : Ki;
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
 #pragma unroll
           for (int jj = 0; jj < LPR; ++jj) {
             const int c = __shfl_sync(0xffffffffu, code[u], jj * TPI + grp);
-            if (c >= 0) {
+            if (c < Ki) {
               const uint4 v = __ldg(Sb + int64_t(c) * LPR + sub);
               m0 = __hmax2(m0, u32_as_half2(v.x));
               m1 = __hmax2(m1, u32_as_half2(v.y));
@@ -178,9 +259,8 @@ k3_approx_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* 
 }
 
 // Shuffle-free variant: the LPR lanes of a group load "their" LPR consecutive codes themselves with one
-// vector load (the lanes of a group read the same 4*LPR bytes: a broadcast); the document is walked in
-// 32-token windows aligned to absolute multiples of 32 tokens, so the vector loads are aligned whatever the
-// document offset; tokens outside [o0, o0+len) are masked.  max() is order-free: bit-identical values.
+// vector load (the lanes of a group read the same 4*LPR bytes: a broadcast); the windows of the walk layout
+// are 128-byte aligned, so the vector loads are too.
 template <int LPR>
 __device__ __forceinline__ void load_codes(int (&c)[LPR], const int32_t* p) {
   if constexpr (LPR == 2) {
@@ -198,14 +278,16 @@ __device__ __forceinline__ void load_codes(int (&c)[LPR], const int32_t* p) {
 template <int LPR, int UNROLL, int MINB>
 __global__ void __launch_bounds__(K3_THREADS, MINB)
 k3_approx_nsh_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
-                     const int32_t* __restrict__ codes, int64_t n_codes, const int32_t* __restrict__ cand,
-                     int cand_cap, const int32_t* __restrict__ n_cand, const int32_t* __restrict__ list,
-                     const int32_t* __restrict__ n_list, int32_t* __restrict__ work, int B,
-                     float* __restrict__ approx, unsigned long long* __restrict__ stats) {
+                     const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
+                     const int32_t* __restrict__ cand, int cand_cap, const int32_t* __restrict__ n_cand,
+                     const int32_t* __restrict__ list, const int32_t* __restrict__ n_list,
+                     int32_t* __restrict__ work, int B, float* __restrict__ approx,
+                     unsigned long long* __restrict__ stats) {
   constexpr int QP = LPR * 8;
   __shared__ int s_b, s_c;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int sub = lane % LPR, grp = lane / LPR;
+  const int Ki = int(K);
   const __half2 sentinel = __float2half2_rn(FPB_PAD_SENTINEL);
   unsigned long long rows = 0;
 
@@ -227,32 +309,25 @@ k3_approx_nsh_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64
       const int64_t o0 = doc_offsets[d];
       const int len = int(doc_offsets[d + 1] - o0);
       rows += unsigned(len);
-      // frame: token f of the frame is absolute token w0 + f; the document is [lo, hi)
-      const int64_t w0 = o0 & ~int64_t(31);
-      const int lo = int(o0 - w0), hi = lo + len;
-      const int32_t* cw = codes + w0 + grp * LPR;
-      // the last window may reach past the end of the code array: lanes whose LPR codes are not all
-      // inside it take the scalar path (at most once per index)
-      const int64_t readable = n_codes - (w0 + grp * LPR);
+      const int nw = (len + 31) >> 5;
+      const int32_t* cw = walk_codes + walk_win[d] * 32 + grp * LPR;
       __half2 m0 = sentinel, m1 = sentinel, m2 = sentinel, m3 = sentinel;
-      for (int f0 = 0; f0 < hi; f0 += 32 * UNROLL) {
+      for (int w0 = 0; w0 < nw; w0 += UNROLL) {
         int c[UNROLL][LPR];
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
-          const int fo = f0 + u * 32;
-          if (fo + LPR <= readable) {
-            load_codes<LPR>(c[u], cw + fo);
+          if (w0 + u < nw) {
+            load_codes<LPR>(c[u], cw + (w0 + u) * 32);
           } else {
 #pragma unroll
-            for (int jj = 0; jj < LPR; ++jj) c[u][jj] = (fo + jj < readable) ? __ldg(cw + fo + jj) : 0;
+            for (int jj = 0; jj < LPR; ++jj) c[u][jj] = Ki;
           }
         }
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u) {
 #pragma unroll
           for (int jj = 0; jj < LPR; ++jj) {
-            const int f = f0 + u * 32 + grp * LPR + jj;
-            if (unsigned(f - lo) < unsigned(len)) {
+            if (c[u][jj] < Ki) {
               const uint4 v = __ldg(Sb + int64_t(c[u][jj]) * LPR);
               m0 = __hmax2(m0, u32_as_half2(v.x));
               m1 = __hmax2(m1, u32_as_half2(v.y));
@@ -289,7 +364,8 @@ constexpr int K3_TAU_THREADS = 1024;
 template <int LPR>
 __global__ void __launch_bounds__(K3_TAU_THREADS)
 k3_tau_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
-              const int32_t* __restrict__ codes, const int32_t* __restrict__ cand, int cand_cap,
+              const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
+              const int32_t* __restrict__ cand, int cand_cap,
               const int32_t* __restrict__ n_cand, const __half* __restrict__ tmax, int n_tiles, float lambda,
               __half* __restrict__ tau) {
   constexpr int QP = LPR * 8, TPI = 32 / LPR;
@@ -300,6 +376,7 @@ k3_tau_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __r
   __shared__ int s_redo;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int sub = lane % LPR, grp = lane / LPR;
+  const int Ki = int(K);
   uint16_t* out = reinterpret_cast<uint16_t*>(tau) + int64_t(b) * QP;
   const int n = n_cand[b];
   const int ns = min(n, K3_TAU_DOCS);
@@ -333,11 +410,10 @@ k3_tau_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __r
       for (int e = 0; e < 8; ++e) fl[e] = (mine && !s_redo) ? s_floor[qrow + e] : 0u;
       for (int j = warp; j < ns; j += K3_TAU_THREADS / 32) {
         const int d = cb[int64_t(j) * n / ns];
-        const int64_t o0 = doc_offsets[d];
-        const int len = int(doc_offsets[d + 1] - o0);
-        for (int base = 0; base < len; base += 32) {
-          const int t = base + lane;
-          const int code = (t < len) ? __ldg(codes + o0 + t) : -1;
+        const int nw = int((doc_offsets[d + 1] - doc_offsets[d] + 31) >> 5);
+        const int32_t* cw = walk_codes + walk_win[d] * 32 + lane;
+        for (int w = 0; w < nw; ++w) {
+          const int code = __ldg(cw + w * 32);
           // all LPR row gathers of the window go out before the first histogram update (the kernel is a chain of
           // dependent latencies otherwise)
           constexpr int JB = LPR < 8 ? LPR : 8;  // gathers in flight per lane
@@ -349,12 +425,12 @@ k3_tau_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __r
           for (int jj = 0; jj < JB; ++jj) {
             cc[jj] = __shfl_sync(0xffffffffu, code, (j0 + jj) * TPI + grp);
             vv[jj] = make_uint4(0u, 0u, 0u, 0u);
-            if (cc[jj] >= 0 && mine) vv[jj] = __ldg(Sb + int64_t(cc[jj]) * LPR + sub);
+            if (cc[jj] < Ki && mine) vv[jj] = __ldg(Sb + int64_t(cc[jj]) * LPR + sub);
           }
 #pragma unroll
           for (int jj = 0; jj < JB; ++jj) {
             const int c = cc[jj];
-            if (c >= 0 && mine) {
+            if (c < Ki && mine) {
               const uint4 v = vv[jj];
               const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
@@ -453,7 +529,8 @@ k3_hibits_kernel(const __half* __restrict__ S, int64_t K, const __half* __restri
 // window, a third of them branches and generic-address arithmetic around the shared-memory accesses), so the
 // per-window path is written branch-free with explicit 32-bit
 // shared addresses: predicated code load, one LDS of the bitmap word, a wrap-around funnel shift for the bit, ballot,
-// predicated STS into the ring.  Tokens outside the document carry the code K3_INV whose bit is a spare zero word.
+// predicated STS into the ring.  The 32 words after the bitmap are zero: the walk layout's padding codes test them,
+// and so do the windows of a group past the end of the document (all lanes one word: a broadcast).
 __device__ __forceinline__ uint32_t k3_lds(uint32_t addr) {
   uint32_t v;
   asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
@@ -491,7 +568,8 @@ __device__ __forceinline__ unsigned k3_push(uint32_t word, uint32_t code, uint32
 template <int LPR, int MINB, int W, int U, bool FULLQ, bool PAIR>
 __global__ void __launch_bounds__(K3_THREADS, MINB)
 k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
-                const int32_t* __restrict__ codes, const int32_t* __restrict__ cand, int cand_cap,
+                const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
+                const int32_t* __restrict__ cand, int cand_cap,
                 const int32_t* __restrict__ n_cand, int32_t* __restrict__ work, int B,
                 const __half* __restrict__ tau, const uint32_t* __restrict__ hibits, int hb_words,
                 float* __restrict__ ub_out, float* __restrict__ lb_out, unsigned long long* __restrict__ stats) {
@@ -501,22 +579,22 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
   constexpr int DPW = K3A_DOCS_PER_CHUNK / (K3_THREADS / 32);  // documents per warp and chunk
   constexpr int WQ = K3_WQ_FOR(W, FLUSH);  // ring entries per warp: one group of pushes on top of an unflushed rest
   static_assert(FLUSH + 32 * W <= WQ, "ring too small");
-  extern __shared__ __align__(16) uint32_t k3_smem[];  // [hb_words + 4] bitmap (+ a zero word) | [warps][WQ] rings
+  extern __shared__ __align__(16) uint32_t k3_smem[];  // [hb_words + 32] bitmap + 32 zero words | [warps][WQ] rings
   __shared__ int s_b, s_c;
-  __shared__ int64_t s_o0[K3A_DOCS_PER_CHUNK];
+  __shared__ int64_t s_w0[K3A_DOCS_PER_CHUNK];
   __shared__ int s_len[K3A_DOCS_PER_CHUNK];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int sub = lane % LPR, grp = lane / LPR;
   const uint32_t sb_bm = smem_u32(k3_smem);
   // rings: aligned to their size (WQ * 4 bytes) so that k3_push can OR the base in
-  const uint32_t sb_wq = ((sb_bm + uint32_t(hb_words + 4) * 4u + (WQ * 4u - 1u)) & ~(WQ * 4u - 1u)) + uint32_t(warp) * (WQ * 4u);
-  const int INV = hb_words * 32;  // a code whose bit lives in the spare zero word
+  const uint32_t sb_wq = ((sb_bm + uint32_t(hb_words + 32) * 4u + (WQ * 4u - 1u)) & ~(WQ * 4u - 1u)) + uint32_t(warp) * (WQ * 4u);
+  const int INV = hb_words * 32;  // a code whose bit lives in a zero word
   unsigned lt_mask;
   asm("mov.u32 %0, %%lanemask_lt;" : "=r"(lt_mask));
   const __half2 sentinel = __float2half2_rn(FPB_PAD_SENTINEL);
   unsigned rows = 0, toks = 0;  // per warp over the CTA's life: far below 2^32
   int cur_b = -1;
-  if (tid < 4) k3_smem[hb_words + tid] = 0u;  // never overwritten: the bitmap copy below covers hb_words words
+  if (tid < 32) k3_smem[hb_words + tid] = 0u;  // never overwritten: the bitmap copy below covers hb_words words
 
   for (;;) {
     k3_next_chunk(work, B, &s_b, &s_c);
@@ -526,14 +604,14 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
     const int32_t* cb = cand + int64_t(b) * cand_cap;
     if (tid < K3A_DOCS_PER_CHUNK) {  // stage the chunk's document extents
       const int idx = s_c * K3A_DOCS_PER_CHUNK + tid;
-      int64_t o0 = 0;
+      int64_t w0 = 0;
       int len = -1;  // -1: no such document
       if (idx < n) {
         const int d = cb[idx];
-        o0 = doc_offsets[d];
-        len = int(doc_offsets[d + 1] - o0);
+        w0 = walk_win[d];
+        len = int(doc_offsets[d + 1] - doc_offsets[d]);
       }
-      s_o0[tid] = o0;
+      s_w0[tid] = w0;
       s_len[tid] = len;
     }
     if (b != cur_b) {  // CTA-uniform; every warp is past the previous chunk (barrier in k3_next_chunk)
@@ -552,22 +630,14 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
     const int slot_end = slot + DPW;
     int len = s_len[slot];
     if (len < 0) continue;  // warp-uniform: this warp has no document in the (last, partial) chunk
-    // rel = index inside the document of this lane's token in window 0 of the group (negative before the start);
-    // nwin = windows of the frame [0, lo + len) aligned to absolute multiples of 32 tokens (one 128-byte line each)
-    int rel, left;  // left = windows of the document not yet walked (including the current group's)
-    const int32_t* cw;
-    {
-      const int64_t o0 = s_o0[slot];
-      const int lo = int(o0 & 31);
-      rel = lane - lo;
-      left = (lo + len + 31) >> 5;
-      cw = codes + (o0 - lo) + lane;
-    }
+    // left = windows of the document not yet walked (including the current group's), one 128-byte line each
+    int left = (len + 31) >> 5;
+    const int32_t* cw = walk_codes + s_w0[slot] * 32 + lane;
     int c[W];
 #pragma unroll
     for (int u = 0; u < W; ++u) {
       c[u] = INV;
-      if (unsigned(rel + 32 * u) < unsigned(len)) c[u] = __ldg(cw + 32 * u);
+      if (u < left) c[u] = __ldg(cw + 32 * u);
     }
     uint32_t head = 0, tail = 0;
     __half2 m0 = sentinel, m1 = sentinel, m2 = sentinel, m3 = sentinel;
@@ -580,26 +650,21 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
     for (;;) {
       // ---- the next group: same document or the next slot; its code loads go out now ----
       const bool last_of_doc = left <= W;
-      int nlen = len, nrel = rel + 32 * W, nleft = left - W;
+      int nlen = len, nleft = left - W;
       const int32_t* ncw = cw + 32 * W;
       if (last_of_doc) {
         nlen = (slot + 1 < slot_end) ? s_len[slot + 1] : -1;
+        nleft = 0;
         if (nlen >= 0) {
-          const int64_t o0 = s_o0[slot + 1];
-          const int lo = int(o0 & 31);
-          nrel = lane - lo;
-          nleft = (lo + nlen + 31) >> 5;
-          ncw = codes + (o0 - lo) + lane;
+          nleft = (nlen + 31) >> 5;
+          ncw = walk_codes + s_w0[slot + 1] * 32 + lane;
         }
       }
       int nx[W];
-      {
-        const unsigned nlen_u = nlen < 0 ? 0u : unsigned(nlen);
 #pragma unroll
-        for (int u = 0; u < W; ++u) {
-          nx[u] = INV;
-          if (unsigned(nrel + 32 * u) < nlen_u) nx[u] = __ldg(ncw + 32 * u);
-        }
+      for (int u = 0; u < W; ++u) {
+        nx[u] = INV;
+        if (u < nleft) nx[u] = __ldg(ncw + 32 * u);
       }
       // ---- current group: bit of every token (W independent shared loads), queue the high codes ----
       uint32_t wbit[W];
@@ -706,7 +771,6 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
 #pragma unroll
       for (int u = 0; u < W; ++u) c[u] = nx[u];
       len = nlen;
-      rel = nrel;
       left = nleft;
       cw = ncw;
     }
@@ -1171,35 +1235,54 @@ int launch_k3_exact(const fpb_index* ix, const Ws& ws, const int32_t* list, cons
                     cudaStream_t st) {
   const fpb_layout& L = *ws.L;
   const int blocks = ix->sm_count * 8;
-  if constexpr (LPR <= 4) {
-    // shuffle-free up to Qp = 32 (the vector code loads need a 16-byte aligned code array; any torch allocation
-    // is); at Qp = 64 the shuffle kernel is used
-    if ((reinterpret_cast<uintptr_t>(ix->doc_codes) & 15u) == 0) {
-      k3_approx_nsh_kernel<LPR, 2, 6><<<blocks, K3_THREADS, 0, st>>>(
-          ws.S(), ix->K, L.Q, ix->doc_offsets, ix->doc_codes, ix->E, ws.cand(), L.cand_cap, ws.n_cand(), list, n_list,
-          work, L.B, ws.approx(), ws.stats());
-      FPB_LAUNCH_CHECK("k3_approx_nsh");
-      return FPB_OK;
-    }
+  if constexpr (LPR <= 4) {  // shuffle-free up to Qp = 32; at Qp = 64 and above the shuffle kernel is used
+    k3_approx_nsh_kernel<LPR, 2, 6><<<blocks, K3_THREADS, 0, st>>>(
+        ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes, ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), list,
+        n_list, work, L.B, ws.approx(), ws.stats());
+    FPB_LAUNCH_CHECK("k3_approx_nsh");
+    return FPB_OK;
   }
-  k3_approx_kernel<LPR, 2, 6><<<blocks, K3_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->doc_codes,
-                                                             ws.cand(), L.cand_cap, ws.n_cand(), list, n_list, work,
-                                                             L.B, ws.approx(), ws.stats());
+  k3_approx_kernel<LPR, 2, 6><<<blocks, K3_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes,
+                                                             ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), list,
+                                                             n_list, work, L.B, ws.approx(), ws.stats());
   FPB_LAUNCH_CHECK("k3_approx");
   return FPB_OK;
 }
 
 // LAMBDA of k3_tau_kernel: the expected number of tokens per candidate and column at or above tau.  A document is
 // resolved when all of its Q columns are, so the useful level grows with log Q: LAMBDA = ln(Q) - 1.45 (2.0 at
-// Q = 32, 2.7 at Q = 64).  FPB_K3_LAMBDA overrides it
-// (tuning only: every value gives the same results).
+// Q = 32, 2.7 at Q = 64).  FPB_K3_LAMBDA overrides it (tuning only: every value gives the same results); it is read
+// at every launch so that one process can sweep it (tools/profile_approx.py).
 float k3_tau_lambda(int Q) {
-  static const float pinned = [] {
-    const char* e = getenv("FPB_K3_LAMBDA");
-    return e ? float(atof(e)) : 0.f;
-  }();
+  const char* e = getenv("FPB_K3_LAMBDA");
+  const float pinned = e ? float(atof(e)) : 0.f;
   const float x = pinned > 0.f ? pinned : logf(float(Q < 2 ? 2 : Q)) - 1.45f;
   return x < 0.5f ? 0.5f : (x > 64.f ? 64.f : x);
+}
+
+// The bound pass with W windows per group (all their code loads in flight at once, the next group's prefetched), 4
+// gathers per lane and batch, 4 CTAs per SM at 64 registers, paired epilogues.
+template <int LPR, int W>
+int launch_k3_bound(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
+  const fpb_layout& L = *ws.L;
+  constexpr int TPI = 32 / LPR;
+  constexpr int U = 4, MINB = 4;
+  const bool fullq = L.Q == L.Qp;
+  auto kern = fullq ? k3_bound_kernel<LPR, MINB, W, U, true, true> : k3_bound_kernel<LPR, MINB, W, U, false, true>;
+  const int minb = MINB, wq = K3_WQ_FOR(W, U * TPI);
+  // bitmap + 32 zero words, then the rings (+ alignment slack)
+  const size_t smem = size_t(L.hb_words + 32) * 4 + size_t(K3_THREADS / 32 + 1) * wq * 4;
+  FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  // resident CTAs per SM: limited by the bitmap (228 KB of shared memory per SM, 1 KB reserved per CTA; the
+  // static shared memory is ~1.6 KB)
+  int per_sm = int((227 * 1024) / (smem + 1024 + 2048));
+  per_sm = per_sm < 1 ? 1 : (per_sm > minb ? minb : per_sm);
+  kern<<<ix->sm_count * per_sm, K3_THREADS, smem, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes,
+                                                        ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), ws.work(),
+                                                        L.B, ws.tau(), ws.hibits(), L.hb_words, ws.approx(), ws.lb(),
+                                                        ws.stats());
+  FPB_LAUNCH_CHECK("k3_bound");
+  return FPB_OK;
 }
 
 template <int LPR>
@@ -1215,9 +1298,9 @@ int launch_k3_t(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st) {
     FPB_LAUNCH_CHECK("k3_prefix");
     return launch_k3_exact<LPR>(ix, ws, nullptr, nullptr, ws.work(), st);
   }
-  k3_tau_kernel<LPR><<<L.B, K3_TAU_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->doc_codes, ws.cand(),
-                                                     L.cand_cap, ws.n_cand(), ws.tmax(), L.n_tiles, k3_tau_lambda(L.Q),
-                                                     ws.tau());
+  k3_tau_kernel<LPR><<<L.B, K3_TAU_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes,
+                                                     ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), ws.tmax(),
+                                                     L.n_tiles, k3_tau_lambda(L.Q), ws.tau());
   FPB_LAUNCH_CHECK("k3_tau");
   {
     dim3 grid(unsigned((ix->K + 255) / 256), unsigned(L.B));
@@ -1227,23 +1310,13 @@ int launch_k3_t(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st) {
   k3_prefix_kernel<<<1, 32, 0, st>>>(ws.n_cand(), L.B, K3A_DOCS_PER_CHUNK, ws.work());
   FPB_LAUNCH_CHECK("k3_prefix");
   {
-    // resident CTAs per SM: limited by the bitmap (228 KB of shared memory per SM, 1 KB reserved per CTA)
-    // shape of the walk: 6 32-token windows per group (all their code loads in flight at once, the next group's
-    // prefetched), 4 gathers per lane and batch, 4 CTAs per SM at 64 registers, paired epilogues.
-    constexpr int TPI = 32 / LPR;
-    constexpr int W = 6, U = 4, MINB = 4;
-    const bool fullq = L.Q == L.Qp;
-    auto kern = fullq ? k3_bound_kernel<LPR, MINB, W, U, true, true> : k3_bound_kernel<LPR, MINB, W, U, false, true>;
-    const int minb = MINB, wq = K3_WQ_FOR(W, U * TPI);
-    const size_t smem = size_t(L.hb_words + 4) * 4 + size_t(K3_THREADS / 32 + 1) * wq * 4;  // + alignment slack of the rings
-    FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-    // resident CTAs per SM: limited by the bitmap (228 KB of shared memory per SM, 1 KB reserved per CTA)
-    int per_sm = int((227 * 1024) / (smem + 1024 + 2048));
-    per_sm = per_sm < 1 ? 1 : (per_sm > minb ? minb : per_sm);
-    kern<<<ix->sm_count * per_sm, K3_THREADS, smem, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->doc_codes, ws.cand(),
-                                                          L.cand_cap, ws.n_cand(), ws.work(), L.B, ws.tau(),
-                                                          ws.hibits(), L.hb_words, ws.approx(), ws.lb(), ws.stats());
-    FPB_LAUNCH_CHECK("k3_bound");
+    // windows per group: the index's choice (fpb_index::walk_group), FPB_K3_GROUP overrides it (tuning only: every
+    // value gives the same results; read at every launch like FPB_K3_LAMBDA)
+    const char* e = getenv("FPB_K3_GROUP");
+    const int g = e ? atoi(e) : ix->walk_group;
+    const int rc = g == 4 ? launch_k3_bound<LPR, 4>(ix, ws, st)
+                 : g == 5 ? launch_k3_bound<LPR, 5>(ix, ws, st) : launch_k3_bound<LPR, 6>(ix, ws, st);
+    if (rc != FPB_OK) return rc;
   }
   k3_refine_list_kernel<<<L.B, 1024, 0, st>>>(ws.approx(), ws.lb(), L.cand_cap, ws.n_cand(), L.R,
                                               (flags & FPB_FLAG_APPROX_EXACT_ALL) ? 1 : 0, ws.refine(), ws.n_refine(),
@@ -1268,6 +1341,17 @@ int launch_approx(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st)
       fpb_set_error("approx scoring: unsupported padded query length %d", L.Qp);
       return FPB_ERR_UNSUPPORTED;
   }
+}
+
+int launch_walk_layout(const fpb_index* ix, cudaStream_t st) {
+  if (ix->N == 0) return FPB_OK;
+  const int64_t warps = K3_WALK_THREADS / 32;
+  const int64_t need = (ix->N + warps - 1) / warps;
+  const int blocks = int(need < int64_t(ix->sm_count) * 16 ? need : int64_t(ix->sm_count) * 16);
+  k3_walk_layout_kernel<<<blocks, K3_WALK_THREADS, 0, st>>>(ix->doc_offsets, ix->doc_codes, ix->walk_win, ix->N,
+                                                            fpb_hb_words(ix->K), ix->walk_codes);
+  FPB_LAUNCH_CHECK("k3_walk_layout");
+  return FPB_OK;
 }
 
 int launch_select(const fpb_index* ix, const Ws& ws, cudaStream_t st) {

@@ -46,6 +46,7 @@ int launch_subset(const fpb_index* ix, const Ws& ws, const int32_t* d_ids, const
 int launch_compact(const uint32_t* bitmap, const uint32_t* mask, int words, int32_t* out, int cap, int32_t* n_out,
                    int B, cudaStream_t st);
 int launch_approx(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st); // K3 (flags: FPB_FLAG_APPROX_*)
+int launch_walk_layout(const fpb_index* ix, cudaStream_t st);                     // K3's walk_codes (index load)
 int launch_select(const fpb_index* ix, const Ws& ws, cudaStream_t st);            // K3b
 int launch_maxsim(const fpb_index* ix, const Ws& ws, cudaStream_t st);            // K5 (dispatch)
 int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st);      // per-token fp16 norms (index load)

@@ -100,6 +100,7 @@ EXPORTED_SYMBOLS = [
     "fpb_abi_version",
     "fpb_index_create",
     "fpb_index_destroy",
+    "fpb_index_walk_layout",
     "fpb_workspace_layout",
     "fpb_search_batch",
     "fpb_search_batch_subset",
@@ -167,6 +168,8 @@ def load_library() -> ctypes.CDLL:
         ]
         lib.fpb_index_destroy.restype = None
         lib.fpb_index_destroy.argtypes = [vp]
+        lib.fpb_index_walk_layout.restype = i32
+        lib.fpb_index_walk_layout.argtypes = [vp, ctypes.POINTER(i64), vp, vp]
         lib.fpb_workspace_layout.restype = i32
         lib.fpb_workspace_layout.argtypes = [vp, i32, i32, ctypes.POINTER(FpbParams), ctypes.POINTER(FpbLayout)]
         lib.fpb_search_batch.restype = i32
@@ -1122,6 +1125,17 @@ class DeviceIndex:
             "thresh": v(lay.off_thresh, B * 4, torch.float32, (B,)),
             "stats": v(lay.off_stats, 64, torch.int64, (8,)),
         }
+
+    def walk_layout(self) -> tuple[torch.Tensor, torch.Tensor]:
+        """Copies of the approximate stage's walk layout (csrc/common.cuh): codes int32 [windows, 32] and each
+        document's first window, int64 [N + 1]."""
+        n = ctypes.c_int64()
+        with self._exclusive(), torch.cuda.device(self.device):
+            _check(self._lib.fpb_index_walk_layout(self._handle, ctypes.byref(n), None, None))
+            codes = torch.empty((max(n.value, 1), 32), dtype=torch.int32, device=self.device)
+            win = torch.empty(self.num_documents + 1, dtype=torch.int64, device=self.device)
+            _check(self._lib.fpb_index_walk_layout(self._handle, ctypes.byref(n), codes.data_ptr(), win.data_ptr()))
+        return codes[: n.value], win
 
     # -- by-products -----------------------------------------------------------------------
     def reconstruct(self, doc_ids: list[int]) -> list[torch.Tensor]:

@@ -63,6 +63,10 @@ int fpb_abi_version(void);
  *
  * The two 256-entry LUTs of the reference collapse into one (1<<nbits)-entry permuted
  * weight table w_perm[i] = bucket_weights[bitrev_nbits(i)] built here on the host.
+ *
+ * The handle also allocates and owns one derived device array that fpb_index_destroy frees: the approximate
+ * stage's copy of the codes, each document's tokens reordered into whole 32-token windows (4 bytes per token
+ * rounded up to a multiple of 32 per document, plus 8 bytes per document).
  */
 int fpb_index_create(fpb_index** out, int device, int nbits, int dim, int64_t n_centroids,
                      const void* d_centroids, const void* d_bucket_weights, int64_t n_docs,
@@ -71,6 +75,10 @@ int fpb_index_create(fpb_index** out, int device, int nbits, int dim, int64_t n_
                      const int32_t* d_ivf_pids, int64_t n_ivf, int64_t max_doc_len,
                      int64_t doc_id_base);
 void fpb_index_destroy(fpb_index* index);
+/* The walk layout of an index (tests and tools): *n_windows = number of 32-code windows; when non-NULL, d_codes
+ * (i32 [32 * n_windows]) and d_win (i64 [n_docs + 1], first window of each document) receive device copies.
+ * Synchronous. */
+int fpb_index_walk_layout(const fpb_index* index, int64_t* n_windows, int32_t* d_codes, int64_t* d_win);
 
 /* Search parameters -- mirrors `SearchParameters` (rust/search/search.rs:171-200).
  * `batch_size` (document batch of the approximate stage) only bounds memory in the
