@@ -302,8 +302,8 @@ int launch_pad_queries(const fpb_index* ix, const Ws& ws, const __half* d_querie
 }
 
 int launch_centroid_scores(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
-  // FPB_K1=v1 pins the mma.sync kernel; default is the wgmma kernel where it applies.
-  static const char* pin = getenv("FPB_K1");
+  // FPB_K1=v1 pins the mma.sync kernel; default is the wgmma kernel where it applies.  Read at every launch.
+  const char* pin = getenv("FPB_K1");
   if (!pin || pin[1] != '1') {
     bool handled = false;
     const int rc = launch_centroid_scores_v2(ix, ws, st, &handled);

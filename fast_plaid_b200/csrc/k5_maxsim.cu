@@ -288,8 +288,8 @@ int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st) {
 int launch_maxsim(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   // dim 128, nbits 4: Qp <= 32 -> v4 (register-resident operands, mma.sync), 32 < Qp <= 128 -> v5 (wgmma);
   // everything else (dim 64, nbits 2, Qp = 256, documents longer than v5's pass table) -> the generic kernel here.
-  // FPB_K5=v1 pins the generic kernel (the A/B alternative).
-  static const char* pin = getenv("FPB_K5");
+  // FPB_K5=v1 pins the generic kernel (the A/B alternative); read at every launch, so one process can switch.
+  const char* pin = getenv("FPB_K5");
   const bool generic_only = pin && pin[1] == '1';
   bool handled = false;
   int rc = FPB_OK;

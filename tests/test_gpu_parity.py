@@ -31,6 +31,14 @@ CONFIGS = {
     "probe1": (500, 20, 80, 128, 4, 4, 16, 5, 64, 1, True),
     "q64": (300, 50, 120, 128, 4, 3, 64, 10, 256, 16, True),
     "q100": (300, 10, 90, 128, 4, 2, 100, 10, 256, 8, True),
+    # every (dim, nbits) at query lengths past 32, up to the 256-token limit (Qp = 256: generic K5, K1 v1, and the
+    # approximate stage with 32 lanes per S row)
+    "q129": (300, 20, 90, 128, 4, 2, 129, 10, 256, 8, True),
+    "q256": (300, 20, 90, 128, 4, 2, 256, 10, 256, 8, True),
+    "nbits2_q100": (300, 20, 80, 128, 2, 2, 100, 10, 256, 8, True),
+    "dim64_q64": (300, 20, 80, 64, 4, 3, 64, 10, 256, 8, True),
+    "dim64_nbits2": (400, 20, 80, 64, 2, 3, 32, 10, 256, 8, True),
+    "dim64_nbits2_q256": (300, 20, 80, 64, 2, 2, 256, 10, 256, 8, True),
 }
 
 _cache: dict = {}
