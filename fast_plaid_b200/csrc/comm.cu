@@ -62,12 +62,6 @@ NcclApi& nccl() {
     }                                                                                          \
   } while (0)
 
-#define FPB_TRY(expr)              \
-  do {                             \
-    const int _rc = (expr);        \
-    if (_rc != FPB_OK) return _rc; \
-  } while (0)
-
 }  // namespace
 
 struct fpb_comm {
@@ -216,7 +210,7 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
     FPB_TRY(launch_probe(ix, ws, false, st));
     FPB_TRY(launch_candidates(ix, ws, false, st));
     FPB_TRY(launch_approx(ix, ws, L.flags, st));
-    FPB_TRY(launch_select(ix, ws, st));
+    FPB_TRY(launch_select(ws, st));
     FPB_TRY(launch_emit_keys(ix, ws, keys, st));
   }
   FPB_NCCL_CHECK(nccl().AllGather(keys, all_keys, size_t(per_rank) * 8, ncclUint8, comm->comm, st));

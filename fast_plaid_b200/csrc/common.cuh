@@ -76,6 +76,13 @@ void fpb_set_error(const char* fmt, ...);
     }                                                                                     \
   } while (0)
 
+// evaluate an FPB_* status expression; return its status from the caller unless it is FPB_OK
+#define FPB_TRY(expr)              \
+  do {                             \
+    const int _rc = (expr);        \
+    if (_rc != FPB_OK) return _rc; \
+  } while (0)
+
 static inline int64_t fpb_align256(int64_t x) { return (x + 255) & ~int64_t(255); }
 // Words of a query's K-bit map of high centroids (two-pass approximate stage): a multiple of 4, so that the map is
 // uint4-copyable.  The bound pass keeps 32 zero words after it in shared memory, one per bank.

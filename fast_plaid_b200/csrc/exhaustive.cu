@@ -1,8 +1,6 @@
 // Exhaustive exact search behind the C ABI: K7 scores every document of the index against every query, then
-// the approximate pipeline's own selection (k3b_select) and ranking (k6_rank) turn the [B, N] score array into
-// the top_k.  Works on every index, including compress_only ones (no IVF is read).
-#include <string.h>
-
+// the approximate pipeline's own selection (k3b_select, with every document a candidate) and ranking (k6_rank)
+// turn the [B, N] score array into the top_k.  Works on every index, including compress_only ones (no IVF is read).
 #include "kernels.h"
 
 namespace {
@@ -46,8 +44,6 @@ int exhaustive_layout(const fpb_index* ix, int B, int Q, int top_k, ExLayout* X)
   X->off_counter = take(4);
   const bool sel = top_k > 0;
   X->off_scores = take(sel ? int64_t(B) * cap * 4 : 0);
-  X->off_cand = take(sel ? int64_t(B) * cap * 4 : 0);
-  X->off_n_cand = take(sel ? int64_t(B) * 4 : 0);
   X->off_n_rerank = take(sel ? int64_t(B) * 4 : 0);
   X->off_rerank = take(sel ? int64_t(B) * top_k * 4 : 0);
   X->off_rerank_approx = take(sel ? int64_t(B) * top_k * 4 : 0);
@@ -70,21 +66,6 @@ int check_workspace(const ExLayout& X, void* d_ws, size_t ws_bytes) {
   }
   return FPB_OK;
 }
-
-// every document is a candidate of every query: cand[b, i] = i, n_cand[b] = N
-__global__ void ex_candidates_kernel(int32_t* __restrict__ cand, int32_t* __restrict__ n_cand, int B, int64_t N) {
-  const int64_t total = int64_t(B) * N;
-  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x)
-    cand[i] = int32_t(i % N);
-  for (int64_t b = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; b < B; b += int64_t(gridDim.x) * blockDim.x)
-    n_cand[b] = int32_t(N);
-}
-
-#define FPB_TRY(expr)              \
-  do {                             \
-    const int _rc = (expr);        \
-    if (_rc != FPB_OK) return _rc; \
-  } while (0)
 
 }  // namespace
 
@@ -138,31 +119,15 @@ extern "C" int fpb_search_exhaustive(const fpb_index* ix, const void* d_queries,
   FPB_CUDA_CHECK(cudaSetDevice(ix->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   char* base = static_cast<char*>(d_ws);
-  FPB_TRY(launch_exhaustive_scores(ix, X, base, static_cast<const __half*>(d_queries),
-                                   reinterpret_cast<float*>(base + X.off_scores), st));
-  // the selection stages see every document as a candidate whose "approximate" score is its exact one; the
-  // re-rank list they keep then holds exact scores already, so off_exact aliases off_rerank_approx
-  fpb_layout L;
-  memset(&L, 0, sizeof(L));
-  L.B = B;
-  L.Q = Q;
-  L.R = top_k;
-  L.cand_cap = int(ix->N > 0 ? ix->N : 1);
-  L.off_approx = X.off_scores;
-  L.off_cand = X.off_cand;
-  L.off_n_cand = X.off_n_cand;
-  L.off_n_rerank = X.off_n_rerank;
-  L.off_rerank = X.off_rerank;
-  L.off_rerank_approx = X.off_rerank_approx;
-  L.off_exact = X.off_rerank_approx;
-  L.total_bytes = X.total_bytes;
-  Ws ws{&L, base};
-  const int64_t total = int64_t(B) * ix->N;
-  const int64_t want = ((total > B ? total : int64_t(B)) + 255) / 256;
-  const int blocks = int(want < int64_t(ix->sm_count) * 16 ? want : int64_t(ix->sm_count) * 16);
-  ex_candidates_kernel<<<blocks, 256, 0, st>>>(ws.cand(), ws.n_cand(), B, ix->N);
-  FPB_LAUNCH_CHECK("ex_candidates");
-  FPB_TRY(launch_select(ix, ws, st));
-  FPB_TRY(launch_rank(ix, ws, top_k, d_out_ids, d_out_scores, d_out_counts, st));
+  float* scores = reinterpret_cast<float*>(base + X.off_scores);
+  int32_t* n_sel = reinterpret_cast<int32_t*>(base + X.off_n_rerank);
+  int32_t* sel_ids = reinterpret_cast<int32_t*>(base + X.off_rerank);
+  float* sel_scores = reinterpret_cast<float*>(base + X.off_rerank_approx);
+  FPB_TRY(launch_exhaustive_scores(ix, X, base, static_cast<const __half*>(d_queries), scores, st));
+  // every document is a candidate, and its "approximate" score is its exact one: the selected list holds the exact
+  // scores that k6_rank orders
+  FPB_TRY(launch_select(scores, nullptr, nullptr, int(ix->N), B, top_k, sel_ids, sel_scores, n_sel, st));
+  FPB_TRY(launch_rank(sel_scores, sel_ids, n_sel, top_k, B, top_k, ix->doc_id_base, d_out_ids, d_out_scores,
+                      d_out_counts, st));
   return FPB_OK;
 }

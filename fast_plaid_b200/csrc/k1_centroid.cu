@@ -11,6 +11,7 @@
 #include <stdlib.h>
 
 #include "kernels.h"
+#include "select.cuh"
 
 namespace {
 
@@ -179,10 +180,10 @@ k1b_probe_kernel(const __half* __restrict__ S, const __half* __restrict__ tmax, 
   for (int base = 0; base < n_tiles; base += 32) {
     const int tix = base + lane;
     uint64_t key = 0;
-    if (tix < n_tiles) key = (uint64_t(f16_key(tm[tix])) << 32) | uint64_t(0xffffffffu - uint32_t(tix));
+    if (tix < n_tiles) key = rank_key_f16(tm[tix], uint32_t(tix));
     topn_offer(mine, n_probe, key, lane);
   }
-  const uint32_t tau = uint32_t(shfl64(mine, n_probe - 1) >> 32);  // 0 when fewer than n tiles
+  const uint32_t tau = rank_key_vkey(shfl64(mine, n_probe - 1));  // 0 when fewer than n tiles
 
   // pass 2: exact top-n over the rows of the qualifying tiles
   mine = 0;
@@ -202,7 +203,7 @@ k1b_probe_kernel(const __half* __restrict__ S, const __half* __restrict__ tmax, 
         uint64_t key = 0;
         if (row < K) {
           const uint32_t k16 = f16_key(Sb[int64_t(row) * Qp]);
-          if (k16 >= tau) key = (uint64_t(k16) << 32) | uint64_t(0xffffffffu - uint32_t(row));
+          if (k16 >= tau) key = rank_key(k16, uint32_t(row));
         }
         topn_offer(mine, n_probe, key, lane);
       }
@@ -210,7 +211,7 @@ k1b_probe_kernel(const __half* __restrict__ S, const __half* __restrict__ tmax, 
   }
   if (lane < n_probe) {
     int32_t c = -1;
-    if (mine != 0) c = int32_t(0xffffffffu - uint32_t(mine));
+    if (mine != 0) c = int32_t(rank_key_id(mine));
     cells[(int64_t(b) * Q + q) * n_probe + lane] = c;
   }
 }
@@ -236,14 +237,14 @@ k1b_probe_subset_kernel(const __half* __restrict__ S, int K, int B, int Q, int Q
       uint64_t key = 0;
       if (i < nc) {
         const int c = cl[i];
-        key = (uint64_t(f16_key(Sb[int64_t(c) * Qp])) << 32) | uint64_t(0xffffffffu - uint32_t(c));
+        key = rank_key_f16(Sb[int64_t(c) * Qp], uint32_t(c));
       }
       topn_offer(mine, n, key, lane);
     }
   }
   if (lane < n_probe) {
     int32_t c = -1;
-    if (lane < n && mine != 0) c = int32_t(0xffffffffu - uint32_t(mine));
+    if (lane < n && mine != 0) c = int32_t(rank_key_id(mine));
     cells[(int64_t(b) * Q + q) * n_probe + lane] = c;
   }
 }

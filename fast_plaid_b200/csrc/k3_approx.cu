@@ -1,6 +1,5 @@
 // K3  : approximate (centroid-only) document scores                       (search.rs:554-592)
 //         approx[d] = sum_{q<Q}^{fp32}  max_{t<len(d)}  S[b][code[d,t]][q]     (fp16 max)
-// K3b : pruning to the n_full_scores/4 best candidates                     (search.rs:602-619)
 //
 // The reference gathers S rows into a [tokens, Q] tensor, pads it to [2000, maxlen, Q], masks, maxes and
 // sums, 128 times per query with two host syncs each.  A one-pass GPU formulation (one warp walks one
@@ -26,6 +25,7 @@
 #include <stdlib.h>
 
 #include "kernels.h"
+#include "select.cuh"
 
 namespace {
 
@@ -783,32 +783,11 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
 
 // step 4: per query the pruning threshold T (at least n_dec candidates have lb >= T; found with two levels of
 // 2048 value buckets, so outliers only cost resolution) and the list of unresolved candidates with ub >= T.
-// warp 0: bucket t with count(bucket > t) < need <= count(bucket >= t) over a 2048-bin histogram
-__device__ __forceinline__ void k3_find_bucket(const int* hist, int need, int lane, int* s_t, int* s_need) {
-  int mine = 0;
-  for (int k = 0; k < 64; ++k) mine += hist[lane * 64 + k];
-  int above = 0;
-  for (int l = 31; l >= 0; --l) {
-    const int c = __shfl_sync(0xffffffffu, mine, l);
-    if (l > lane) above += c;
-  }
-  if (above < need && above + mine >= need) {
-    int cum = above, d = lane * 64 + 63;
-    for (; d > lane * 64; --d) {
-      const int h = hist[d];
-      if (cum + h >= need) break;
-      cum += h;
-    }
-    *s_t = d;
-    *s_need = need - cum;  // still to take from bucket d
-  }
-}
-
 __global__ void __launch_bounds__(1024)
 k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb, int cand_cap,
                       const int32_t* __restrict__ n_cand, int n_dec, int refine_all, int32_t* __restrict__ list,
                       int32_t* __restrict__ n_list, float* __restrict__ thresh) {
-  __shared__ int hist[2048];
+  __shared__ int hist[SEL_BINS];
   __shared__ float s_red[64];
   __shared__ int s_t, s_need, s_cnt;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
@@ -830,29 +809,12 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
         mx = fmaxf(mx, v[u]);
       }
     }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, off));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-    }
-    if (lane == 0) {
-      s_red[tid >> 5] = mn;
-      s_red[32 + (tid >> 5)] = mx;
-    }
-    __syncthreads();
-    mn = s_red[lane];
-    mx = s_red[32 + lane];
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, off));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-    }
+    block_min_max(mn, mx, s_red);
     const float range = mx - mn;
     if (range > 0.f && range < 3.0e38f) {
-      // level 1: 2048 buckets over [mn, mx]; bucket() is monotone in v
-      const float scale1 = 2047.0f / range;
-      auto bucket1 = [&](float v) { return min(2047, max(0, __float2int_rz((v - mn) * scale1))); };
-      for (int i = tid; i < 2048; i += 1024) hist[i] = 0;
+      // level 1: 2048 buckets over [mn, mx]
+      const float scale1 = float(SEL_BINS - 1) / range;
+      for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
       __syncthreads();
       for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
         float v[FV];
@@ -860,20 +822,19 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
         for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? lbb[i0 + u * 1024] : 0.f;
 #pragma unroll
         for (int u = 0; u < FV; ++u)
-          if (i0 + u * 1024 < n && v[u] == v[u]) atomicAdd(&hist[bucket1(v[u])], 1);
+          if (i0 + u * 1024 < n && v[u] == v[u]) atomicAdd(&hist[value_bucket(v[u], mn, scale1)], 1);
       }
       if (tid == 0) s_t = -1;
       __syncthreads();
-      if (tid < 32) k3_find_bucket(hist, n_dec, lane, &s_t, &s_need);
+      if (tid < 32) warp_find_bucket(hist, SEL_BINS, n_dec, &s_t, &s_need);
       __syncthreads();
       const int t1 = s_t, need1 = s_need;
       __syncthreads();
       if (t1 >= 0) {  // (t1 < 0 only if NaNs leave fewer than n_dec comparable values: T stays -inf)
         // level 2: 2048 buckets inside bucket t1
         const float lo1 = mn + float(t1) / scale1;
-        const float scale2 = 2047.0f * scale1;
-        auto bucket2 = [&](float v) { return min(2047, max(0, __float2int_rz((v - lo1) * scale2))); };
-        for (int i = tid; i < 2048; i += 1024) hist[i] = 0;
+        const float scale2 = float(SEL_BINS - 1) * scale1;
+        for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
         __syncthreads();
         for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
           float v[FV];
@@ -881,11 +842,12 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
           for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? lbb[i0 + u * 1024] : 0.f;
 #pragma unroll
           for (int u = 0; u < FV; ++u)
-            if (i0 + u * 1024 < n && v[u] == v[u] && bucket1(v[u]) == t1) atomicAdd(&hist[bucket2(v[u])], 1);
+            if (i0 + u * 1024 < n && v[u] == v[u] && value_bucket(v[u], mn, scale1) == t1)
+              atomicAdd(&hist[value_bucket(v[u], lo1, scale2)], 1);
         }
         if (tid == 0) s_t = -1;
         __syncthreads();
-        if (tid < 32) k3_find_bucket(hist, need1, lane, &s_t, &s_need);
+        if (tid < 32) warp_find_bucket(hist, SEL_BINS, need1, &s_t, &s_need);
         __syncthreads();
         const int t2 = s_t;
         // T = the smallest value of the selected upper set {b1 > t1} u {b1 == t1, b2 >= t2}: it holds >= n_dec values
@@ -898,8 +860,8 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
 #pragma unroll
             for (int u = 0; u < FV; ++u) {
               if (v[u] == v[u]) {
-                const int b1 = bucket1(v[u]);
-                if (b1 > t1 || (b1 == t1 && bucket2(v[u]) >= t2)) tmin = fminf(tmin, v[u]);
+                const int b1 = value_bucket(v[u], mn, scale1);
+                if (b1 > t1 || (b1 == t1 && value_bucket(v[u], lo1, scale2) >= t2)) tmin = fminf(tmin, v[u]);
               }
             }
           }
@@ -938,295 +900,6 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
     n_list[b] = s_cnt;
     thresh[b] = T;
   }
-}
-
-// ---------------------------------------------------------------------------------------
-// K3b: top-n_dec by (approx desc, candidate index asc) -- candidate index order is doc id
-// order, so this is the canonical rule "larger score, then smaller doc id".  Equivalent to
-// the reference's topk(n_full) followed by topk(n_full/4) up to tie order.
-// ---------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t approx_key(float a, uint32_t i) {
-  return (uint64_t(f32_key(a)) << 32) | uint64_t(0xffffffffu - i);
-}
-
-// Digits of the 64-bit key, most significant first: 11+11+10 bits cover the score, the rest
-// only matters when scores tie at the threshold.
-__constant__ int K3B_LO[6] = {53, 42, 32, 21, 10, 0};
-__constant__ int K3B_W[6] = {11, 11, 10, 11, 11, 10};
-constexpr int K3B_VPT = 4;  // independent loads in flight per thread
-constexpr int K3B_BCAP = 2048;  // capacity of the threshold bucket on the fast path
-
-__global__ void __launch_bounds__(1024)
-k3b_select_kernel(const float* __restrict__ approx, const int32_t* __restrict__ cand, int cand_cap,
-                  const int32_t* __restrict__ n_cand, int n_dec, int Rp2, int32_t* __restrict__ rerank,
-                  float* __restrict__ rerank_approx, int32_t* __restrict__ n_rerank) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);
-  __shared__ int hist[2048];
-  __shared__ int s_need, s_hd, s_cnt;
-  __shared__ uint64_t s_prefix, s_mask;
-  __shared__ uint64_t bkeys[K3B_BCAP];  // fast path: keys of the threshold bucket
-  __shared__ float s_red[64];
-  __shared__ int s_cnt2, s_fast;
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
-  const int n = n_cand[b];
-  const float* ab = approx + int64_t(b) * cand_cap;
-  const int32_t* cb = cand + int64_t(b) * cand_cap;
-  int32_t* rr = rerank + int64_t(b) * n_dec;
-  float* ra = rerank_approx + int64_t(b) * n_dec;
-  if (n <= n_dec) {  // search.rs:605 / :615 conditions false: nothing is pruned
-    for (int i = tid; i < n; i += 1024) {
-      rr[i] = cb[i];
-      ra[i] = ab[i];
-    }
-    if (tid == 0) n_rerank[b] = n;
-    return;
-  }
-  // ---- fast path: 2048 buckets over the VALUE range [min, max] of this query's scores ----
-  // The radix passes below start from the top bits of the float key, where the scores of one query share
-  // sign, exponent and the leading mantissa bits: a handful of hot bins, so every element pays a ballot +
-  // match_any + contended shared atomic, three passes long (0.49 ms on cfg-3).  A linear bucketisation of the
-  // actual value range spreads the scores, one histogram pass isolates the threshold bucket, and only that
-  // bucket (typically n / 2048 elements) is ordered by the exact 64-bit key.  bucket(v) is monotone in v, so
-  // every element of a higher bucket is strictly larger: the selection is exactly the same.
-  {
-    constexpr int FV = 8;  // independent loads in flight per thread
-    float mn = INFINITY, mx = -INFINITY;
-    for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
-      float v[FV];
-#pragma unroll
-      for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : NAN;  // fmin/fmax skip NaN
-#pragma unroll
-      for (int u = 0; u < FV; ++u) {
-        mn = fminf(mn, v[u]);
-        mx = fmaxf(mx, v[u]);
-      }
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, off));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-    }
-    if (lane == 0) {
-      s_red[tid >> 5] = mn;
-      s_red[32 + (tid >> 5)] = mx;
-    }
-    for (int i = tid; i < 2048; i += 1024) hist[i] = 0;
-    if (tid == 0) {
-      s_cnt = 0;
-      s_cnt2 = 0;
-      s_fast = 0;
-    }
-    __syncthreads();
-    mn = s_red[lane];
-    mx = s_red[32 + lane];
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-      mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, off));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-    }
-    const float range = mx - mn;
-    // finite, non-degenerate range (NaN / inf scores or all-equal scores take the radix path)
-    const bool usable = range > 0.f && range < 3.0e38f;
-    const float scale = usable ? 2047.0f / range : 0.f;
-    auto bucket = [&](float v) { return min(2047, max(0, __float2int_rz((v - mn) * scale))); };
-    if (usable) {
-      for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
-        float v[FV];
-#pragma unroll
-        for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : 0.f;
-#pragma unroll
-        for (int u = 0; u < FV; ++u)
-          if (i0 + u * 1024 < n) atomicAdd(&hist[bucket(v[u])], 1);
-      }
-      __syncthreads();
-      if (tid < 32) {
-        // warp 0: bucket t with  count(bucket > t) < n_dec <= count(bucket >= t)
-        int mine = 0;
-        for (int k = 0; k < 64; ++k) mine += hist[lane * 64 + k];
-        int above = 0;
-        for (int l = 31; l >= 0; --l) {
-          const int c = __shfl_sync(0xffffffffu, mine, l);
-          if (l > lane) above += c;
-        }
-        if (above < n_dec && above + mine >= n_dec) {
-          int cum = above, d = lane * 64 + 63;
-          for (; d > lane * 64; --d) {
-            const int h = hist[d];
-            if (cum + h >= n_dec) break;
-            cum += h;
-          }
-          s_need = n_dec - cum;  // still to take from bucket d
-          s_hd = d;
-          s_fast = hist[d] <= K3B_BCAP ? 1 : 0;
-        }
-      }
-      __syncthreads();
-      if (s_fast) {
-        const int t = s_hd;
-        for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
-          float v[FV];
-#pragma unroll
-          for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : 0.f;
-#pragma unroll
-          for (int u = 0; u < FV; ++u) {
-            const int i = i0 + u * 1024;
-            if (i < n) {
-              const int bk = bucket(v[u]);
-              if (bk > t) {
-                keys[atomicAdd(&s_cnt, 1)] = approx_key(v[u], uint32_t(i));    // fewer than n_dec of these
-              } else if (bk == t) {
-                bkeys[atomicAdd(&s_cnt2, 1)] = approx_key(v[u], uint32_t(i));  // at most K3B_BCAP of these
-              }
-            }
-          }
-        }
-        __syncthreads();
-        const int c2 = s_cnt2, need2 = s_need;
-        for (int i = c2 + tid; i < K3B_BCAP; i += 1024) bkeys[i] = 0ull;
-        __syncthreads();
-        for (int k = 2; k <= K3B_BCAP; k <<= 1) {  // bitonic sort, descending
-          for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = tid; i < K3B_BCAP; i += 1024) {
-              const int ixj = i ^ j;
-              if (ixj > i) {
-                const bool up = (i & k) == 0;
-                const uint64_t x = bkeys[i], y = bkeys[ixj];
-                if ((x < y) == up) {
-                  bkeys[i] = y;
-                  bkeys[ixj] = x;
-                }
-              }
-            }
-            __syncthreads();
-          }
-        }
-        const int c1 = s_cnt;
-        for (int i = tid; i < need2; i += 1024) keys[c1 + i] = bkeys[i];
-        __syncthreads();
-        if (tid == 0) s_cnt = c1 + need2;  // == n_dec
-        __syncthreads();
-      }
-    }
-  }
-  const bool fast_done = s_fast != 0;
-  if (!fast_done) {
-  if (tid == 0) {
-    s_need = n_dec;
-    s_prefix = 0;
-    s_mask = 0;
-  }
-  }
-  const int stride = 1024 * K3B_VPT;
-  const int n_up = (n + stride - 1) / stride * stride;
-  if (!fast_done) {
-  for (int pass = 0; pass < 6; ++pass) {
-    const int lo = K3B_LO[pass], width = K3B_W[pass];
-    const uint64_t dmask = (1ull << width) - 1ull;
-    for (int i = tid; i < 2048; i += 1024) hist[i] = 0;
-    __syncthreads();
-    const uint64_t prefix = s_prefix, mask = s_mask;
-    for (int i0 = tid; i0 < n_up; i0 += stride) {
-      float v[K3B_VPT];
-#pragma unroll
-      for (int u = 0; u < K3B_VPT; ++u) {
-        const int i = i0 + u * 1024;
-        v[u] = (i < n) ? ab[i] : 0.f;
-      }
-#pragma unroll
-      for (int u = 0; u < K3B_VPT; ++u) {
-        const int i = i0 + u * 1024;
-        const bool valid = i < n;
-        const uint64_t key = valid ? approx_key(v[u], uint32_t(i)) : 0ull;
-        const bool in = valid && ((key & mask) == prefix);
-        const unsigned act = __ballot_sync(0xffffffffu, in);
-        if (in) {
-          const int bin = int((key >> lo) & dmask);
-          const unsigned peers = __match_any_sync(act, bin);
-          if (lane == __ffs(peers) - 1) atomicAdd(&hist[bin], __popc(peers));
-        }
-      }
-    }
-    __syncthreads();
-    if (tid < 32) {
-      // warp 0: find the digit d with  count(digit > d) < need <= count(digit >= d)
-      const int nbins = 1 << width;
-      const int per = nbins / 32;  // bins per lane, lane 31 owns the top bins
-      int mine = 0;
-      for (int k = 0; k < per; ++k) mine += hist[lane * per + k];
-      // suffix sums over lanes (lanes above me)
-      int above = 0;
-      for (int l = 31; l >= 0; --l) {
-        const int c = __shfl_sync(0xffffffffu, mine, l);
-        if (l > lane) above += c;
-      }
-      const int need = s_need;
-      const bool here = (above < need) && (above + mine >= need);
-      if (here) {
-        int cum = above, d = lane * per + per - 1;
-        for (; d > lane * per; --d) {
-          const int h = hist[d];
-          if (cum + h >= need) break;
-          cum += h;
-        }
-        s_need = need - cum;
-        s_hd = hist[d];
-        s_prefix = prefix | (uint64_t(d) << lo);
-        s_mask = mask | (dmask << lo);
-      }
-    }
-    __syncthreads();
-    if (s_hd == s_need) break;  // the whole bucket is selected
-  }
-  const uint64_t T = s_prefix;  // unprocessed low bits are zero
-  if (tid == 0) s_cnt = 0;
-  __syncthreads();
-  for (int i0 = tid; i0 < n_up; i0 += stride) {
-    float v[K3B_VPT];
-#pragma unroll
-    for (int u = 0; u < K3B_VPT; ++u) {
-      const int i = i0 + u * 1024;
-      v[u] = (i < n) ? ab[i] : 0.f;
-    }
-#pragma unroll
-    for (int u = 0; u < K3B_VPT; ++u) {
-      const int i = i0 + u * 1024;
-      if (i < n) {
-        const uint64_t key = approx_key(v[u], uint32_t(i));
-        if (key >= T) {
-          const int pos = atomicAdd(&s_cnt, 1);
-          if (pos < Rp2) keys[pos] = key;
-        }
-      }
-    }
-  }
-  }  // radix path
-  __syncthreads();
-  const int cnt = min(s_cnt, Rp2);
-  for (int i = cnt + tid; i < Rp2; i += 1024) keys[i] = 0ull;
-  __syncthreads();
-  for (int k = 2; k <= Rp2; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < Rp2; i += 1024) {
-        const int ixj = i ^ j;
-        if (ixj > i) {
-          const bool up = (i & k) == 0;
-          const uint64_t x = keys[i], y = keys[ixj];
-          if ((x < y) == up) {
-            keys[i] = y;
-            keys[ixj] = x;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  }
-  for (int r = tid; r < n_dec; r += 1024) {
-    const uint32_t idx = 0xffffffffu - uint32_t(keys[r]);
-    rr[r] = cb[idx];
-    ra[r] = ab[idx];
-  }
-  if (tid == 0) n_rerank[b] = n_dec;
 }
 
 // exact scoring of `list` (NULL: every candidate) into approx
@@ -1351,19 +1024,5 @@ int launch_walk_layout(const fpb_index* ix, cudaStream_t st) {
   k3_walk_layout_kernel<<<blocks, K3_WALK_THREADS, 0, st>>>(ix->doc_offsets, ix->doc_codes, ix->walk_win, ix->N,
                                                             fpb_hb_words(ix->K), ix->walk_codes);
   FPB_LAUNCH_CHECK("k3_walk_layout");
-  return FPB_OK;
-}
-
-int launch_select(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
-  (void)ix;
-  const fpb_layout& L = *ws.L;
-  const int Rp2 = fpb_next_pow2(L.R);
-  // dynamic keys[] (8 B x Rp2, 32 KB at the maximum R = 4096) on top of 25 KB of static shared memory: opt in
-  // (per device: cudaFuncSetAttribute applies to the current device only, and the call is cheap)
-  FPB_CUDA_CHECK(cudaFuncSetAttribute(k3b_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Rp2 * 8));
-  k3b_select_kernel<<<L.B, 1024, size_t(Rp2) * 8, st>>>(ws.approx(), ws.cand(), L.cand_cap, ws.n_cand(),
-                                                       L.R, Rp2, ws.rerank(), ws.rerank_approx(),
-                                                       ws.n_rerank());
-  FPB_LAUNCH_CHECK("k3b_select");
   return FPB_OK;
 }

@@ -1,53 +1,218 @@
-// K6 : final ranking (search.rs:659-666) and the document-sharded merge (new, SURVEY.md 8e).
+// Everything that orders documents by the canonical key (select.cuh): K3b, the pruning to the n_full_scores/4 best
+// candidates (search.rs:602-619); K6, the final ranking (search.rs:659-666); and the document-sharded merge and
+// threshold (new, SURVEY.md 8e).
 //
-// Canonical order: larger exact score first, then smaller doc id.  (The reference's
-// non-stable sort(descending) leaves equal scores in an implementation-defined order.)
+// Canonical order: larger score first, then smaller doc id.  (The reference's non-stable sort(descending) leaves
+// equal scores in an implementation-defined order.)
 #include "kernels.h"
+#include "select.cuh"
 
 namespace {
 
-__device__ __forceinline__ void bitonic_desc(uint64_t* keys, int P, int tid, int nthreads) {
-  for (int k = 2; k <= P; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < P; i += nthreads) {
-        const int ixj = i ^ j;
-        if (ixj > i) {
-          const bool up = (i & k) == 0;
-          const uint64_t x = keys[i], y = keys[ixj];
-          if ((x < y) == up) {
-            keys[i] = y;
-            keys[ixj] = x;
+// ---------------------------------------------------------------------------------------
+// K3b: top-n_dec by (score desc, candidate index asc) -- candidate index order is doc id
+// order, so this is the canonical rule "larger score, then smaller doc id".  Equivalent to
+// the reference's topk(n_full) followed by topk(n_full/4) up to tie order.
+// ---------------------------------------------------------------------------------------
+
+// Digits of the 64-bit key, most significant first: 11+11+10 bits cover the score, the rest
+// only matters when scores tie at the threshold.
+__constant__ int K3B_LO[6] = {53, 42, 32, 21, 10, 0};
+__constant__ int K3B_W[6] = {11, 11, 10, 11, 11, 10};
+constexpr int K3B_VPT = 4;  // independent loads in flight per thread
+constexpr int K3B_BCAP = 2048;  // capacity of the threshold bucket on the fast path
+
+// Row b of `approx` (stride cand_cap) holds the scores of n_cand[b] candidates, candidate i being document
+// cand[b, i].  cand == NULL: all cand_cap entries of the row are candidates, candidate i being document i.
+__global__ void __launch_bounds__(1024)
+k3b_select_kernel(const float* __restrict__ approx, const int32_t* __restrict__ cand, int cand_cap,
+                  const int32_t* __restrict__ n_cand, int n_dec, int Rp2, int32_t* __restrict__ rerank,
+                  float* __restrict__ rerank_approx, int32_t* __restrict__ n_rerank) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);
+  __shared__ int hist[SEL_BINS];
+  __shared__ int s_need, s_hd, s_cnt;
+  __shared__ uint64_t s_prefix, s_mask;
+  __shared__ uint64_t bkeys[K3B_BCAP];  // fast path: keys of the threshold bucket
+  __shared__ float s_red[64];
+  __shared__ int s_cnt2, s_fast;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+  const int n = cand ? n_cand[b] : cand_cap;
+  const float* ab = approx + int64_t(b) * cand_cap;
+  const int32_t* cb = cand ? cand + int64_t(b) * cand_cap : nullptr;
+  int32_t* rr = rerank + int64_t(b) * n_dec;
+  float* ra = rerank_approx + int64_t(b) * n_dec;
+  if (n <= n_dec) {  // search.rs:605 / :615 conditions false: nothing is pruned
+    for (int i = tid; i < n; i += 1024) {
+      rr[i] = cb ? cb[i] : i;
+      ra[i] = ab[i];
+    }
+    if (tid == 0) n_rerank[b] = n;
+    return;
+  }
+  // ---- fast path: 2048 buckets over the VALUE range [min, max] of this query's scores ----
+  // The radix passes below start from the top bits of the float key, where the scores of one query share
+  // sign, exponent and the leading mantissa bits: a handful of hot bins, so every element pays a ballot +
+  // match_any + contended shared atomic, three passes long (0.49 ms on cfg-3).  A linear bucketisation of the
+  // actual value range spreads the scores, one histogram pass isolates the threshold bucket, and only that
+  // bucket (typically n / 2048 elements) is ordered by the exact 64-bit key.  value_bucket() is monotone, so
+  // every element of a higher bucket is strictly larger: the selection is exactly the same.
+  {
+    constexpr int FV = 8;  // independent loads in flight per thread
+    float mn = INFINITY, mx = -INFINITY;
+    for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
+      float v[FV];
+#pragma unroll
+      for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : NAN;  // fmin/fmax skip NaN
+#pragma unroll
+      for (int u = 0; u < FV; ++u) {
+        mn = fminf(mn, v[u]);
+        mx = fmaxf(mx, v[u]);
+      }
+    }
+    for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
+    if (tid == 0) {
+      s_cnt = 0;
+      s_cnt2 = 0;
+      s_fast = 0;
+    }
+    block_min_max(mn, mx, s_red);
+    const float range = mx - mn;
+    // finite, non-degenerate range (NaN / inf scores or all-equal scores take the radix path)
+    const bool usable = range > 0.f && range < 3.0e38f;
+    const float scale = usable ? float(SEL_BINS - 1) / range : 0.f;
+    if (usable) {
+      for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
+        float v[FV];
+#pragma unroll
+        for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : 0.f;
+#pragma unroll
+        for (int u = 0; u < FV; ++u)
+          if (i0 + u * 1024 < n) atomicAdd(&hist[value_bucket(v[u], mn, scale)], 1);
+      }
+      __syncthreads();
+      int hd, rest;
+      if (tid < 32 && warp_find_bucket(hist, SEL_BINS, n_dec, &hd, &rest)) {
+        s_need = rest;
+        s_hd = hd;
+        s_fast = hist[hd] <= K3B_BCAP ? 1 : 0;
+      }
+      __syncthreads();
+      if (s_fast) {
+        const int t = s_hd;
+        for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
+          float v[FV];
+#pragma unroll
+          for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : 0.f;
+#pragma unroll
+          for (int u = 0; u < FV; ++u) {
+            const int i = i0 + u * 1024;
+            if (i < n) {
+              const int bk = value_bucket(v[u], mn, scale);
+              if (bk > t) {
+                keys[atomicAdd(&s_cnt, 1)] = rank_key_f32(v[u], uint32_t(i));    // fewer than n_dec of these
+              } else if (bk == t) {
+                bkeys[atomicAdd(&s_cnt2, 1)] = rank_key_f32(v[u], uint32_t(i));  // at most K3B_BCAP of these
+              }
+            }
+          }
+        }
+        __syncthreads();
+        const int c2 = s_cnt2, need2 = s_need;
+        for (int i = c2 + tid; i < K3B_BCAP; i += 1024) bkeys[i] = 0ull;
+        __syncthreads();
+        block_sort_desc(bkeys, K3B_BCAP);
+        const int c1 = s_cnt;
+        for (int i = tid; i < need2; i += 1024) keys[c1 + i] = bkeys[i];
+        __syncthreads();
+        if (tid == 0) s_cnt = c1 + need2;  // == n_dec
+        __syncthreads();
+      }
+    }
+  }
+  if (!s_fast) {  // ---- radix passes over the 64-bit key: the threshold key T, then every key >= T ----
+    if (tid == 0) {
+      s_need = n_dec;
+      s_prefix = 0;
+      s_mask = 0;
+    }
+    const int stride = 1024 * K3B_VPT;
+    const int n_up = (n + stride - 1) / stride * stride;
+    for (int pass = 0; pass < 6; ++pass) {
+      const int lo = K3B_LO[pass], width = K3B_W[pass];
+      const uint64_t dmask = (1ull << width) - 1ull;
+      for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
+      __syncthreads();
+      const uint64_t prefix = s_prefix, mask = s_mask;
+      for (int i0 = tid; i0 < n_up; i0 += stride) {
+        float v[K3B_VPT];
+#pragma unroll
+        for (int u = 0; u < K3B_VPT; ++u) {
+          const int i = i0 + u * 1024;
+          v[u] = (i < n) ? ab[i] : 0.f;
+        }
+#pragma unroll
+        for (int u = 0; u < K3B_VPT; ++u) {
+          const int i = i0 + u * 1024;
+          const bool valid = i < n;
+          const uint64_t key = valid ? rank_key_f32(v[u], uint32_t(i)) : 0ull;
+          const bool in = valid && ((key & mask) == prefix);
+          const unsigned act = __ballot_sync(0xffffffffu, in);
+          if (in) {
+            const int bin = int((key >> lo) & dmask);
+            const unsigned peers = __match_any_sync(act, bin);
+            if (lane == __ffs(peers) - 1) atomicAdd(&hist[bin], __popc(peers));
           }
         }
       }
       __syncthreads();
+      int d, rest;
+      if (tid < 32 && warp_find_bucket(hist, 1 << width, s_need, &d, &rest)) {
+        s_need = rest;
+        s_hd = hist[d];
+        s_prefix = prefix | (uint64_t(d) << lo);
+        s_mask = mask | (dmask << lo);
+      }
+      __syncthreads();
+      if (s_hd == s_need) break;  // the whole bucket is selected
     }
-  }
-}
-
-__device__ __forceinline__ void bitonic_desc_payload(uint64_t* keys, uint32_t* pay, int P, int tid, int nthreads) {
-  for (int k = 2; k <= P; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < P; i += nthreads) {
-        const int ixj = i ^ j;
-        if (ixj > i) {
-          const bool up = (i & k) == 0;
-          const uint64_t x = keys[i], y = keys[ixj];
-          if ((x < y) == up) {
-            keys[i] = y;
-            keys[ixj] = x;
-            const uint32_t px = pay[i];
-            pay[i] = pay[ixj];
-            pay[ixj] = px;
+    const uint64_t T = s_prefix;  // unprocessed low bits are zero
+    if (tid == 0) s_cnt = 0;
+    __syncthreads();
+    for (int i0 = tid; i0 < n_up; i0 += stride) {
+      float v[K3B_VPT];
+#pragma unroll
+      for (int u = 0; u < K3B_VPT; ++u) {
+        const int i = i0 + u * 1024;
+        v[u] = (i < n) ? ab[i] : 0.f;
+      }
+#pragma unroll
+      for (int u = 0; u < K3B_VPT; ++u) {
+        const int i = i0 + u * 1024;
+        if (i < n) {
+          const uint64_t key = rank_key_f32(v[u], uint32_t(i));
+          if (key >= T) {
+            const int pos = atomicAdd(&s_cnt, 1);
+            if (pos < Rp2) keys[pos] = key;
           }
         }
       }
-      __syncthreads();
     }
   }
+  __syncthreads();
+  const int cnt = min(s_cnt, Rp2);
+  for (int i = cnt + tid; i < Rp2; i += 1024) keys[i] = 0ull;
+  __syncthreads();
+  block_sort_desc(keys, Rp2);
+  for (int r = tid; r < n_dec; r += 1024) {
+    const uint32_t idx = rank_key_id(keys[r]);
+    rr[r] = cb ? cb[idx] : int32_t(idx);
+    ra[r] = ab[idx];
+  }
+  if (tid == 0) n_rerank[b] = n_dec;
 }
 
-// one CTA per query
+// K6, one CTA per query: row b of exact / rerank (stride R) holds the scores and ids of n_rerank[b] documents
 __global__ void __launch_bounds__(1024)
 k6_rank_kernel(const float* __restrict__ exact, const int32_t* __restrict__ rerank,
                const int32_t* __restrict__ n_rerank, int R, int Rp2, int top_k, int64_t doc_id_base,
@@ -58,19 +223,18 @@ k6_rank_kernel(const float* __restrict__ exact, const int32_t* __restrict__ rera
   const int n = n_rerank[b];
   for (int i = tid; i < Rp2; i += 1024) {
     uint64_t k = 0;
-    if (i < n) k = (uint64_t(f32_key(exact[int64_t(b) * R + i])) << 32) |
-                   uint64_t(0xffffffffu - uint32_t(rerank[int64_t(b) * R + i]));
+    if (i < n) k = rank_key_f32(exact[int64_t(b) * R + i], uint32_t(rerank[int64_t(b) * R + i]));
     keys[i] = k;
   }
   __syncthreads();
-  bitonic_desc(keys, Rp2, tid, 1024);
+  block_sort_desc(keys, Rp2);
   const int cnt = min(top_k, n);
   for (int i = tid; i < top_k; i += 1024) {
     int64_t id = -1;
     float sc = -INFINITY;
     if (i < cnt) {
-      id = doc_id_base + int64_t(0xffffffffu - uint32_t(keys[i]));
-      sc = f32_unkey(uint32_t(keys[i] >> 32));
+      id = doc_id_base + int64_t(rank_key_id(keys[i]));
+      sc = rank_key_f32_value(keys[i]);
     }
     out_ids[int64_t(b) * top_k + i] = id;
     out_scores[int64_t(b) * top_k + i] = sc;
@@ -125,7 +289,7 @@ k6_merge_kernel(const fpb_record* __restrict__ all_groups, int n_shards, int B, 
       const int s = i / R, r = i % R;
       const fpb_record rec = all[(int64_t(s) * B + b) * R + r];
       if (rec.doc_id >= 0) {
-        k = (uint64_t(f32_key(rec.approx)) << 32) | uint64_t(0xffffffffu - uint32_t(rec.doc_id));
+        k = rank_key_f32(rec.approx, uint32_t(rec.doc_id));
         ++local_valid;
       }
     }
@@ -134,7 +298,7 @@ k6_merge_kernel(const fpb_record* __restrict__ all_groups, int n_shards, int B, 
   }
   if (local_valid) atomicAdd(&s_valid, local_valid);
   __syncthreads();
-  bitonic_desc_payload(keys, pay, P, tid, 1024);
+  block_sort_desc(keys, P, pay);
   const int keep = min(s_valid, R);
   for (int i = tid; i < Rp2; i += 1024) {
     uint64_t k2 = 0;
@@ -142,19 +306,19 @@ k6_merge_kernel(const fpb_record* __restrict__ all_groups, int n_shards, int B, 
       const int j = int(pay[i]);
       const int s = j / R, r = j % R;
       const fpb_record rec = all[(int64_t(s) * B + b) * R + r];
-      k2 = (uint64_t(f32_key(rec.exact)) << 32) | uint64_t(0xffffffffu - uint32_t(rec.doc_id));
+      k2 = rank_key_f32(rec.exact, uint32_t(rec.doc_id));
     }
     keys2[i] = k2;
   }
   __syncthreads();
-  bitonic_desc(keys2, Rp2, tid, 1024);
+  block_sort_desc(keys2, Rp2);
   const int cnt = min(top_k, keep);
   for (int i = tid; i < top_k; i += 1024) {
     int64_t id = -1;
     float sc = -INFINITY;
     if (i < cnt) {
-      id = int64_t(0xffffffffu - uint32_t(keys2[i]));
-      sc = f32_unkey(uint32_t(keys2[i] >> 32));
+      id = int64_t(rank_key_id(keys2[i]));
+      sc = rank_key_f32_value(keys2[i]);
     }
     out_ids[int64_t(b) * top_k + i] = id;
     out_scores[int64_t(b) * top_k + i] = sc;
@@ -170,8 +334,7 @@ __global__ void emit_keys_kernel(const float* __restrict__ rerank_approx, const 
   if (i >= int64_t(B) * R) return;
   const int b = int(i / R), r = int(i % R);
   uint64_t k = 0;
-  if (r < n_rerank[b])
-    k = (uint64_t(f32_key(rerank_approx[i])) << 32) | uint64_t(0xffffffffu - uint32_t(doc_id_base + rerank[i]));
+  if (r < n_rerank[b]) k = rank_key_f32(rerank_approx[i], uint32_t(doc_id_base + rerank[i]));
   keys[i] = k;
 }
 
@@ -193,7 +356,7 @@ apply_threshold_kernel(const uint64_t* __restrict__ all, int n_shards, int rank,
     keys[i] = k;
   }
   __syncthreads();
-  bitonic_desc(keys, P, tid, 1024);
+  block_sort_desc(keys, P);
   const uint64_t T = keys[R - 1];  // 0 when the whole index has fewer than R candidates
   // ordered compaction of the local list (it is in id order when nothing was pruned locally):
   // thread t owns entries [t*PER, (t+1)*PER), one block-wide exclusive scan gives the positions
@@ -287,12 +450,24 @@ int launch_apply_threshold(const Ws& ws, const uint64_t* d_all_keys, int n_shard
   return FPB_OK;
 }
 
-int launch_rank(const fpb_index* ix, const Ws& ws, int top_k, int64_t* d_out_ids, float* d_out_scores,
-                int32_t* d_out_counts, cudaStream_t st) {
-  const fpb_layout& L = *ws.L;
-  const int Rp2 = fpb_next_pow2(L.R);
-  k6_rank_kernel<<<L.B, 1024, size_t(Rp2) * 8, st>>>(ws.exact(), ws.rerank(), ws.n_rerank(), L.R, Rp2, top_k,
-                                                    ix->doc_id_base, d_out_ids, d_out_scores, d_out_counts);
+int launch_select(const float* scores, const int32_t* cand, const int32_t* n_cand, int stride, int B, int R,
+                  int32_t* rerank, float* rerank_scores, int32_t* n_rerank, cudaStream_t st) {
+  const int Rp2 = fpb_next_pow2(R);
+  // dynamic keys[] (8 B x Rp2, 32 KB at the maximum R = 4096) on top of 25 KB of static shared memory: opt in
+  // (per device: cudaFuncSetAttribute applies to the current device only, and the call is cheap)
+  FPB_CUDA_CHECK(cudaFuncSetAttribute(k3b_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Rp2 * 8));
+  k3b_select_kernel<<<B, 1024, size_t(Rp2) * 8, st>>>(scores, cand, stride, n_cand, R, Rp2, rerank, rerank_scores,
+                                                     n_rerank);
+  FPB_LAUNCH_CHECK("k3b_select");
+  return FPB_OK;
+}
+
+int launch_rank(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,
+                int64_t doc_id_base, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
+                cudaStream_t st) {
+  const int Rp2 = fpb_next_pow2(R);
+  k6_rank_kernel<<<B, 1024, size_t(Rp2) * 8, st>>>(scores, ids, n, R, Rp2, top_k, doc_id_base, d_out_ids,
+                                                  d_out_scores, d_out_counts);
   FPB_LAUNCH_CHECK("k6_rank");
   return FPB_OK;
 }

@@ -47,13 +47,20 @@ int launch_compact(const uint32_t* bitmap, const uint32_t* mask, int words, int3
                    int B, cudaStream_t st);
 int launch_approx(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st); // K3 (flags: FPB_FLAG_APPROX_*)
 int launch_walk_layout(const fpb_index* ix, cudaStream_t st);                     // K3's walk_codes (index load)
-int launch_select(const fpb_index* ix, const Ws& ws, cudaStream_t st);            // K3b
+// K3b: per query b the R best of the n_cand[b] scores in row b of `scores` (row stride `stride`) by (score desc,
+// candidate index asc); their ids (cand[b, i], or i itself when cand is NULL: then every one of the `stride` entries
+// of a row is a candidate and n_cand is not read), their scores and their count go to rerank, rerank_scores [B, R]
+// and n_rerank.
+int launch_select(const float* scores, const int32_t* cand, const int32_t* n_cand, int stride, int B, int R,
+                  int32_t* rerank, float* rerank_scores, int32_t* n_rerank, cudaStream_t st);
 int launch_maxsim(const fpb_index* ix, const Ws& ws, cudaStream_t st);            // K5 (dispatch)
 int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st);      // per-token fp16 norms (index load)
 int launch_maxsim_v4(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K5 v4 (register operands)
 int launch_maxsim_v5(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K5 v5 (wgmma, 16 decode warps)
-int launch_rank(const fpb_index* ix, const Ws& ws, int top_k, int64_t* d_out_ids, float* d_out_scores,
-                int32_t* d_out_counts, cudaStream_t st);                          // K6
+// K6: per query b the top_k of the n[b] (score, id) pairs in row b of scores / ids (row stride R) in the canonical
+// order, ids offset by doc_id_base
+int launch_rank(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,
+                int64_t doc_id_base, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t st);
 int launch_emit_keys(const fpb_index* ix, const Ws& ws, uint64_t* d_keys, cudaStream_t st);
 int launch_apply_threshold(const Ws& ws, const uint64_t* d_all_keys, int n_shards, int rank, cudaStream_t st,
                            int b_stride = 0);
@@ -61,15 +68,26 @@ int launch_merge(const fpb_record* d_all_records, int n_shards, int b_stride, in
                  int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t stream);
 int launch_emit_records(const fpb_index* ix, const Ws& ws, fpb_record* d_records, cudaStream_t st);
 
-// Workspace of the exhaustive search (exhaustive.cu).  The selection part (top_k > 0) is laid out so that an
-// fpb_layout can point k3b_select and k6_rank at it: the score array plays off_approx, an iota plays off_cand.
+// K3b and K6 of the search: select by the candidates' approximate scores, rank by the exact ones
+inline int launch_select(const Ws& ws, cudaStream_t st) {
+  return launch_select(ws.approx(), ws.cand(), ws.n_cand(), ws.L->cand_cap, ws.L->B, ws.L->R, ws.rerank(),
+                       ws.rerank_approx(), ws.n_rerank(), st);
+}
+inline int launch_rank(const fpb_index* ix, const Ws& ws, int top_k, int64_t* d_out_ids, float* d_out_scores,
+                       int32_t* d_out_counts, cudaStream_t st) {
+  return launch_rank(ws.exact(), ws.rerank(), ws.n_rerank(), ws.L->R, ws.L->B, top_k, ix->doc_id_base, d_out_ids,
+                     d_out_scores, d_out_counts, st);
+}
+
+// Workspace of the exhaustive search (exhaustive.cu).  The selection part (top_k > 0) holds the [B, N] scores that
+// k3b_select reads (every document a candidate) and the [B, top_k] list it writes for k6_rank.
 struct ExLayout {
   int B, Q, Qs, n_rows, top_k, grid;  // Qs = Q rounded up to 16; n_rows = B*Qs rounded up to 128; grid = K7 CTAs
   int64_t off_rows;     // f16 [n_rows, dim] dense query rows
   int64_t off_acc;      // u64 [B, N] fixed-point score sums
   int64_t off_carry;    // f32 [grid, n_rows] running maxima of documents that cross a tile boundary
   int64_t off_counter;  // i32 chunk counter
-  int64_t off_scores, off_cand, off_n_cand, off_n_rerank, off_rerank, off_rerank_approx;  // selection (top_k > 0)
+  int64_t off_scores, off_n_rerank, off_rerank, off_rerank_approx;  // selection (top_k > 0)
   int64_t total_bytes;
 };
 int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,

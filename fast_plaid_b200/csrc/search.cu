@@ -33,12 +33,6 @@ int prepare(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws, 
   return FPB_OK;
 }
 
-#define FPB_TRY(expr)            \
-  do {                           \
-    const int _rc = (expr);      \
-    if (_rc != FPB_OK) return _rc; \
-  } while (0)
-
 int run_until_maxsim(const fpb_index* ix, const Ws& ws, const __half* d_queries, cudaStream_t st,
                      const int32_t* d_subset_ids = nullptr, const int64_t* d_subset_offsets = nullptr,
                      int64_t max_subset_len = 0) {
@@ -49,7 +43,7 @@ int run_until_maxsim(const fpb_index* ix, const Ws& ws, const __half* d_queries,
   FPB_TRY(launch_probe(ix, ws, subset, st));
   FPB_TRY(launch_candidates(ix, ws, subset, st));
   FPB_TRY(launch_approx(ix, ws, ws.L->flags, st));
-  FPB_TRY(launch_select(ix, ws, st));
+  FPB_TRY(launch_select(ws, st));
   FPB_TRY(launch_maxsim(ix, ws, st));
   return FPB_OK;
 }
@@ -150,7 +144,7 @@ extern "C" int fpb_shard_approx_keys(const fpb_index* ix, const void* d_queries,
   FPB_TRY(launch_probe(ix, ws, false, st));
   FPB_TRY(launch_candidates(ix, ws, false, st));
   FPB_TRY(launch_approx(ix, ws, ws.L->flags, st));
-  FPB_TRY(launch_select(ix, ws, st));
+  FPB_TRY(launch_select(ws, st));
   return launch_emit_keys(ix, ws, d_keys, st);
 }
 
@@ -189,7 +183,7 @@ extern "C" int fpb_shard_subset_keys(const fpb_index* ix, int B, int Q, const fp
   FPB_TRY(launch_probe(ix, ws, true, st));
   FPB_TRY(launch_candidates(ix, ws, true, st));
   FPB_TRY(launch_approx(ix, ws, ws.L->flags, st));
-  FPB_TRY(launch_select(ix, ws, st));
+  FPB_TRY(launch_select(ws, st));
   return launch_emit_keys(ix, ws, d_keys, st);
 }
 
@@ -265,7 +259,7 @@ extern "C" int fpb_stage_approx(const fpb_index* ix, int B, int Q, const fpb_par
 extern "C" int fpb_stage_select(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws,
                                 size_t ws_bytes, void* stream) {
   FPB_STAGE_PROLOGUE(false)
-  return launch_select(ix, ws, st);
+  return launch_select(ws, st);
 }
 extern "C" int fpb_stage_maxsim(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws,
                                 size_t ws_bytes, void* stream) {

@@ -151,16 +151,20 @@ def _canonical(scores: torch.Tensor, k: int):
     return order, [float(scores[d]) for d in order]
 
 
-@pytest.mark.gpu
-def test_ranking_is_the_canonical_sort_with_ties(cuda_device):
-    base = make_docs(120, 5, 30, seed=81)
-    docs = base + [base[i].clone() for i in (3, 3, 50, 77, 119)]  # duplicated documents: exact ties
+def _check_canonical_ranking(docs, copies, query_docs, device, tied_top: bool) -> None:
+    """search_exhaustive at several k against the canonical sort of the exhaustive scores; `copies` are the indices
+    of copies of document 3.  tied_top: also assert that the copies hold the top score of every query, more than
+    2048 of them tied."""
     oidx, _ = build_oracle_index(docs)
-    didx = _device_index(oidx, cuda_device)
+    didx = _device_index(oidx, device)
     n = len(docs)
-    queries = make_queries(5, 32, seed=82, docs=docs).half().to(cuda_device)
+    queries = make_queries(5, 32, seed=82, docs=query_docs).half().to(device)
     scores = didx.exhaustive_scores(queries).cpu()
-    assert torch.equal(scores[:, 3], scores[:, 120]) and torch.equal(scores[:, 3], scores[:, 121])
+    assert torch.equal(scores[:, copies], scores[:, [3]].expand(-1, len(copies)))
+    if tied_top:
+        top = scores.max(dim=1, keepdim=True).values
+        assert torch.equal(scores[:, [3]], top), "the copied document does not hold the top score"
+        assert torch.all((scores == top).sum(dim=1) > 2048)
     for k in (1, 10, 124, n, 300, 4096):
         ids, sc, counts = (t.cpu() for t in didx.search_exhaustive(queries, k))
         assert ids.shape == (5, k) and sc.shape == (5, k)
@@ -168,9 +172,21 @@ def test_ranking_is_the_canonical_sort_with_ties(cuda_device):
             exp_ids, exp_sc = _canonical(scores[b], k)
             m = min(k, n)
             assert int(counts[b]) == m
-            assert ids[b, :m].tolist() == exp_ids, f"k={k} query {b}"
+            assert ids[b, :m].tolist() == exp_ids, f"n={n} k={k} query {b}"
             assert sc[b, :m].tolist() == exp_sc
             assert torch.all(ids[b, m:] == -1) and torch.all(sc[b, m:] == float("-inf"))
+
+
+@pytest.mark.gpu
+def test_ranking_is_the_canonical_sort_with_ties(cuda_device):
+    base = make_docs(120, 5, 30, seed=81)
+    docs = base + [base[i].clone() for i in (3, 3, 50, 77, 119)]  # duplicated documents: exact ties
+    _check_canonical_ranking(docs, [120, 121], docs, cuda_device, tied_top=False)
+    # more than 2048 copies of document 3, and queries drawn from it: the copies tie at the top of every query, so for
+    # every k <= 2048 the k-th best score lies in a value bucket of more than 2048 scores, more than k3b_select's
+    # bucket fast path orders, and the radix passes must select the smallest ids among the copies
+    docs = base + [base[3].clone() for _ in range(2100)]
+    _check_canonical_ranking(docs, list(range(120, len(docs))), [base[3]], cuda_device, tied_top=True)
 
 
 @pytest.mark.gpu

@@ -2,8 +2,7 @@
 
     python tools/bench_exhaustive.py --config cfg2 [--seconds 1.0] [--warmup 2]
 
-Times fpb_exhaustive_scores (K7 + finalize) and the whole fpb_search_exhaustive (plus the candidate fill, k3b_select
-and k6_rank) with CUDA events over at least --seconds of work after warm-up, and compares the approximate search()
+Times fpb_exhaustive_scores (K7 + finalize) and the whole fpb_search_exhaustive (plus k3b_select and k6_rank) with CUDA events over at least --seconds of work after warm-up, and compares the approximate search()
 (default parameters) against the exact result of the same batch: recall@top_k and the number of search() results
 whose score disagrees with the exhaustive score of the same document.  Needs a CUDA device; there is no fallback.
 """
