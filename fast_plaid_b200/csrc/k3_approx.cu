@@ -6,11 +6,12 @@
 // candidate, every token gathers its Qp*2-byte S row) is bound by the L1 data pipe: one wavefront per
 // gathered row, 4.87 G rows per batch on cfg-3.  Going faster needs FEWER ROWS, exactly:
 //
-//   1. tau[b,q]   = a quantile of the per-128-centroid-tile column maxima K1 already produces
-//                   (any value is correct; it only moves work between the two passes)
+//   1. tau[b,q]   = the level a candidate holds on average LAMBDA tokens at or above, estimated from sampled
+//                   candidates (K1's tile maxima only floor the histogram).  Any value is correct; it only moves
+//                   work between the two passes
 //   2. hi[b,c]    = exists q: S[b,c,q] >= tau[b,q]          (a K-bit map per query, in shared memory)
 //   3. bound pass : walk every candidate, test one bit per token, gather ONLY the rows of high centroids
-//                   (~16 % of the tokens at the median tile maximum).  With m_q = max over the gathered rows:
+//                   (19.4 % of the tokens on cfg-3 at LAMBDA = 2, DESIGN §4).  With m_q = max over the gathered rows:
 //                     m_q >= tau_q  =>  m_q is the true column maximum (every skipped row is < tau_q <= m_q)
 //                     otherwise     =>  m_q <= true maximum < tau_q
 //                   so   lb = sum_q m_q  <=  approx  <=  sum_q max(m_q, tau_q) = ub,  with lb == ub == approx
@@ -70,41 +71,60 @@ __device__ __forceinline__ void k3_next_chunk(int32_t* work, int B, int* s_b, in
   __syncthreads();
 }
 
-// maxima of the four half2 registers across the lane groups, then the fp32 sum over the real query tokens
-// (sum_dim_intlist(.., Kind::Float), search.rs:401).  The order of the additions is part of the contract between
-// the bound pass and the exact pass: both call this.
-template <int LPR>
-__device__ __forceinline__ void k3_reduce_groups(__half2& m0, __half2& m1, __half2& m2, __half2& m3) {
-#pragma unroll
-  for (int off = LPR; off < 32; off <<= 1) {
-    m0 = __hmax2(m0, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(m0), off)));
-    m1 = __hmax2(m1, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(m1), off)));
-    m2 = __hmax2(m2, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(m2), off)));
-    m3 = __hmax2(m3, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(m3), off)));
+// One lane's running column maxima: the 8 columns col0 = 8 * (lane % LPR) .. col0 + 7 of its S rows, as four half2.
+struct K3Cols {
+  __half2 h[4];
+
+  // every column at the padding sentinel, below any score.  The kernels make one before their loops and copy it: the
+  // conversion is an asm statement that the compiler does not hoist.
+  static __device__ __forceinline__ K3Cols empty() {
+    const __half2 s = __float2half2_rn(FPB_PAD_SENTINEL);
+    return K3Cols{{s, s, s, s}};
   }
-}
-template <int LPR, bool FULLQ = false>
-__device__ __forceinline__ float k3_sum_columns(__half2 m0, __half2 m1, __half2 m2, __half2 m3, int col0, int Q) {
-  float s = 0.f;
-  const float2 f0 = __half22float2(m0), f1 = __half22float2(m1), f2 = __half22float2(m2), f3 = __half22float2(m3);
-  if constexpr (FULLQ) {  // Q == Qp: every column is a real query token; same additions in the same order
-    s += f0.x; s += f0.y; s += f1.x; s += f1.y; s += f2.x; s += f2.y; s += f3.x; s += f3.y;
+  // the columns as the lane's 16 bytes of an S row
+  __device__ __forceinline__ uint4 row() const {
+    return make_uint4(half2_as_u32(h[0]), half2_as_u32(h[1]), half2_as_u32(h[2]), half2_as_u32(h[3]));
+  }
+  // fold in the lane's 16 bytes of one S row (or of tau)
+  __device__ __forceinline__ void fold(uint4 v) {
+    h[0] = __hmax2(h[0], u32_as_half2(v.x));
+    h[1] = __hmax2(h[1], u32_as_half2(v.y));
+    h[2] = __hmax2(h[2], u32_as_half2(v.z));
+    h[3] = __hmax2(h[3], u32_as_half2(v.w));
+  }
+  // fold in the maxima that lane ^ off holds in src
+  __device__ __forceinline__ void fold_xor(const K3Cols& src, int off) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      h[i] = __hmax2(h[i], u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(src.h[i]), off)));
+  }
+  // maxima across the lane groups: xor offsets FROM, 2 * FROM, .. below TO
+  template <int FROM, int TO = 32>
+  __device__ __forceinline__ void reduce() {
+#pragma unroll
+    for (int off = FROM; off < TO; off <<= 1) fold_xor(*this, off);
+  }
+  // The fp32 sum over the real query tokens (sum_dim_intlist(.., Kind::Float), search.rs:401), after reduce<LPR>():
+  // the lane's 8 columns in order, then across the LPR lanes of a row.  This order of the additions is the contract
+  // between the bound pass and the exact pass: lb, ub and the exact score are all summed here, which is what makes
+  // lb == ub == approx bit for bit when every column is resolved.  FULLQ (Q == Qp: every column is a real query
+  // token) makes the same additions in the same order.
+  template <int LPR, bool FULLQ = false>
+  __device__ __forceinline__ float sum(int col0, int Q) const {
+    float s = 0.f;
+    float2 f[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) f[i] = __half22float2(h[i]);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      if (FULLQ || col0 + 2 * i < Q) s += f[i].x;
+      if (FULLQ || col0 + 2 * i + 1 < Q) s += f[i].y;
+    }
 #pragma unroll
     for (int off = 1; off < LPR; off <<= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
     return s;
   }
-  if (col0 + 0 < Q) s += f0.x;
-  if (col0 + 1 < Q) s += f0.y;
-  if (col0 + 2 < Q) s += f1.x;
-  if (col0 + 3 < Q) s += f1.y;
-  if (col0 + 4 < Q) s += f2.x;
-  if (col0 + 5 < Q) s += f2.y;
-  if (col0 + 6 < Q) s += f3.x;
-  if (col0 + 7 < Q) s += f3.y;
-#pragma unroll
-  for (int off = 1; off < LPR; off <<= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-  return s;
-}
+};
 
 // ---------------------------------------------------------------------------------------
 // The walk layout (fpb_index::walk_codes, built once at index load by k3_walk_layout_kernel).  Every K3 walker
@@ -190,77 +210,21 @@ k3_walk_layout_kernel(const int64_t* __restrict__ doc_offsets, const int32_t* __
 // Exact pass / one-pass scoring.  One warp walks one candidate; each S row (Qp fp16 = LPR x 16 B) is fetched
 // by LPR adjacent lanes, so a warp-wide load touches 32/LPR distinct rows, and the running maxima stay in
 // registers.  `list` (the bound pass's refine list) selects the candidates; NULL = all of them.
-// Two code-distribution schemes: shuffles (any Qp) or, for Qp <= 32, shuffle-free vector loads of the
-// LPR consecutive codes a lane group gathers (the __shfl_sync run through the same L1 data pipe as the gathers).
+// How the codes reach the lanes depends on Qp.  Up to Qp = 32 the LPR lanes of a group load "their" LPR
+// consecutive codes themselves with one vector load (the lanes of a group read the same 4*LPR bytes: a broadcast;
+// the windows of the walk layout are 128-byte aligned, so the vector loads are too), which keeps __shfl_sync -- it
+// runs through the same L1 data pipe as the gathers -- out of the loop.  Above that each lane loads one code of a
+// window and the codes are shuffled to the groups.
 // ---------------------------------------------------------------------------------------
-template <int LPR, int UNROLL, int MINB>
-__global__ void __launch_bounds__(K3_THREADS, MINB)
-k3_approx_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
-                 const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
-                 const int32_t* __restrict__ cand, int cand_cap,
-                 const int32_t* __restrict__ n_cand, const int32_t* __restrict__ list,
-                 const int32_t* __restrict__ n_list, int32_t* __restrict__ work, int B,
-                 float* __restrict__ approx, unsigned long long* __restrict__ stats) {
-  constexpr int QP = LPR * 8;
-  constexpr int TPI = 32 / LPR;
-  __shared__ int s_b, s_c;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int sub = lane % LPR, grp = lane / LPR;
-  const int Ki = int(K);
-  const __half2 sentinel = __float2half2_rn(FPB_PAD_SENTINEL);
-  unsigned long long rows = 0;
+constexpr int K3_EXACT_UNROLL = 2;  // windows whose code loads are in flight at once
+constexpr int K3_EXACT_MINB = 6;    // resident CTAs per SM
 
-  for (;;) {
-    k3_next_chunk(work, B, &s_b, &s_c);
-    const int b = s_b;
-    if (b < 0) break;
-    const int n = list ? n_list[b] : n_cand[b];
-    const uint4* Sb = reinterpret_cast<const uint4*>(S + int64_t(b) * K * QP);
-    const int32_t* cb = cand + int64_t(b) * cand_cap;
-    const int32_t* lb = list ? list + int64_t(b) * cand_cap : nullptr;
-    float* ab = approx + int64_t(b) * cand_cap;
-
-    for (int i = 0; i < K3_DOCS_PER_CHUNK / 8; ++i) {
-      const int j = s_c * K3_DOCS_PER_CHUNK + i * 8 + warp;
-      if (j >= n) break;
-      const int idx = lb ? lb[j] : j;
-      const int d = cb[idx];
-      const int64_t o0 = doc_offsets[d];
-      const int len = int(doc_offsets[d + 1] - o0);
-      rows += unsigned(len);
-      const int nw = (len + 31) >> 5;
-      const int32_t* cw = walk_codes + walk_win[d] * 32 + lane;
-      __half2 m0 = sentinel, m1 = sentinel, m2 = sentinel, m3 = sentinel;
-      for (int w0 = 0; w0 < nw; w0 += UNROLL) {
-        int code[UNROLL];
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u) code[u] = (w0 + u < nw) ? __ldg(cw + (w0 + u) * 32) : Ki;
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-#pragma unroll
-          for (int jj = 0; jj < LPR; ++jj) {
-            const int c = __shfl_sync(0xffffffffu, code[u], jj * TPI + grp);
-            if (c < Ki) {
-              const uint4 v = __ldg(Sb + int64_t(c) * LPR + sub);
-              m0 = __hmax2(m0, u32_as_half2(v.x));
-              m1 = __hmax2(m1, u32_as_half2(v.y));
-              m2 = __hmax2(m2, u32_as_half2(v.z));
-              m3 = __hmax2(m3, u32_as_half2(v.w));
-            }
-          }
-        }
-      }
-      k3_reduce_groups<LPR>(m0, m1, m2, m3);
-      const float s = k3_sum_columns<LPR>(m0, m1, m2, m3, sub * 8, Q);
-      if (lane == 0) ab[idx] = s;
-    }
-  }
-  if (stats && lane == 0 && rows) atomicAdd(stats + 2, rows);
+// the slot of a window that holds the first code a lane loads: its group's first (vector loads) or its own
+template <int LPR>
+__device__ __forceinline__ int first_code(int lane) {
+  if constexpr (LPR <= 4) return lane / LPR * LPR;
+  else return lane;
 }
-
-// Shuffle-free variant: the LPR lanes of a group load "their" LPR consecutive codes themselves with one
-// vector load (the lanes of a group read the same 4*LPR bytes: a broadcast); the windows of the walk layout
-// are 128-byte aligned, so the vector loads are too.
 template <int LPR>
 __device__ __forceinline__ void load_codes(int (&c)[LPR], const int32_t* p) {
   if constexpr (LPR == 2) {
@@ -275,20 +239,22 @@ __device__ __forceinline__ void load_codes(int (&c)[LPR], const int32_t* p) {
   }
 }
 
-template <int LPR, int UNROLL, int MINB>
-__global__ void __launch_bounds__(K3_THREADS, MINB)
-k3_approx_nsh_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
-                     const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
-                     const int32_t* __restrict__ cand, int cand_cap, const int32_t* __restrict__ n_cand,
-                     const int32_t* __restrict__ list, const int32_t* __restrict__ n_list,
-                     int32_t* __restrict__ work, int B, float* __restrict__ approx,
-                     unsigned long long* __restrict__ stats) {
+template <int LPR>
+__global__ void __launch_bounds__(K3_THREADS, K3_EXACT_MINB)
+k3_exact_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
+                const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
+                const int32_t* __restrict__ cand, int cand_cap, const int32_t* __restrict__ n_cand,
+                const int32_t* __restrict__ list, const int32_t* __restrict__ n_list,
+                int32_t* __restrict__ work, int B, float* __restrict__ approx,
+                unsigned long long* __restrict__ stats) {
   constexpr int QP = LPR * 8;
+  constexpr int TPI = 32 / LPR;
+  constexpr int UNROLL = K3_EXACT_UNROLL;
   __shared__ int s_b, s_c;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int sub = lane % LPR, grp = lane / LPR;
   const int Ki = int(K);
-  const __half2 sentinel = __float2half2_rn(FPB_PAD_SENTINEL);
+  const K3Cols empty = K3Cols::empty();
   unsigned long long rows = 0;
 
   for (;;) {
@@ -301,8 +267,8 @@ k3_approx_nsh_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64
     const int32_t* lb = list ? list + int64_t(b) * cand_cap : nullptr;
     float* ab = approx + int64_t(b) * cand_cap;
 
-    for (int i = 0; i < K3_DOCS_PER_CHUNK / 8; ++i) {
-      const int j = s_c * K3_DOCS_PER_CHUNK + i * 8 + warp;
+    for (int i = 0; i < K3_DOCS_PER_CHUNK / (K3_THREADS / 32); ++i) {
+      const int j = s_c * K3_DOCS_PER_CHUNK + i * (K3_THREADS / 32) + warp;
       if (j >= n) break;
       const int idx = lb ? lb[j] : j;
       const int d = cb[idx];
@@ -310,35 +276,43 @@ k3_approx_nsh_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64
       const int len = int(doc_offsets[d + 1] - o0);
       rows += unsigned(len);
       const int nw = (len + 31) >> 5;
-      const int32_t* cw = walk_codes + walk_win[d] * 32 + grp * LPR;
-      __half2 m0 = sentinel, m1 = sentinel, m2 = sentinel, m3 = sentinel;
+      const int32_t* cw = walk_codes + walk_win[d] * 32 + first_code<LPR>(lane);
+      K3Cols m = empty;
       for (int w0 = 0; w0 < nw; w0 += UNROLL) {
-        int c[UNROLL][LPR];
+        if constexpr (LPR <= 4) {  // vector loads of the group's codes
+          int c[UNROLL][LPR];
 #pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-          if (w0 + u < nw) {
-            load_codes<LPR>(c[u], cw + (w0 + u) * 32);
-          } else {
+          for (int u = 0; u < UNROLL; ++u) {
+            if (w0 + u < nw) {
+              load_codes<LPR>(c[u], cw + (w0 + u) * 32);
+            } else {
 #pragma unroll
-            for (int jj = 0; jj < LPR; ++jj) c[u][jj] = Ki;
+              for (int jj = 0; jj < LPR; ++jj) c[u][jj] = Ki;
+            }
           }
-        }
 #pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
+          for (int u = 0; u < UNROLL; ++u) {
 #pragma unroll
-          for (int jj = 0; jj < LPR; ++jj) {
-            if (c[u][jj] < Ki) {
-              const uint4 v = __ldg(Sb + int64_t(c[u][jj]) * LPR);
-              m0 = __hmax2(m0, u32_as_half2(v.x));
-              m1 = __hmax2(m1, u32_as_half2(v.y));
-              m2 = __hmax2(m2, u32_as_half2(v.z));
-              m3 = __hmax2(m3, u32_as_half2(v.w));
+            for (int jj = 0; jj < LPR; ++jj) {
+              if (c[u][jj] < Ki) m.fold(__ldg(Sb + int64_t(c[u][jj]) * LPR));
+            }
+          }
+        } else {  // one code per lane, shuffled to the groups
+          int code[UNROLL];
+#pragma unroll
+          for (int u = 0; u < UNROLL; ++u) code[u] = (w0 + u < nw) ? __ldg(cw + (w0 + u) * 32) : Ki;
+#pragma unroll
+          for (int u = 0; u < UNROLL; ++u) {
+#pragma unroll
+            for (int jj = 0; jj < LPR; ++jj) {
+              const int c = __shfl_sync(0xffffffffu, code[u], jj * TPI + grp);
+              if (c < Ki) m.fold(__ldg(Sb + int64_t(c) * LPR));
             }
           }
         }
       }
-      k3_reduce_groups<LPR>(m0, m1, m2, m3);
-      const float s = k3_sum_columns<LPR>(m0, m1, m2, m3, sub * 8, Q);
+      m.reduce<LPR>();
+      const float s = m.sum<LPR>(sub * 8, Q);
       if (lane == 0) ab[idx] = s;
     }
   }
@@ -565,8 +539,50 @@ __device__ __forceinline__ unsigned k3_push(uint32_t word, uint32_t code, uint32
   return mask;
 }
 
-template <int LPR, int MINB, int W, int U, bool FULLQ, bool PAIR>
-__global__ void __launch_bounds__(K3_THREADS, MINB)
+constexpr int K3_BOUND_U = 4;     // gathers in flight per lane and batch
+constexpr int K3_BOUND_MINB = 4;  // resident CTAs per SM (64 registers)
+
+// One batch of gathers from the warp's ring: entry head + k * TPI + grp (k < K3_BOUND_U) is lane group grp's k-th
+// row, all loads go out before the first fold.  A full batch takes FLUSH = K3_BOUND_U * TPI entries; the drain
+// (DRAIN) at the end of a document takes the rem < FLUSH that are left and folds `empty` in place of the rest.
+template <int LPR, int WQ, bool DRAIN>
+__device__ __forceinline__ void k3_gather(K3Cols& m, const K3Cols& empty, const uint4* Sb, uint32_t sb_wq,
+                                          uint32_t head, uint32_t rem, int grp) {
+  constexpr int TPI = 32 / LPR;
+  uint4 v[K3_BOUND_U];
+#pragma unroll
+  for (int k = 0; k < K3_BOUND_U; ++k) {
+    const uint32_t jj = k * TPI + grp;
+    if (DRAIN) v[k] = empty.row();
+    if (!DRAIN || jj < rem) {
+      const uint32_t code = k3_lds(sb_wq + (((head + jj) & (WQ - 1)) << 2));
+      v[k] = __ldg(Sb + int64_t(code) * LPR);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < K3_BOUND_U; ++k) m.fold(v[k]);
+}
+
+// End of a document in the bound pass: the maxima across the lane groups (xor offsets LPR .. below TO; a paired
+// epilogue has folded offset 16 already), then lower bound = the maxima over the gathered rows, upper bound = the
+// unresolved columns raised to tau, stored at [at] by `writer`.  Both are K3Cols::sum, the exact pass's order, and fp32
+// addition is monotone, so lb <= approx <= ub; when no column was raised the two are the same additions of the same
+// values, and whenever lb == ub the score is pinned between them: "resolved" needs no flag, it IS lb == ub.
+template <int LPR, bool FULLQ, int TO>
+__device__ __forceinline__ void k3_store_bounds(K3Cols m, uint4 tq, int col0, int Q, bool writer, float* ub,
+                                                float* lb, int at) {
+  m.reduce<LPR, TO>();
+  const float l = m.sum<LPR, FULLQ>(col0, Q);
+  m.fold(tq);  // every column raised to tau
+  const float u = m.sum<LPR, FULLQ>(col0, Q);
+  if (writer) {
+    ub[at] = u;
+    lb[at] = l;
+  }
+}
+
+template <int LPR, int W, bool FULLQ>
+__global__ void __launch_bounds__(K3_THREADS, K3_BOUND_MINB)
 k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
                 const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
                 const int32_t* __restrict__ cand, int cand_cap,
@@ -575,7 +591,7 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
                 float* __restrict__ ub_out, float* __restrict__ lb_out, unsigned long long* __restrict__ stats) {
   constexpr int QP = LPR * 8;
   constexpr int TPI = 32 / LPR;   // rows per warp-wide gather
-  constexpr int FLUSH = U * TPI;  // rows per batch of gathers (<= 64)
+  constexpr int FLUSH = K3_BOUND_U * TPI;  // rows per batch of gathers (<= 64)
   constexpr int DPW = K3A_DOCS_PER_CHUNK / (K3_THREADS / 32);  // documents per warp and chunk
   constexpr int WQ = K3_WQ_FOR(W, FLUSH);  // ring entries per warp: one group of pushes on top of an unflushed rest
   static_assert(FLUSH + 32 * W <= WQ, "ring too small");
@@ -591,7 +607,7 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
   const int INV = hb_words * 32;  // a code whose bit lives in a zero word
   unsigned lt_mask;
   asm("mov.u32 %0, %%lanemask_lt;" : "=r"(lt_mask));
-  const __half2 sentinel = __float2half2_rn(FPB_PAD_SENTINEL);
+  const K3Cols empty = K3Cols::empty();
   unsigned rows = 0, toks = 0;  // per warp over the CTA's life: far below 2^32
   int cur_b = -1;
   if (tid < 32) k3_smem[hb_words + tid] = 0u;  // never overwritten: the bitmap copy below covers hb_words words
@@ -640,11 +656,11 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
       if (u < left) c[u] = __ldg(cw + 32 * u);
     }
     uint32_t head = 0, tail = 0;
-    __half2 m0 = sentinel, m1 = sentinel, m2 = sentinel, m3 = sentinel;
-    // PAIR: the end-of-document work (maxima across the lane groups, two column sums) is done for two documents at
-    // once -- the first of a pair is parked in a0..a3, then the lower half of the warp finishes one document and the
-    // upper half the other: half the shuffles, conversions and additions per document
-    __half2 a0 = sentinel, a1 = sentinel, a2 = sentinel, a3 = sentinel;
+    K3Cols m = empty;
+    // Up to Qp = 64 (LPR <= 8) the end-of-document work (maxima across the lane groups, two column sums) is done for
+    // two documents at once -- the first of a pair is parked in `a`, then the lower half of the warp finishes one
+    // document and the upper half the other: half the shuffles, conversions and additions per document
+    K3Cols a = empty;
     int slot_a = -1;
 
     for (;;) {
@@ -678,93 +694,36 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
       __syncwarp();
       // ---- gather in full batches ----
       while (tail - head >= FLUSH) {
-        uint4 v[U];
-#pragma unroll
-        for (int k = 0; k < U; ++k) {
-          const uint32_t code = k3_lds(sb_wq + (((head + k * TPI + grp) & (WQ - 1)) << 2));
-          v[k] = __ldg(Sb + int64_t(code) * LPR);
-        }
-#pragma unroll
-        for (int k = 0; k < U; ++k) {
-          m0 = __hmax2(m0, u32_as_half2(v[k].x));
-          m1 = __hmax2(m1, u32_as_half2(v[k].y));
-          m2 = __hmax2(m2, u32_as_half2(v[k].z));
-          m3 = __hmax2(m3, u32_as_half2(v[k].w));
-        }
+        k3_gather<LPR, WQ, false>(m, empty, Sb, sb_wq, head, 0u, grp);
         head += FLUSH;
       }
       if (last_of_doc) {
-        {  // drain: fewer than FLUSH codes left
-          const uint32_t rem = tail - head;
-          uint4 v[U];
-#pragma unroll
-          for (int k = 0; k < U; ++k) {
-            const uint32_t jj = k * TPI + grp;
-            v[k] = make_uint4(half2_as_u32(sentinel), half2_as_u32(sentinel), half2_as_u32(sentinel),
-                              half2_as_u32(sentinel));
-            if (jj < rem) {
-              const uint32_t code = k3_lds(sb_wq + (((head + jj) & (WQ - 1)) << 2));
-              v[k] = __ldg(Sb + int64_t(code) * LPR);
-            }
-          }
-#pragma unroll
-          for (int k = 0; k < U; ++k) {
-            m0 = __hmax2(m0, u32_as_half2(v[k].x));
-            m1 = __hmax2(m1, u32_as_half2(v[k].y));
-            m2 = __hmax2(m2, u32_as_half2(v[k].z));
-            m3 = __hmax2(m3, u32_as_half2(v[k].w));
-          }
-        }
+        k3_gather<LPR, WQ, true>(m, empty, Sb, sb_wq, head, tail - head, grp);  // drain: fewer than FLUSH codes left
         rows += tail;
         toks += unsigned(len);
         const uint4 tq = __ldg(tqp);
         const int col0 = sub * 8;
-        // lower bound: the maxima over the gathered rows; upper bound: unresolved columns raised to tau.  Both sums
-        // use the exact kernel's order, fp32 addition is monotone, so lb <= approx <= ub; when no column was raised
-        // the two are the same additions of the same values, and whenever lb == ub the score is pinned between them:
-        // "resolved" needs no flag, it IS lb == ub.
-        if (PAIR && LPR <= 8 && slot_a < 0 && nlen >= 0) {
-          a0 = m0; a1 = m1; a2 = m2; a3 = m3;  // park: the next document completes the pair
+        if (LPR <= 8 && slot_a < 0 && nlen >= 0) {
+          a = m;  // park: the next document completes the pair
           slot_a = slot;
-        } else if (PAIR && LPR <= 8 && slot_a >= 0) {
+        } else if (LPR <= 8 && slot_a >= 0) {
           const bool up = lane >= 16;  // lower half: the parked document, upper half: this one
-          __half2 x0 = up ? m0 : a0, x1 = up ? m1 : a1, x2 = up ? m2 : a2, x3 = up ? m3 : a3;
-          const __half2 y0 = up ? a0 : m0, y1 = up ? a1 : m1, y2 = up ? a2 : m2, y3 = up ? a3 : m3;
-          x0 = __hmax2(x0, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(y0), 16)));
-          x1 = __hmax2(x1, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(y1), 16)));
-          x2 = __hmax2(x2, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(y2), 16)));
-          x3 = __hmax2(x3, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(y3), 16)));
+          K3Cols x, y;
 #pragma unroll
-          for (int off = LPR; off < 16; off <<= 1) {
-            x0 = __hmax2(x0, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(x0), off)));
-            x1 = __hmax2(x1, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(x1), off)));
-            x2 = __hmax2(x2, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(x2), off)));
-            x3 = __hmax2(x3, u32_as_half2(__shfl_xor_sync(0xffffffffu, half2_as_u32(x3), off)));
+          for (int i = 0; i < 4; ++i) {  // select values: a select of m's and a's addresses puts them in local memory
+            const uint32_t mi = half2_as_u32(m.h[i]), ai = half2_as_u32(a.h[i]);
+            x.h[i] = u32_as_half2(up ? mi : ai);
+            y.h[i] = u32_as_half2(up ? ai : mi);
           }
-          const float lb = k3_sum_columns<LPR, FULLQ>(x0, x1, x2, x3, col0, Q);
-          const float ub = k3_sum_columns<LPR, FULLQ>(__hmax2(x0, u32_as_half2(tq.x)), __hmax2(x1, u32_as_half2(tq.y)),
-                                                      __hmax2(x2, u32_as_half2(tq.z)), __hmax2(x3, u32_as_half2(tq.w)),
-                                                      col0, Q);
-          if ((lane & 15) == 0) {
-            const int at = up ? slot : slot_a;
-            ub_chunk[at] = ub;
-            lb_chunk[at] = lb;
-          }
+          x.fold_xor(y, 16);
+          k3_store_bounds<LPR, FULLQ, 16>(x, tq, col0, Q, (lane & 15) == 0, ub_chunk, lb_chunk, up ? slot : slot_a);
           slot_a = -1;
         } else {
-          k3_reduce_groups<LPR>(m0, m1, m2, m3);
-          const float lb = k3_sum_columns<LPR, FULLQ>(m0, m1, m2, m3, col0, Q);
-          const float ub = k3_sum_columns<LPR, FULLQ>(__hmax2(m0, u32_as_half2(tq.x)), __hmax2(m1, u32_as_half2(tq.y)),
-                                                      __hmax2(m2, u32_as_half2(tq.z)), __hmax2(m3, u32_as_half2(tq.w)),
-                                                      col0, Q);
-          if (lane == 0) {
-            ub_chunk[slot] = ub;
-            lb_chunk[slot] = lb;
-          }
+          k3_store_bounds<LPR, FULLQ, 32>(m, tq, col0, Q, lane == 0, ub_chunk, lb_chunk, slot);
         }
         if (nlen < 0) break;  // no further document for this warp in the chunk
         head = tail = 0;
-        m0 = m1 = m2 = m3 = sentinel;
+        m = empty;
         ++slot;
       }
       __syncwarp();  // the ring slots read above may be overwritten by the next group's pushes
@@ -907,18 +866,10 @@ template <int LPR>
 int launch_k3_exact(const fpb_index* ix, const Ws& ws, const int32_t* list, const int32_t* n_list, int32_t* work,
                     cudaStream_t st) {
   const fpb_layout& L = *ws.L;
-  const int blocks = ix->sm_count * 8;
-  if constexpr (LPR <= 4) {  // shuffle-free up to Qp = 32; at Qp = 64 and above the shuffle kernel is used
-    k3_approx_nsh_kernel<LPR, 2, 6><<<blocks, K3_THREADS, 0, st>>>(
-        ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes, ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), list,
-        n_list, work, L.B, ws.approx(), ws.stats());
-    FPB_LAUNCH_CHECK("k3_approx_nsh");
-    return FPB_OK;
-  }
-  k3_approx_kernel<LPR, 2, 6><<<blocks, K3_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes,
-                                                             ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), list,
-                                                             n_list, work, L.B, ws.approx(), ws.stats());
-  FPB_LAUNCH_CHECK("k3_approx");
+  k3_exact_kernel<LPR><<<ix->sm_count * 8, K3_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes,
+                                                                 ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), list,
+                                                                 n_list, work, L.B, ws.approx(), ws.stats());
+  FPB_LAUNCH_CHECK("k3_exact");
   return FPB_OK;
 }
 
@@ -933,23 +884,20 @@ float k3_tau_lambda(int Q) {
   return x < 0.5f ? 0.5f : (x > 64.f ? 64.f : x);
 }
 
-// The bound pass with W windows per group (all their code loads in flight at once, the next group's prefetched), 4
-// gathers per lane and batch, 4 CTAs per SM at 64 registers, paired epilogues.
+// The bound pass with W windows per group (all their code loads in flight at once, the next group's prefetched),
+// K3_BOUND_U gathers per lane and batch, up to K3_BOUND_MINB CTAs per SM.
 template <int LPR, int W>
 int launch_k3_bound(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   const fpb_layout& L = *ws.L;
-  constexpr int TPI = 32 / LPR;
-  constexpr int U = 4, MINB = 4;
-  const bool fullq = L.Q == L.Qp;
-  auto kern = fullq ? k3_bound_kernel<LPR, MINB, W, U, true, true> : k3_bound_kernel<LPR, MINB, W, U, false, true>;
-  const int minb = MINB, wq = K3_WQ_FOR(W, U * TPI);
+  auto kern = L.Q == L.Qp ? k3_bound_kernel<LPR, W, true> : k3_bound_kernel<LPR, W, false>;
+  const int wq = K3_WQ_FOR(W, K3_BOUND_U * (32 / LPR));
   // bitmap + 32 zero words, then the rings (+ alignment slack)
   const size_t smem = size_t(L.hb_words + 32) * 4 + size_t(K3_THREADS / 32 + 1) * wq * 4;
   FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
   // resident CTAs per SM: limited by the bitmap (228 KB of shared memory per SM, 1 KB reserved per CTA; the
   // static shared memory is ~1.6 KB)
   int per_sm = int((227 * 1024) / (smem + 1024 + 2048));
-  per_sm = per_sm < 1 ? 1 : (per_sm > minb ? minb : per_sm);
+  per_sm = per_sm < 1 ? 1 : (per_sm > K3_BOUND_MINB ? K3_BOUND_MINB : per_sm);
   kern<<<ix->sm_count * per_sm, K3_THREADS, smem, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes,
                                                         ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), ws.work(),
                                                         L.B, ws.tau(), ws.hibits(), L.hb_words, ws.approx(), ws.lb(),

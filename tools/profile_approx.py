@@ -36,7 +36,7 @@ KERNELS = [  # (label, kernel-name pattern) in launch order
     ("k3_prefix", r"k3_prefix_kernel"),
     ("k3_bound", r"k3_bound_kernel"),
     ("k3_refine_list", r"k3_refine_list_kernel"),
-    ("exact_pass", r"k3_approx(_nsh)?_kernel"),
+    ("exact_pass", r"k3_exact_kernel"),
 ]
 
 
