@@ -21,7 +21,7 @@
 
 #include <mutex>
 
-#include "kernels.h"
+#include "entry.h"
 
 namespace {
 
@@ -151,12 +151,7 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
     fpb_set_error("fpb_search_batch_sharded: subset search goes through the fpb_shard_subset_* steps");
     return FPB_ERR_UNSUPPORTED;
   }
-  if (!ix->ivf_offsets) {
-    fpb_set_error(
-        "This index was built with compress_only=True and does not support search. "
-        "Rebuild with compress_only=False to enable search.");
-    return FPB_ERR_NO_IVF;
-  }
+  FPB_TRY(fpb_require_ivf(ix));
   const int n_shards = comm->nranks / n_query_groups;  // document shards per query group
   const int group = comm->rank / n_shards, shard = comm->rank % n_shards;
   const int b_local = (B + n_query_groups - 1) / n_query_groups;   // slots per rank in the gathered arrays
@@ -171,21 +166,12 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
   if (R < 1) R = 1;
   if (nb > 0) {
     FPB_TRY(fpb_workspace_layout(ix, nb, Q, p, &L));
-    if (size_t(L.total_bytes) > ws_bytes) {
-      fpb_set_error("workspace too small: need %lld bytes, have %zu", (long long)L.total_bytes, ws_bytes);
-      return FPB_ERR_WORKSPACE;
-    }
+    FPB_TRY(fpb_require_bytes("workspace", L.total_bytes, ws_bytes));
     R = L.R;
   }
-  if (int64_t(scratch_bytes) < fpb_sharded_scratch_bytes(b_local, R, comm->nranks)) {
-    fpb_set_error("scratch too small: need %lld bytes, have %zu",
-                  (long long)fpb_sharded_scratch_bytes(b_local, R, comm->nranks), scratch_bytes);
-    return FPB_ERR_WORKSPACE;
-  }
-  if ((reinterpret_cast<uintptr_t>(d_ws) & 255u) || (reinterpret_cast<uintptr_t>(d_scratch) & 255u)) {
-    fpb_set_error("workspace and scratch must be 256-byte aligned");
-    return FPB_ERR_INVALID;
-  }
+  FPB_TRY(fpb_require_bytes("scratch", fpb_sharded_scratch_bytes(b_local, R, comm->nranks), scratch_bytes));
+  FPB_TRY(fpb_require_aligned("workspace", d_ws));
+  FPB_TRY(fpb_require_aligned("scratch", d_scratch));
   const int64_t per_rank = int64_t(b_local) * R;
   char* sc = static_cast<char*>(d_scratch);
   uint64_t* keys = reinterpret_cast<uint64_t*>(sc);
@@ -204,13 +190,8 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
   }
   // ---- step 1: local stages up to the pruned list, keys of it ----
   if (nb > 0) {
-    const __half* q = static_cast<const __half*>(d_queries) + int64_t(q0) * Q * ix->dim;
-    FPB_TRY(launch_pad_queries(ix, ws, q, st));
-    FPB_TRY(launch_centroid_scores(ix, ws, st));
-    FPB_TRY(launch_probe(ix, ws, false, st));
-    FPB_TRY(launch_candidates(ix, ws, false, st));
-    FPB_TRY(launch_approx(ix, ws, L.flags, st));
-    FPB_TRY(launch_select(ws, st));
+    FPB_TRY(run_centroid_scores(ix, ws, static_cast<const __half*>(d_queries) + int64_t(q0) * Q * ix->dim, st));
+    FPB_TRY(run_probe_to_select(ix, ws, false, st));
     FPB_TRY(launch_emit_keys(ix, ws, keys, st));
   }
   FPB_NCCL_CHECK(nccl().AllGather(keys, all_keys, size_t(per_rank) * 8, ncclUint8, comm->comm, st));
@@ -233,19 +214,10 @@ extern "C" int fpb_search_batch_sharded_host(const fpb_index* ix, fpb_comm* comm
                                              void* d_queries_staging, int64_t* d_out_ids, float* d_out_scores,
                                              int32_t* d_out_counts, int64_t* h_out_ids, float* h_out_scores,
                                              int32_t* h_out_counts, void* stream) {
-  if (!ix || !p || !h_queries || !d_queries_staging || !h_out_ids || !h_out_scores || !h_out_counts) {
-    fpb_set_error("fpb_search_batch_sharded_host: NULL pointer");
-    return FPB_ERR_INVALID;
-  }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  FPB_CUDA_CHECK(cudaSetDevice(ix->device));
-  FPB_CUDA_CHECK(cudaMemcpyAsync(d_queries_staging, h_queries, size_t(B) * Q * ix->dim * 2, cudaMemcpyHostToDevice, st));
-  FPB_TRY(fpb_search_batch_sharded(ix, comm, n_query_groups, d_queries_staging, B, Q, p, d_ws, ws_bytes, d_scratch,
-                                   scratch_bytes, d_out_ids, d_out_scores, d_out_counts, stream));
-  const size_t n = size_t(B) * p->top_k;
-  FPB_CUDA_CHECK(cudaMemcpyAsync(h_out_ids, d_out_ids, n * 8, cudaMemcpyDeviceToHost, st));
-  FPB_CUDA_CHECK(cudaMemcpyAsync(h_out_scores, d_out_scores, n * 4, cudaMemcpyDeviceToHost, st));
-  FPB_CUDA_CHECK(cudaMemcpyAsync(h_out_counts, d_out_counts, size_t(B) * 4, cudaMemcpyDeviceToHost, st));
-  FPB_CUDA_CHECK(cudaStreamSynchronize(st));
-  return FPB_OK;
+  return search_via_host("fpb_search_batch_sharded_host", ix, h_queries, B, Q, p, d_queries_staging, d_out_ids,
+                         d_out_scores, d_out_counts, h_out_ids, h_out_scores, h_out_counts, stream, [&] {
+                           return fpb_search_batch_sharded(ix, comm, n_query_groups, d_queries_staging, B, Q, p, d_ws,
+                                                           ws_bytes, d_scratch, scratch_bytes, d_out_ids,
+                                                           d_out_scores, d_out_counts, stream);
+                         });
 }

@@ -615,11 +615,6 @@ class DeviceIndex:
         return FpbParams(params.n_ivf_probe, params.n_full_scores, params.top_k, params.batch_size,
                          params.flags | int(flags))
 
-    @staticmethod
-    def with_subset_flag(params: FpbParams) -> FpbParams:
-        return FpbParams(params.n_ivf_probe, params.n_full_scores, params.top_k, params.batch_size,
-                         params.flags | FPB_FLAG_SUBSET)
-
     def layout(self, B: int, Q: int, params: FpbParams) -> FpbLayout:
         lay = FpbLayout()
         _check(self._lib.fpb_workspace_layout(self._handle, B, Q, ctypes.byref(params), ctypes.byref(lay)))
@@ -635,11 +630,15 @@ class DeviceIndex:
                 if len(self._ws) > 64:
                     self._ws.clear()
                 self._ws[key] = lay
-            need = int(lay.total_bytes)
-            if self._buf is None or self._buf.numel() < need:
-                self._buf = None
-                self._buf = torch.empty(need, dtype=torch.uint8, device=self.device)
-            return self._buf, lay
+        return self._buffer(int(lay.total_bytes)), lay
+
+    def _buffer(self, nbytes: int) -> torch.Tensor:
+        """The grow-only device buffer that `workspace` and the exhaustive search carve up (callers hold _exclusive)."""
+        with self._lock:
+            if self._buf is None or self._buf.numel() < nbytes:
+                self._buf = None  # free the old buffer before allocating the larger one
+                self._buf = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+            return self._buf
 
     def max_queries_per_call(self, Q: int, params: FpbParams, budget_bytes: int = 6 << 30) -> int:
         key = ("maxq", Q, params.n_ivf_probe, params.n_full_scores, params.top_k, params.flags, budget_bytes)
@@ -676,14 +675,8 @@ class DeviceIndex:
         (ids int64 [B, top_k], scores f32 [B, top_k], counts int32 [B]).  Asynchronous.
         `subset`: per query a list of GLOBAL doc ids to restrict the search to
         (search.rs:494-517, :544-547)."""
-        if queries.dim() != 3:
-            raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
-        if queries.dtype != torch.float16 or queries.device != self.device:
-            raise ValueError("DeviceIndex.search expects fp16 queries on the index device")
-        queries = queries.contiguous()
-        B, Q, D = queries.shape
-        if D != self.dim:
-            raise ValueError(f"query dim {D} != index dim {self.dim}")
+        queries = self._check_queries(queries)
+        B, Q, _ = queries.shape
         k = params.top_k
         ids = torch.empty((B, k), dtype=torch.int64, device=self.device)
         scores = torch.empty((B, k), dtype=torch.float32, device=self.device)
@@ -693,8 +686,7 @@ class DeviceIndex:
         if subset is not None:
             if len(subset) != B:
                 raise ValueError("Subset length must match number of queries.")
-            params = FpbParams(params.n_ivf_probe, params.n_full_scores, params.top_k, params.batch_size,
-                               params.flags | FPB_FLAG_SUBSET)
+            params = self.with_flags(params, FPB_FLAG_SUBSET)
         step = self.max_queries_per_call(Q, params)
         with self._exclusive(), torch.cuda.device(self.device):
             for s in range(0, B, step):
@@ -727,22 +719,28 @@ class DeviceIndex:
         _check(self._lib.fpb_exhaustive_workspace_bytes(self._handle, B, Q, top_k, ctypes.byref(out)))
         return int(out.value)
 
-    def _exhaustive_buffer(self, nbytes: int) -> torch.Tensor:
-        """The grow-only workspace `search` uses (both run under _exclusive)."""
-        with self._lock:
-            if self._buf is None or self._buf.numel() < nbytes:
-                self._buf = None
-                self._buf = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-            return self._buf
-
-    def _check_queries(self, queries: torch.Tensor) -> torch.Tensor:
+    def _check_queries(self, queries: torch.Tensor, host: bool = False) -> torch.Tensor:
+        """Device queries as the kernels read them: fp16 [B, Q, dim] on this device, made contiguous.  host=True: the
+        host-buffer path's queries, floating-point [B, Q, dim] in host memory (cast to fp16 while they are staged)."""
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
-        if queries.dtype != torch.float16 or queries.device != self.device:
+        if host:
+            if queries.device.type != "cpu" or not queries.dtype.is_floating_point:
+                raise ValueError("DeviceIndex expects floating-point queries in host memory")
+        elif queries.dtype != torch.float16 or queries.device != self.device:
             raise ValueError("DeviceIndex expects fp16 queries on the index device")
         if queries.shape[2] != self.dim:
             raise ValueError(f"query dim {queries.shape[2]} != index dim {self.dim}")
-        return queries.contiguous()
+        return queries if host else queries.contiguous()
+
+    def _check_gathered(self, t: torch.Tensor, dtype: torch.dtype, trailing: tuple) -> torch.Tensor:
+        """An all-gathered input as the kernels read it: `dtype` [n_shards, B, *trailing] on this device (None in
+        `trailing`: any size), contiguous."""
+        if (t.dtype != dtype or t.device != self.device or t.dim() != 2 + len(trailing)
+                or any(n is not None and n != m for n, m in zip(trailing, t.shape[2:]))):
+            raise ValueError(f"expected gathered {dtype} [n_shards, B, *{trailing}] on {self.device}, "
+                             f"got {t.dtype} {list(t.shape)} on {t.device}")
+        return t.contiguous()
 
     def _exhaustive_step(self, B: int, Q: int, top_k: int, budget_bytes: int) -> int:
         """Most queries per call whose workspace fits the budget (at least one).  The size grows with B but not
@@ -767,7 +765,7 @@ class DeviceIndex:
         if B == 0:
             return scores
         with self._exclusive(), torch.cuda.device(self.device):
-            buf = self._exhaustive_buffer(self.exhaustive_workspace_bytes(B, Q, 0))
+            buf = self._buffer(self.exhaustive_workspace_bytes(B, Q, 0))
             _check(
                 self._lib.fpb_exhaustive_scores(
                     self._handle, queries.data_ptr(), B, Q, buf.data_ptr(), buf.numel(), scores.data_ptr(),
@@ -793,7 +791,7 @@ class DeviceIndex:
         with self._exclusive(), torch.cuda.device(self.device):
             for s in range(0, B, step):
                 e = min(B, s + step)
-                buf = self._exhaustive_buffer(self.exhaustive_workspace_bytes(e - s, Q, k))
+                buf = self._buffer(self.exhaustive_workspace_bytes(e - s, Q, k))
                 _check(
                     self._lib.fpb_search_exhaustive(
                         self._handle, queries[s:e].data_ptr(), e - s, Q, k, buf.data_ptr(), buf.numel(),
@@ -846,13 +844,7 @@ class DeviceIndex:
         """queries_host: float [B, Q, D] in HOST memory.  The H2D copy, the search and the D2H copies of the
         results all happen inside the C-ABI call, which synchronises the stream.  Returns HOST tensors
         (ids, scores, counts)."""
-        if queries_host.dim() != 3:
-            raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries_host.shape)}")
-        if queries_host.device.type != "cpu" or not queries_host.dtype.is_floating_point:
-            raise ValueError("search_host expects floating-point queries in host memory")
-        B, Q, D = queries_host.shape
-        if D != self.dim:
-            raise ValueError(f"query dim {D} != index dim {self.dim}")
+        B, Q, _ = self._check_queries(queries_host, host=True).shape
         if B == 0:
             k = params.top_k
             return (torch.empty((0, k), dtype=torch.int64), torch.empty((0, k), dtype=torch.float32),
@@ -883,7 +875,7 @@ class DeviceIndex:
     def search_records(self, queries: torch.Tensor, params: FpbParams) -> torch.Tensor:
         """Sharded mode, local half: returns uint8 [B, R, 16] records (approx f32, exact f32,
         global doc id i64) for this shard's n_full_scores/4 best candidates per query."""
-        queries = queries.contiguous()
+        queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         buf, lay = self.workspace(B, Q, params)
         rec = torch.empty((B, lay.R, 16), dtype=torch.uint8, device=self.device)
@@ -942,7 +934,7 @@ class DeviceIndex:
                        params: FpbParams) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries: fp16 [B, Q, D] on this device, the SAME batch on every rank of `comm` (collective call).
         Returns device tensors (ids, scores, counts) for all B queries."""
-        queries = queries.contiguous()
+        queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k = params.top_k
         ids = torch.empty((B, k), dtype=torch.int64, device=self.device)
@@ -959,9 +951,7 @@ class DeviceIndex:
     def search_sharded_host(self, comm: ShardComm, n_query_groups: int, queries_host: torch.Tensor,
                             params: FpbParams) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Host-buffer form of `search_sharded`: fp32/fp16 queries in HOST memory in, host tensors out."""
-        B, Q, D = queries_host.shape
-        if D != self.dim:
-            raise ValueError(f"query dim {D} != index dim {self.dim}")
+        B, Q, _ = self._check_queries(queries_host, host=True).shape
         with self._exclusive(), torch.cuda.device(self.device):
             io = self._host_io(B, Q, params.top_k)
             self._cast_into_pinned(queries_host, io["h_q"])
@@ -975,7 +965,7 @@ class DeviceIndex:
 
     # two-step sharded search (exact-scores only the globally surviving documents)
     def shard_approx_keys(self, queries: torch.Tensor, params: FpbParams) -> torch.Tensor:
-        queries = queries.contiguous()
+        queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         buf, lay = self.workspace(B, Q, params)
         keys = torch.empty((B, lay.R), dtype=torch.int64, device=self.device)
@@ -988,7 +978,7 @@ class DeviceIndex:
         """Sharded search with a `subset`, step 1a: centroid scores and this shard's bitmaps.  Returns the
         shard's centroid bitmap, int32 [B, cbitmap_words], for the all-gather.  `params.flags` must carry
         FPB_FLAG_SUBSET; `subset` holds GLOBAL document ids."""
-        queries = queries.contiguous()
+        queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         buf, lay = self.workspace(B, Q, params)
         sid, soff, smax = self._subset_csr(subset, 0, B)
@@ -1002,23 +992,25 @@ class DeviceIndex:
 
     def shard_subset_keys(self, all_cbitmaps: torch.Tensor, Q: int, params: FpbParams) -> torch.Tensor:
         """Step 1b: all_cbitmaps int32 [n_shards, B, cbitmap_words] (all-gathered) -> int64 keys [B, R]."""
+        buf, lay = self.workspace(all_cbitmaps.shape[1], Q, params)
+        all_cbitmaps = self._check_gathered(all_cbitmaps, torch.int32, (lay.cbitmap_words,))
         n_shards, B, _ = all_cbitmaps.shape
-        buf, lay = self.workspace(B, Q, params)
         keys = torch.empty((B, lay.R), dtype=torch.int64, device=self.device)
         with self._exclusive(), torch.cuda.device(self.device):
             _check(self._lib.fpb_shard_subset_keys(self._handle, B, Q, ctypes.byref(params), buf.data_ptr(),
-                                                   buf.numel(), all_cbitmaps.contiguous().data_ptr(), n_shards,
+                                                   buf.numel(), all_cbitmaps.data_ptr(), n_shards,
                                                    keys.data_ptr(), self._stream()))
         return keys
 
     def shard_exact_records(self, all_keys: torch.Tensor, rank: int, Q: int, params: FpbParams) -> torch.Tensor:
         """all_keys: int64 [n_shards, B, R] (all-gathered).  Applies the global pruning threshold to
         this shard's list, exact-scores the survivors, returns uint8 [B, R, 16] records."""
+        buf, lay = self.workspace(all_keys.shape[1], Q, params)
+        all_keys = self._check_gathered(all_keys, torch.int64, (lay.R,))
         n_shards, B, R = all_keys.shape
-        buf, lay = self.workspace(B, Q, params)
         rec = torch.empty((B, R, 16), dtype=torch.uint8, device=self.device)
         with self._exclusive(), torch.cuda.device(self.device):
-            _check(self._lib.fpb_shard_apply_threshold(self._handle, all_keys.contiguous().data_ptr(), n_shards, rank,
+            _check(self._lib.fpb_shard_apply_threshold(self._handle, all_keys.data_ptr(), n_shards, rank,
                                                        B, Q, ctypes.byref(params), buf.data_ptr(), buf.numel(),
                                                        self._stream()))
             _check(self._lib.fpb_shard_exact_records(self._handle, B, Q, ctypes.byref(params), buf.data_ptr(),
@@ -1029,6 +1021,7 @@ class DeviceIndex:
         self, all_records: torch.Tensor, top_k: int
     ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """all_records: uint8 [n_shards, B, R, 16] (all-gathered).  Global prune + rank."""
+        all_records = self._check_gathered(all_records, torch.uint8, (None, 16))
         n_shards, B, R, _ = all_records.shape
         ids = torch.empty((B, top_k), dtype=torch.int64, device=self.device)
         scores = torch.empty((B, top_k), dtype=torch.float32, device=self.device)
@@ -1036,7 +1029,7 @@ class DeviceIndex:
         with self._exclusive(), torch.cuda.device(self.device):
             _check(
                 self._lib.fpb_merge_shards(
-                    all_records.contiguous().data_ptr(), n_shards, B, R, top_k, ids.data_ptr(),
+                    all_records.data_ptr(), n_shards, B, R, top_k, ids.data_ptr(),
                     scores.data_ptr(), counts.data_ptr(), self._stream(),
                 )
             )
@@ -1048,10 +1041,9 @@ class DeviceIndex:
         """Run the pipeline stage by stage and return views of every intermediate."""
         order = ["centroid_scores", "probe", "candidates", "approx", "select", "maxsim", "rank"]
         if subset is not None:
-            params = FpbParams(params.n_ivf_probe, params.n_full_scores, params.top_k, params.batch_size,
-                               params.flags | FPB_FLAG_SUBSET)
+            params = self.with_flags(params, FPB_FLAG_SUBSET)
             order.insert(1, "subset")
-        queries = queries.contiguous()
+        queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         buf, lay = self.workspace(B, Q, params)
         st = self._stream()
@@ -1085,7 +1077,7 @@ class DeviceIndex:
 
     def stage_fn(self, name: str, queries: torch.Tensor, params: FpbParams):
         """A zero-argument callable that launches one stage on the cached workspace (bench)."""
-        queries = queries.contiguous()
+        queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         buf, lay = self.workspace(B, Q, params)
         p = ctypes.byref(params)
@@ -1160,7 +1152,7 @@ class DeviceIndex:
 
     def token_scores(self, queries: torch.Tensor, query_of: torch.Tensor, doc_ids: torch.Tensor) -> torch.Tensor:
         """fp16 [n, max_len, Q] token matrices for explicit (query, local doc) pairs."""
-        queries = queries.contiguous()
+        queries = self._check_queries(queries)
         n = int(doc_ids.shape[0])
         Q = int(queries.shape[1])
         out = torch.zeros((max(n, 1), max(self.max_doc_len, 1), Q), dtype=torch.float16, device=self.device)

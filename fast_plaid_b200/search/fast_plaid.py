@@ -538,16 +538,12 @@ class FastPlaid:
             q16 = idx.stage_queries(queries, params.top_k)  # host cast (fast_plaid.py:241) + async H2D
         else:
             q16 = queries.to(device=idx.device, dtype=torch.float16, non_blocking=True)
-        # step 1: local pruning, all-gather of the approximate-score keys
-        if subset is None:
-            keys = idx.shard_approx_keys(q16, params)
-        else:
-            # the probe is restricted to the centroids the subset documents touch (search.rs:494-517);
-            # with sharded documents that set is the union of the shards' centroid bitmaps
-            params = DeviceIndex.with_subset_flag(params)
-            cbitmap = idx.shard_subset_begin(q16, params, subset)
-            keys = idx.shard_subset_keys(all_gather(cbitmap), int(q16.shape[1]), params)
-        all_keys = all_gather(keys)
+        # step 1: local pruning, all-gather of the approximate-score keys.  The probe is restricted to the centroids
+        # the subset documents touch (search.rs:494-517); with sharded documents that set is the union of the
+        # shards' centroid bitmaps
+        params = DeviceIndex.with_flags(params, _engine.FPB_FLAG_SUBSET)
+        cbitmap = idx.shard_subset_begin(q16, params, subset)
+        all_keys = all_gather(idx.shard_subset_keys(all_gather(cbitmap), int(q16.shape[1]), params))
         # step 2: exact scores of the globally surviving documents only, all-gather of the records
         rec = idx.shard_exact_records(all_keys, rank, int(q16.shape[1]), params)
         ids, scores, counts = idx.merge_records(all_gather(rec), params.top_k)

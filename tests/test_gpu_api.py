@@ -220,7 +220,7 @@ def test_sharded_subset_search_equals_the_unsharded_subset_search(cuda_device):
     """subset= with documents sharded: the centroid bitmaps of the shards are OR-ed (the all-gather is
     emulated by stacking, all shards live on one device) and the result must equal the single-index
     subset search bit for bit, including a subset that lives entirely in one shard and an empty one."""
-    from fast_plaid_b200.engine import DeviceIndex, shard_tensors
+    from fast_plaid_b200.engine import FPB_FLAG_SUBSET, DeviceIndex, shard_tensors
 
     docs = make_docs(900, 10, 60, seed=31)
     oidx, _ = build_oracle_index(docs)
@@ -241,7 +241,7 @@ def test_sharded_subset_search_equals_the_unsharded_subset_search(cuda_device):
             for r in range(world):
                 sh, base = shard_tensors(t, r, world)
                 shards.append(DeviceIndex(sh, cuda_device, doc_id_base=base))
-            ps = DeviceIndex.with_subset_flag(params)
+            ps = DeviceIndex.with_flags(params, FPB_FLAG_SUBSET)
             Q = int(queries.shape[1])
             cbs = torch.stack([d.shard_subset_begin(queries, ps, subset) for d in shards])
             all_keys = torch.stack([d.shard_subset_keys(cbs, Q, ps) for d in shards])

@@ -30,7 +30,7 @@ def _worker(rank: int, world: int, port: int, out):
     import torch.distributed as dist
     from util import build_oracle_index, make_docs, make_queries, to_index_tensors
 
-    from fast_plaid_b200.engine import DeviceIndex, shard_tensors
+    from fast_plaid_b200.engine import FPB_FLAG_SUBSET, DeviceIndex, shard_tensors
 
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
@@ -69,7 +69,7 @@ def _worker(rank: int, world: int, port: int, out):
         subset = [torch.randperm(700, generator=g)[:200].tolist() for _ in range(queries.shape[0])]
         subset[1] = list(range(0, 100))  # lives in shard 0 only
         i4, s4, c4 = whole.search(queries, params, subset=subset)
-        ps = DeviceIndex.with_subset_flag(params)
+        ps = DeviceIndex.with_flags(params, FPB_FLAG_SUBSET)
         cb = mine.shard_subset_begin(queries, ps, subset)
         all_cb = torch.empty((world,) + tuple(cb.shape), dtype=torch.int32, device=dev)
         dist.all_gather_into_tensor(all_cb.view(-1), cb.view(-1))
