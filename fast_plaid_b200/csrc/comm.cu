@@ -169,6 +169,8 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
     FPB_TRY(fpb_require_bytes("workspace", L.total_bytes, ws_bytes));
     R = L.R;
   }
+  // refused here, before the first collective: every rank has the same parameters, so every rank returns here
+  FPB_TRY(check_merge_records("fpb_search_batch_sharded", n_shards, R));
   FPB_TRY(fpb_require_bytes("scratch", fpb_sharded_scratch_bytes(b_local, R, comm->nranks), scratch_bytes));
   FPB_TRY(fpb_require_aligned("workspace", d_ws));
   FPB_TRY(fpb_require_aligned("scratch", d_scratch));

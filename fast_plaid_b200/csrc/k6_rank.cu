@@ -270,7 +270,7 @@ k6_merge_kernel(const fpb_record* __restrict__ all_groups, int n_shards, int B, 
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);  // [P]
   uint64_t* keys2 = keys + P;                               // [Rp2]
-  uint32_t* pay = reinterpret_cast<uint32_t*>(keys2 + Rp2);  // [P] record index carried through the sort
+  uint16_t* pay = reinterpret_cast<uint16_t*>(keys2 + Rp2);  // [P] record index carried through the sort (P <= 2^14)
   __shared__ int s_valid;
   // query blockIdx.x of the whole batch = query `b` of query group blockIdx.x / B, whose records are the
   // [n_shards, B, R] block of that group (one group: the block index is the query)
@@ -294,7 +294,7 @@ k6_merge_kernel(const fpb_record* __restrict__ all_groups, int n_shards, int B, 
       }
     }
     keys[i] = k;
-    pay[i] = uint32_t(i);
+    pay[i] = uint16_t(i);
   }
   if (local_valid) atomicAdd(&s_valid, local_valid);
   __syncthreads();
@@ -423,6 +423,17 @@ apply_threshold_kernel(const uint64_t* __restrict__ all, int n_shards, int rank,
 
 }  // namespace
 
+// The merge sorts a query's n_shards*R records in shared memory: (P + Rp2)*8 + P*2 bytes with P = next_pow2 of
+// their number, 196 608 B at the limit, under the 200 KB the merge and the threshold opt in to.
+int check_merge_records(const char* who, int n_shards, int R) {
+  if (int64_t(n_shards) * R > FPB_MERGE_MAX_RECORDS) {
+    fpb_set_error("%s: n_shards*R = %d*%d records per query exceed the %d the shard merge sorts in shared memory", who,
+                  n_shards, R, FPB_MERGE_MAX_RECORDS);
+    return FPB_ERR_UNSUPPORTED;
+  }
+  return FPB_OK;
+}
+
 int launch_emit_keys(const fpb_index* ix, const Ws& ws, uint64_t* d_keys, cudaStream_t st) {
   const fpb_layout& L = *ws.L;
   const int64_t n = int64_t(L.B) * L.R;
@@ -436,12 +447,9 @@ int launch_apply_threshold(const Ws& ws, const uint64_t* d_all_keys, int n_shard
                            int b_stride) {
   const fpb_layout& L = *ws.L;
   if (b_stride <= 0) b_stride = L.B;  // queries per shard in the gathered key array
+  FPB_TRY(check_merge_records("apply_threshold", n_shards, L.R));
   const int P = fpb_next_pow2(n_shards * L.R);
   const size_t smem = size_t(P) * 8;
-  if (smem > 200 * 1024) {
-    fpb_set_error("apply_threshold: n_shards*R=%d keys per query exceed the shared-memory sort", n_shards * L.R);
-    return FPB_ERR_UNSUPPORTED;
-  }
   // opt in on every launch: the attribute is per device and the call costs about a microsecond
   FPB_CUDA_CHECK(cudaFuncSetAttribute(apply_threshold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   apply_threshold_kernel<<<L.B, 1024, smem, st>>>(d_all_keys, n_shards, rank, b_stride, L.R, P, ws.n_rerank(),
@@ -496,14 +504,11 @@ int launch_merge(const fpb_record* d_all_records, int n_shards, int b_stride, in
     fpb_set_error("fpb_merge_shards: bad arguments");
     return FPB_ERR_INVALID;
   }
+  FPB_TRY(check_merge_records("fpb_merge_shards", n_shards, R));
   if (n_queries == 0) return FPB_OK;
   const int P = fpb_next_pow2(n_shards * R);
   const int Rp2 = fpb_next_pow2(R);
-  const size_t smem = size_t(P + Rp2) * 8 + size_t(P) * 4;
-  if (smem > 200 * 1024) {
-    fpb_set_error("fpb_merge_shards: n_shards*R=%d records per query exceed the shared-memory sort", n_shards * R);
-    return FPB_ERR_UNSUPPORTED;
-  }
+  const size_t smem = size_t(P + Rp2) * 8 + size_t(P) * sizeof(uint16_t);
   // opt in on every launch: the attribute is per device and the call costs about a microsecond
   FPB_CUDA_CHECK(cudaFuncSetAttribute(k6_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   k6_merge_kernel<<<n_queries, 1024, smem, stream>>>(d_all_records, n_shards, B, R, P, Rp2, top_k, d_out_ids,

@@ -61,6 +61,11 @@ int launch_maxsim_v5(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* h
 // order, ids offset by doc_id_base
 int launch_rank(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,
                 int64_t doc_id_base, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t st);
+// The shard threshold and the shard merge sort all n_shards*R records of a query in shared memory: at most
+// FPB_MERGE_MAX_RECORDS of them.  check_merge_records sets the error (prefixed by `who`) and returns
+// FPB_ERR_UNSUPPORTED above that, FPB_OK otherwise.
+constexpr int FPB_MERGE_MAX_RECORDS = 16384;
+int check_merge_records(const char* who, int n_shards, int R);
 int launch_emit_keys(const fpb_index* ix, const Ws& ws, uint64_t* d_keys, cudaStream_t st);
 int launch_apply_threshold(const Ws& ws, const uint64_t* d_all_keys, int n_shards, int rank, cudaStream_t st,
                            int b_stride = 0);

@@ -26,8 +26,10 @@ __device__ __forceinline__ float rank_key_f32_value(uint64_t key) { return f32_u
 // ---- block-wide steps ----
 
 // Bitonic sort of keys[0, P) into descending order, P a power of two; pay[0, P), when given, is permuted along with
-// the keys.  Ends with __syncthreads().
-__device__ __forceinline__ void block_sort_desc(uint64_t* keys, int P, uint32_t* pay = nullptr) {
+// the keys (a payload of any trivially copyable type: the merge carries 16-bit record indices to save shared
+// memory).  Ends with __syncthreads().
+template <typename Pay = uint32_t>
+__device__ __forceinline__ void block_sort_desc(uint64_t* keys, int P, Pay* pay = nullptr) {
   const int tid = threadIdx.x;
   for (int k = 2; k <= P; k <<= 1) {
     for (int j = k >> 1; j > 0; j >>= 1) {
@@ -40,7 +42,7 @@ __device__ __forceinline__ void block_sort_desc(uint64_t* keys, int P, uint32_t*
             keys[i] = y;
             keys[ixj] = x;
             if (pay) {
-              const uint32_t px = pay[i];
+              const Pay px = pay[i];
               pay[i] = pay[ixj];
               pay[ixj] = px;
             }
@@ -77,6 +79,13 @@ __device__ __forceinline__ void block_min_max(float& mn, float& mx, float* s_red
 
 // The SEL_BINS linear value buckets from lo, `scale` buckets per unit value (scale = (SEL_BINS - 1) / range): a
 // larger v never falls into a lower bucket, so every value of a higher bucket is strictly larger.
+//
+// NaN is outside this order: value_bucket puts it in bucket 0, while rank_key_f32 ranks a (positive) NaN above
+// +inf.  So a selection that mixes the bucket search with the key order (K3b's fast and radix paths) would rank a
+// NaN differently by path.  No NaN reaches one: every score is a sum of maxima (__hmax2 in K3 / K5, K7's maxima)
+// that drop NaN operands.  (Those maxima start from the padding sentinel -10000, so centroid scores below it are
+// clipped to it, which the reference does only when the batch is padded: the selection tests keep their injected
+// tables above it.)
 __device__ __forceinline__ int value_bucket(float v, float lo, float scale) {
   return min(SEL_BINS - 1, max(0, __float2int_rz((v - lo) * scale)));
 }

@@ -494,6 +494,20 @@ def shard_grid(rank: int, world: int, n_query_groups: int) -> tuple[int, int, in
     return rank // n_shards, rank % n_shards, n_shards
 
 
+# The shard merge (and the shard threshold) sorts the n_shards * n_full_scores/4 records of a query in shared memory
+# (csrc/k6_rank.cu): at most this many.
+MERGE_MAX_RECORDS = 16384
+
+
+def check_merge_records(n_shards: int, n_full_scores: int) -> None:
+    """Raise ValueError when a document-sharded search over `n_shards` shards cannot merge its records, the rule
+    fpb_merge_shards and fpb_search_batch_sharded apply, so that a search is refused before any collective."""
+    R = max(int(n_full_scores) // 4, 1)
+    if n_shards * R > MERGE_MAX_RECORDS:
+        raise ValueError(f"n_full_scores={n_full_scores} over {n_shards} document shards: {n_shards}*{R} records per "
+                         f"query exceed the {MERGE_MAX_RECORDS} the shard merge supports")
+
+
 class DeviceIndex:
     """One index (or shard) resident in HBM + its ``fpb_index`` handle."""
 

@@ -524,6 +524,8 @@ class FastPlaid:
             return out
 
         rank, world = self.shard
+        # refused before the communicator or any all-gather exists (subset search: query_groups == 1)
+        _engine.check_merge_records(world // self.query_groups if subset is None else world, params.n_full_scores)
         if subset is None:
             # the whole exchange below the C ABI: one call per batch, both all-gathers on the search stream
             comm = self._shard_comm(idx)

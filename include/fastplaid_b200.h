@@ -218,7 +218,9 @@ int fpb_stage_records(const fpb_index*, int B, int Q, const fpb_params*, void* d
  * query list, fast_plaid.py:893-928).  Each rank runs fpb_search_shard on its shard and
  * emits R fixed-size records per query; the host all-gathers them (NCCL) and every rank
  * runs fpb_merge_shards, which re-applies the reference's GLOBAL pruning rule
- * (top n_full_scores/4 by approximate score, search.rs:605-619) before the final sort. */
+ * (top n_full_scores/4 by approximate score, search.rs:605-619) before the final sort.
+ * The merge sorts a query's n_shards*R records in shared memory: n_shards*R <= 16384 (e.g. 4 shards at
+ * n_full_scores = 16384, 8 at 8192), FPB_ERR_UNSUPPORTED above.  fpb_shard_apply_threshold has the same limit. */
 struct fpb_record {
   float approx;   /* -inf for padding */
   float exact;
@@ -277,7 +279,9 @@ int fpb_shard_exact_records(const fpb_index* index, int B, int Q, const fpb_para
  * issued on `stream` from inside the call; every rank returns the result of every query.
  *   d_queries  f16 [B, Q, dim]  the same batch on every rank
  *   d_ws       workspace of fpb_workspace_layout(index, ceil(B / n_query_groups), Q, params)
- *   d_scratch  fpb_sharded_scratch_bytes(ceil(B / n_query_groups), n_full_scores / 4, nranks) bytes */
+ *   d_scratch  fpb_sharded_scratch_bytes(ceil(B / n_query_groups), n_full_scores / 4, nranks) bytes
+ * The merge limit of fpb_merge_shards applies with n_shards = nranks / n_query_groups; a search above it
+ * returns FPB_ERR_UNSUPPORTED on every rank before the first all-gather. */
 #define FPB_COMM_ID_BYTES 128
 typedef struct fpb_comm fpb_comm;
 int fpb_comm_unique_id(void* out_id /* FPB_COMM_ID_BYTES */);

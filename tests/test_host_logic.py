@@ -148,6 +148,37 @@ def test_result_lists_c_helper_equals_the_python_zip():
     assert fp._results_to_lists(torch.empty((0, 4), dtype=torch.int64), torch.empty((0, 4)), torch.empty(0, dtype=torch.int32)) == []
 
 
+def test_sharded_merge_record_limit():
+    """The shard merge takes up to 16384 records per query (n_shards * n_full_scores/4): every n_full_scores one GPU
+    accepts on 4 shards, up to 8192 (R = 2048) on 8.  A sharded search above that raises ValueError before it makes a
+    communicator or gathers anything, in the one-call path and in the step-wise subset path."""
+    from fast_plaid_b200.engine import MERGE_MAX_RECORDS, DeviceIndex, check_merge_records
+    from fast_plaid_b200.search.fast_plaid import FastPlaid
+
+    assert MERGE_MAX_RECORDS == 16384
+    for n_shards, n_full in ((1, 16384), (4, 16384), (4, 16387), (8, 8192), (8, 8195), (16, 4096), (3, 1)):
+        check_merge_records(n_shards, n_full)
+    for n_shards, n_full in ((8, 8196), (8, 16384), (5, 16384), (16, 4100), (16385, 1)):
+        with pytest.raises(ValueError, match="exceed the 16384"):
+            check_merge_records(n_shards, n_full)
+
+    class Reached(Exception):
+        pass
+
+    def shard_comm(idx):
+        raise Reached
+
+    fp = FastPlaid.__new__(FastPlaid)
+    fp.shard = (0, 8)  # 8 ranks
+    fp._shard_comm = shard_comm
+    q = torch.zeros(1, 4, 128)
+    for groups, n_full, subset, error in ((1, 8196, None, ValueError), (1, 8196, [[0, 1]], ValueError),
+                                          (1, 8192, None, Reached), (2, 16384, None, Reached)):
+        fp.query_groups = groups  # 8 / groups document shards
+        with pytest.raises(error):
+            fp._search_sharded(None, q, DeviceIndex.make_params(10, n_full, 8), subset)
+
+
 def test_device_list_resolution():
     """fast_plaid.py:350-362: one string, a list, bare "cuda" -> cuda:0, duplicates dropped in order;
     anything else is refused like parse_device (load.rs:16-37)."""
