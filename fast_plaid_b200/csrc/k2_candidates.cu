@@ -88,7 +88,8 @@ k2_compact_kernel(const uint32_t* __restrict__ bitmap, const uint32_t* __restric
 }
 
 // The subset's documents as a bitmap and the centroids occurring in them as a second bitmap
-// (search.rs:496-503: lookup of the subset's codes + unique).  One warp per subset document.
+// (search.rs:496-503: lookup of the subset's codes + unique).  One warp per subset document.  cbitmap == NULL: the
+// document bitmap alone.
 __global__ void __launch_bounds__(256)
 subset_mark_kernel(const int32_t* __restrict__ ids, const int64_t* __restrict__ offsets,
                    const int64_t* __restrict__ doc_offsets, const int32_t* __restrict__ codes, int64_t n_docs,
@@ -101,6 +102,7 @@ subset_mark_kernel(const int32_t* __restrict__ ids, const int64_t* __restrict__ 
   const int64_t d = int64_t(ids[i]) - doc_id_base;
   if (d < 0 || d >= n_docs) return;  // not in this shard / invalid id: ignored
   if (lane == 0) atomicOr(sbitmap + int64_t(b) * bitmap_words + (d >> 5), 1u << (d & 31));
+  if (!cbitmap) return;
   uint32_t* cb = cbitmap + int64_t(b) * cbitmap_words;
   const int64_t o0 = doc_offsets[d], o1 = doc_offsets[d + 1];
   for (int64_t t = o0 + lane; t < o1; t += 32) {
@@ -133,6 +135,18 @@ int launch_subset_mark(const fpb_index* ix, const Ws& ws, const int32_t* d_ids, 
     subset_mark_kernel<<<grid, 256, 0, st>>>(d_ids, d_offsets, ix->doc_offsets, ix->doc_codes, ix->N,
                                              ix->doc_id_base, ws.sbitmap(), L.bitmap_words, ws.cbitmap(),
                                              L.cbitmap_words);
+    FPB_LAUNCH_CHECK("subset_mark");
+  }
+  return FPB_OK;
+}
+
+int launch_doc_bitmap(const fpb_index* ix, const int32_t* d_ids, const int64_t* d_offsets, int64_t max_len,
+                      int n_lists, uint32_t* bitmap, int words, cudaStream_t st) {
+  FPB_CUDA_CHECK(cudaMemsetAsync(bitmap, 0, size_t(n_lists) * words * 4, st));
+  if (max_len > 0) {
+    dim3 grid(unsigned((max_len + 7) / 8), n_lists);
+    subset_mark_kernel<<<grid, 256, 0, st>>>(d_ids, d_offsets, ix->doc_offsets, ix->doc_codes, ix->N,
+                                             ix->doc_id_base, bitmap, words, nullptr, 0);
     FPB_LAUNCH_CHECK("subset_mark");
   }
   return FPB_OK;

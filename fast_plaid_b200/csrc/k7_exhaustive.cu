@@ -28,6 +28,13 @@
 //     associative: the result does not depend on the order of the atomics, on the grid or on how a batch is
 //     split into calls.  Where the fp32 running sum of K5 / the reference is exact (every partial sum fits 24
 //     significant bits, the usual case) the two are bit-identical; elsewhere they can differ in the last bit.
+//
+// The list walk (LIST = true, fpb_search_exhaustive_subset) is the same kernel over per-list document lists instead
+// of the range [0, N): a chunk is (list l, positions i0 .. i0+nd) of l's sorted-unique list, the query rows are
+// grouped by list (list l's rows [row0[l], row1[l]) start on a 64-row boundary, so one warpgroup's rows belong to one
+// list), only the A stages that hold rows of l are streamed, a warpgroup without rows of l runs no MMA, and a row
+// counts only when its query searches l.  Decoder, MMA sequence and fixed-point sum are those of the full scan, so
+// every score is bit-identical to the full scan's score of the same document.
 #include <stdlib.h>
 #include <string.h>
 
@@ -84,13 +91,23 @@ __device__ __forceinline__ long long k7_fixed(float m) {
 // alone (tools/bench_exhaustive.py, FPB_K7=mma|decode).  Their scores are meaningless.
 enum K7Part { K7_ALL = 0, K7_MMA_ONLY = 1, K7_DECODE_ONLY = 2 };
 
-template <int D, int NBITS, int PART>
+// The lists of a list walk (read only when LIST): the kernel's N is then the list capacity `cap`, the row stride of
+// `ids` and of `acc`
+struct K7Lists {
+  const int32_t* ids;        // [n_lists, cap] sorted-unique local document ids of every list
+  const int32_t* count;      // [n_lists] their numbers
+  const int32_t* chunk_pfx;  // [n_lists + 1] first chunk of every list (a list without queries has none)
+  ExListTable t;             // query-row ranges of the lists, query and first token of every 16-row group
+  int n_lists;
+};
+
+template <int D, int NBITS, int PART, bool LIST = false>
 __global__ void __launch_bounds__(K7_THREADS, 1)
 k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ doc_offsets,
                      const int32_t* __restrict__ codes, const uint8_t* __restrict__ residuals,
                      const __half* __restrict__ norms, WPerm wp, const __half* __restrict__ rows, int B, int Q,
                      int Qs, int n_rows, int64_t N, int docs_per_chunk, unsigned long long* __restrict__ acc,
-                     float* __restrict__ carry_all, int* __restrict__ counter) {
+                     float* __restrict__ carry_all, int* __restrict__ counter, K7Lists lst) {
   using S = K7Smem<D>;
   constexpr int PD = D * NBITS / 8;
   constexpr int LPT = PD / 16;           // lanes per token, 16 packed bytes each
@@ -121,7 +138,7 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
   const int c = warp >> 2, w = warp & 3, quad = lane & 3;
   float* carry = carry_all + int64_t(blockIdx.x) * n_rows;
   Decoder<NBITS>::build(lut, wp, tid, K7_THREADS);
-  const int64_t n_chunks = (N + docs_per_chunk - 1) / docs_per_chunk;
+  const int64_t n_chunks = LIST ? int64_t(lst.chunk_pfx[lst.n_lists]) : (N + docs_per_chunk - 1) / docs_per_chunk;
   const int n_rb = n_rows / K7_RB;
 
   // A stage: 128 query rows, K-major SWIZZLE_128B, one cp.async group per stage
@@ -138,19 +155,45 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
   for (;;) {
     __syncthreads();  // every role is done with the previous chunk's tables
     if (tid == 0) misc[0] = atomicAdd(counter, 1);
+    if constexpr (LIST) {
+      if (tid == 0 && misc[0] < n_chunks) {  // the chunk's list: the last l with chunk_pfx[l] <= chunk
+        int lo = 0, hi = lst.n_lists - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi + 1) >> 1;
+          if (lst.chunk_pfx[mid] <= misc[0]) lo = mid;
+          else hi = mid - 1;
+        }
+        misc[4] = lo;
+      }
+    }
     __syncthreads();
     const int64_t chunk = misc[0];
     if (chunk >= n_chunks) break;
-    const int64_t d0 = chunk * docs_per_chunk;
-    const int nd = int(min(int64_t(docs_per_chunk), N - d0));
+    // full scan: documents d0 .. d0+nd-1.  List walk: positions d0 .. d0+nd-1 of list l, whose queries own the
+    // query rows [row0, row1)
+    int64_t d0;
+    int nd, row0 = 0, row1 = 0;
+    const int32_t* list = nullptr;
+    if constexpr (LIST) {
+      const int l = misc[4];
+      d0 = (chunk - lst.chunk_pfx[l]) * docs_per_chunk;
+      nd = min(docs_per_chunk, lst.count[l] - int(d0));
+      list = lst.ids + int64_t(l) * N;
+      row0 = lst.t.row0[l];
+      row1 = lst.t.row1[l];
+    } else {
+      d0 = chunk * docs_per_chunk;
+      nd = int(min(int64_t(docs_per_chunk), N - d0));
+    }
 
     // ---- chunk metadata (warp 0): documents and their pass prefix ----
     if (warp == 0) {
       int np = 0, len = 0;
       int64_t o0 = 0;
       if (lane < nd) {
-        o0 = doc_offsets[d0 + lane];
-        len = int(doc_offsets[d0 + lane + 1] - o0);
+        const int64_t d = LIST ? int64_t(list[d0 + lane]) : d0 + lane;
+        o0 = doc_offsets[d];
+        len = int(doc_offsets[d + 1] - o0);
         np = (len + 7) >> 3;
       }
       int incl = np;
@@ -196,7 +239,10 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
           t_seg[__popc(starts)] = tp;
         }
       }
-      load_a(0, 0);  // in flight during the decode
+      // the A stages to stream: every one, or those that hold rows of the chunk's list
+      const int rb_first = LIST ? row0 / K7_RB : 0;
+      const int rb_end = LIST ? (row1 + K7_RB - 1) / K7_RB : n_rb;
+      load_a(rb_first, rb_first & 1);  // in flight during the decode
       __syncthreads();
 
       // ---- decode the tile once: row r = tile pass r/8, token r%8 ----
@@ -236,8 +282,8 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
 
       // ---- stream every query row past the tile ----
       const bool two_blocks = tp > 16;
-      for (int rb = 0; rb < (PART == K7_DECODE_ONLY ? 0 : n_rb); ++rb) {
-        if (rb + 1 < n_rb) {
+      for (int rb = rb_first; rb < (PART == K7_DECODE_ONLY ? 0 : rb_end); ++rb) {
+        if (rb + 1 < rb_end) {
           load_a(rb + 1, (rb + 1) & 1);
           cp_async_wait<1>();
         } else {
@@ -248,30 +294,39 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
 
         const uint32_t a_addr = smem_u32(smA + (rb & 1) * S::a_stage) + c * 8 * 1024;  // warpgroup c: rows 64c..
         const uint32_t b_addr = smem_u32(smB);
+        // list walk: a warpgroup whose 64 rows hold no query of the chunk's list runs no MMA (warpgroup-uniform)
+        const int wg_row = rb * K7_RB + c * 64;
+        const bool mma = !LIST || (wg_row >= row0 && wg_row < row1);
         float acc0[64], acc1[64];
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
-          const uint32_t ka = (ks >> 2) * S::a_kblock + (ks & 3) * 32;
-          const uint32_t kb = (ks >> 2) * S::b_kblock + (ks & 3) * 32;
-          wgmma_m64n128k16(acc0, gmma_desc(a_addr + ka), gmma_desc(b_addr + kb), ks > 0 ? 1u : 0u);
-        }
-        wgmma_commit();
-        if (two_blocks) {
+        if (mma) {
+          wgmma_fence();
 #pragma unroll
           for (int ks = 0; ks < KS; ++ks) {
             const uint32_t ka = (ks >> 2) * S::a_kblock + (ks & 3) * 32;
             const uint32_t kb = (ks >> 2) * S::b_kblock + (ks & 3) * 32;
-            wgmma_m64n128k16(acc1, gmma_desc(a_addr + ka), gmma_desc(b_addr + 16 * 1024 + kb), ks > 0 ? 1u : 0u);
+            wgmma_m64n128k16(acc0, gmma_desc(a_addr + ka), gmma_desc(b_addr + kb), ks > 0 ? 1u : 0u);
           }
           wgmma_commit();
+          if (two_blocks) {
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) {
+              const uint32_t ka = (ks >> 2) * S::a_kblock + (ks & 3) * 32;
+              const uint32_t kb = (ks >> 2) * S::b_kblock + (ks & 3) * 32;
+              wgmma_m64n128k16(acc1, gmma_desc(a_addr + ka), gmma_desc(b_addr + 16 * 1024 + kb), ks > 0 ? 1u : 0u);
+            }
+            wgmma_commit();
+          }
         }
 
-        // thread (w, lane) holds rows wrow + lane/4 (+8) of the warp's 16 rows, all of query b
+        // thread (w, lane) holds rows wrow + lane/4 (+8) of the warp's 16 rows, all of query b.  List walk: the
+        // table gives the query of the 16-row group (-1: padding) and the token of its first row, and a row is live
+        // only when its query searches the chunk's list
         const int wrow = rb * K7_RB + c * 64 + 16 * w;
         const int r0 = wrow + (lane >> 2);
-        const int b = wrow / Qs, q0 = wrow % Qs + (lane >> 2);
-        const bool live = b < B && wrow % Qs < Q;  // warp-uniform: some row of this warp is a real query token
+        const int gq = LIST ? lst.t.grp_query[wrow >> 4] : 0, gt = LIST ? lst.t.grp_tok[wrow >> 4] : 0;
+        const int b = LIST ? max(gq, 0) : wrow / Qs, q0 = (LIST ? gt : wrow % Qs) + (lane >> 2);
+        // warp-uniform: some row of this warp is a real query token
+        const bool live = LIST ? gq >= 0 && gt < Q && wrow >= row0 && wrow < row1 : b < B && wrow % Qs < Q;
         int di = 0;
         float m0 = -INFINITY, m1 = -INFINITY;
         auto flush = [&]() {
@@ -321,6 +376,10 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
 #pragma unroll
             for (int j = 16; j < K7_PASSES; ++j) pm0[j] = pm1[j] = -INFINITY;
           }
+          if (!mma) {  // a warpgroup that ran no MMA has no maxima
+#pragma unroll
+            for (int j = 0; j < K7_PASSES; ++j) pm0[j] = pm1[j] = -INFINITY;
+          }
           const int n_seg = misc[2];
           for (int sg = 0; sg < n_seg; ++sg) {
             const int j0 = t_seg[sg], j1 = t_seg[sg + 1];
@@ -347,57 +406,132 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
   }
 }
 
-// query b, token q -> row b*Qs + q of the dense row array; every other row is zero
+// query b, token q -> row b*Qs + q of the dense row array; every other row is zero.  With grp_query (list walk):
+// row r belongs to query grp_query[r/16] (-1: padding), token grp_tok[r/16] + r%16
 __global__ void k7_pack_rows_kernel(const __half* __restrict__ q, int B, int Q, int Qs, int D, int64_t n_chunks16,
+                                    const int32_t* __restrict__ grp_query, const int32_t* __restrict__ grp_tok,
                                     __half* __restrict__ rows) {
   const int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
   if (i >= n_chunks16) return;
   const int cpr = D / 8;
   const int64_t r = i / cpr;
   const int cc = int(i % cpr);
-  const int64_t b = r / Qs;
-  const int qq = int(r % Qs);
+  int64_t b = r / Qs;
+  int qq = int(r % Qs);
+  if (grp_query) {
+    b = grp_query[r >> 4];
+    qq = grp_tok[r >> 4] + int(r & 15);
+  }
   uint4 v = make_uint4(0u, 0u, 0u, 0u);
-  if (b < B && qq < Q) v = *reinterpret_cast<const uint4*>(q + (b * Q + qq) * D + cc * 8);
+  if (b >= 0 && b < B && qq < Q) v = *reinterpret_cast<const uint4*>(q + (b * Q + qq) * D + cc * 8);
   reinterpret_cast<uint4*>(rows)[i] = v;
 }
 
-// exact fixed-point sums -> fp32 scores; a document without tokens scores Q times the padding sentinel
+// exact fixed-point sum -> fp32 score; a document without tokens scores Q times the padding sentinel
+__device__ __forceinline__ float k7_score(unsigned long long sum, bool empty, int Q) {
+  return empty ? float(Q) * FPB_PAD_SENTINEL : __ll2float_rn(static_cast<long long>(sum)) * (1.0f / 16777216.0f);
+}
+
 __global__ void k7_finalize_kernel(const unsigned long long* __restrict__ acc, const int64_t* __restrict__ doc_offsets,
                                    int64_t N, int64_t total, int Q, float* __restrict__ scores) {
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
     const int64_t d = i % N;
-    const bool empty = doc_offsets[d + 1] == doc_offsets[d];
-    scores[i] = empty ? float(Q) * FPB_PAD_SENTINEL
-                      : __ll2float_rn(static_cast<long long>(acc[i])) * (1.0f / 16777216.0f);
+    scores[i] = k7_score(acc[i], doc_offsets[d + 1] == doc_offsets[d], Q);
   }
 }
 
-template <int D, int NBITS, int PART>
-int launch_k7_t(const fpb_index* ix, const ExLayout& X, char* ws, cudaStream_t st) {
-  auto kern = k7_exhaustive_kernel<D, NBITS, PART>;
-  constexpr int smem = K7Smem<D>::bytes;
-  // opt in on every launch: the attribute is per device and the call costs about a microsecond
-  FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  // documents per chunk: as many as one warp scans, fewer (down to 4, as in v5) when that leaves too few chunks to
-  // balance the SMs.  FPB_K7_DOCS_PER_CHUNK=n (1..32) pins it: the result does not depend on it, and the tests use
-  // it to run the multi-document chunk walk on small indexes.
+// list walk: row b of the [B, cap] arrays k3b_select reads -- the scores of query b's list, its local document ids
+// (the candidates, ascending) and their number.  Positions past the end of the list are not written.
+__global__ void k7_list_finalize_kernel(const unsigned long long* __restrict__ acc,
+                                        const int64_t* __restrict__ doc_offsets, const int32_t* __restrict__ ids,
+                                        const int32_t* __restrict__ count, const int32_t* __restrict__ qlist,
+                                        int64_t cap, int64_t total, int Q, float* __restrict__ scores,
+                                        int32_t* __restrict__ cand, int32_t* __restrict__ n_cand) {
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
+    const int64_t b = i / cap, p = i % cap;
+    const int l = qlist[b], n = count[l];
+    if (p == 0) n_cand[b] = n;
+    if (p < n) {
+      const int32_t d = ids[l * cap + p];
+      cand[i] = d;
+      scores[i] = k7_score(acc[i], doc_offsets[d + 1] == doc_offsets[d], Q);
+    }
+  }
+}
+
+// list walk, one CTA: pfx[l] = chunks of the lists before l (ceil(count / dpc) for a list that some query searches,
+// none otherwise), pfx[n_lists] = all of them
+__global__ void __launch_bounds__(1024)
+k7_list_chunks_kernel(const int32_t* __restrict__ count, ExListTable t, int n_lists, int dpc, int32_t* __restrict__ pfx) {
+  __shared__ int warp_sums[32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int per = (n_lists + 1023) / 1024, l0 = min(n_lists, tid * per), l1 = min(n_lists, l0 + per);
+  auto chunks = [&](int l) { return t.row1[l] > t.row0[l] ? (count[l] + dpc - 1) / dpc : 0; };
+  int sum = 0;
+  for (int l = l0; l < l1; ++l) sum += chunks(l);
+  int incl = sum;
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, off);
+    if (lane >= off) incl += v;
+  }
+  if (lane == 31) warp_sums[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    const int ws = warp_sums[lane];
+    int wincl = ws;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, wincl, off);
+      if (lane >= off) wincl += v;
+    }
+    warp_sums[lane] = wincl - ws;  // exclusive
+  }
+  __syncthreads();
+  int run = warp_sums[warp] + incl - sum;
+  for (int l = l0; l < l1; ++l) {
+    pfx[l] = run;
+    run += chunks(l);
+  }
+  if (tid == 1023) pfx[n_lists] = run;
+}
+
+// documents per chunk: as many as one warp scans, fewer (down to 4, as in v5) when that leaves too few chunks of
+// `n_docs` documents to balance the SMs.  FPB_K7_DOCS_PER_CHUNK=n (1..32) pins it: the result does not depend on it,
+// and the tests use it to run the multi-document chunk walk on small indexes.
+int k7_docs_per_chunk(const fpb_index* ix, int64_t n_docs) {
   int dpc = K7_MAX_DOCS;
-  while (dpc > 4 && (ix->N + dpc - 1) / dpc < int64_t(ix->sm_count) * 8) dpc >>= 1;
+  while (dpc > 4 && (n_docs + dpc - 1) / dpc < int64_t(ix->sm_count) * 8) dpc >>= 1;
   if (const char* pin = getenv("FPB_K7_DOCS_PER_CHUNK")) {
     const int v = atoi(pin);
     if (v >= 1 && v <= K7_MAX_DOCS) dpc = v;
   }
-  const int64_t chunks = (ix->N + dpc - 1) / dpc;
+  return dpc;
+}
+
+template <int D, int NBITS, int PART, bool LIST = false>
+int launch_k7_t(const fpb_index* ix, const ExLayout& X, char* ws, int dpc, cudaStream_t st,
+                const K7Lists& lst = K7Lists{}) {
+  auto kern = k7_exhaustive_kernel<D, NBITS, PART, LIST>;
+  constexpr int smem = K7Smem<D>::bytes;
+  // opt in on every launch: the attribute is per device and the call costs about a microsecond
+  FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  // list walk: at most one partial chunk per list on top of the expected total length
+  const int64_t chunks = LIST ? (X.list_docs + dpc - 1) / dpc + X.n_lists : (ix->N + dpc - 1) / dpc;
   const int blocks = int(chunks < X.grid ? chunks : X.grid);
   kern<<<blocks, K7_THREADS, smem, st>>>(ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals,
                                          ix->token_norms, ix->w_perm, reinterpret_cast<const __half*>(ws + X.off_rows), X.B,
-                                         X.Q, X.Qs, X.n_rows, ix->N, dpc,
+                                         X.Q, X.Qs, X.n_rows, LIST ? X.cap : ix->N, dpc,
                                          reinterpret_cast<unsigned long long*>(ws + X.off_acc),
                                          reinterpret_cast<float*>(ws + X.off_carry),
-                                         reinterpret_cast<int*>(ws + X.off_counter));
+                                         reinterpret_cast<int*>(ws + X.off_counter), lst);
   FPB_LAUNCH_CHECK("k7_exhaustive");
   return FPB_OK;
+}
+
+int finalize_blocks(const fpb_index* ix, int64_t total) {
+  const int64_t want = (total + 255) / 256;
+  return int(want < int64_t(ix->sm_count) * 16 ? want : int64_t(ix->sm_count) * 16);
 }
 
 }  // namespace
@@ -406,31 +540,73 @@ int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, c
                              float* d_scores, cudaStream_t st) {
   if (ix->N == 0) return FPB_OK;
   const int64_t n16 = int64_t(X.n_rows) * (ix->dim / 8);
-  k7_pack_rows_kernel<<<int((n16 + 255) / 256), 256, 0, st>>>(d_queries, X.B, X.Q, X.Qs, ix->dim, n16,
-                                                               reinterpret_cast<__half*>(ws + X.off_rows));
+  k7_pack_rows_kernel<<<int((n16 + 255) / 256), 256, 0, st>>>(d_queries, X.B, X.Q, X.Qs, ix->dim, n16, nullptr,
+                                                               nullptr, reinterpret_cast<__half*>(ws + X.off_rows));
   FPB_LAUNCH_CHECK("k7_pack_rows");
   FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_acc, 0, size_t(X.B) * ix->N * 8, st));
   FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_counter, 0, sizeof(int), st));
   // FPB_K7=mma | decode: timing variants of dim 128 / nbits 4 (their scores are meaningless)
   const char* part = getenv("FPB_K7");
   const bool mma_only = part && strcmp(part, "mma") == 0, decode_only = part && strcmp(part, "decode") == 0;
+  const int dpc = k7_docs_per_chunk(ix, ix->N);
   int rc;
-  if (ix->dim == 128 && ix->nbits == 4 && mma_only) rc = launch_k7_t<128, 4, K7_MMA_ONLY>(ix, X, ws, st);
-  else if (ix->dim == 128 && ix->nbits == 4 && decode_only) rc = launch_k7_t<128, 4, K7_DECODE_ONLY>(ix, X, ws, st);
-  else if (ix->dim == 128 && ix->nbits == 4) rc = launch_k7_t<128, 4, K7_ALL>(ix, X, ws, st);
-  else if (ix->dim == 128 && ix->nbits == 2) rc = launch_k7_t<128, 2, K7_ALL>(ix, X, ws, st);
-  else if (ix->dim == 64 && ix->nbits == 4) rc = launch_k7_t<64, 4, K7_ALL>(ix, X, ws, st);
-  else if (ix->dim == 64 && ix->nbits == 2) rc = launch_k7_t<64, 2, K7_ALL>(ix, X, ws, st);
+  if (ix->dim == 128 && ix->nbits == 4 && mma_only) rc = launch_k7_t<128, 4, K7_MMA_ONLY>(ix, X, ws, dpc, st);
+  else if (ix->dim == 128 && ix->nbits == 4 && decode_only) rc = launch_k7_t<128, 4, K7_DECODE_ONLY>(ix, X, ws, dpc, st);
+  else if (ix->dim == 128 && ix->nbits == 4) rc = launch_k7_t<128, 4, K7_ALL>(ix, X, ws, dpc, st);
+  else if (ix->dim == 128 && ix->nbits == 2) rc = launch_k7_t<128, 2, K7_ALL>(ix, X, ws, dpc, st);
+  else if (ix->dim == 64 && ix->nbits == 4) rc = launch_k7_t<64, 4, K7_ALL>(ix, X, ws, dpc, st);
+  else if (ix->dim == 64 && ix->nbits == 2) rc = launch_k7_t<64, 2, K7_ALL>(ix, X, ws, dpc, st);
   else {
     fpb_set_error("exhaustive search: unsupported (dim=%d, nbits=%d)", ix->dim, ix->nbits);
     return FPB_ERR_UNSUPPORTED;
   }
   if (rc != FPB_OK) return rc;
   const int64_t total = int64_t(X.B) * ix->N;
-  const int64_t want = (total + 255) / 256;
-  const int blocks = int(want < int64_t(ix->sm_count) * 16 ? want : int64_t(ix->sm_count) * 16);
-  k7_finalize_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const unsigned long long*>(ws + X.off_acc),
-                                             ix->doc_offsets, ix->N, total, X.Q, d_scores);
+  k7_finalize_kernel<<<finalize_blocks(ix, total), 256, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(ws + X.off_acc), ix->doc_offsets, ix->N, total, X.Q, d_scores);
   FPB_LAUNCH_CHECK("k7_finalize");
+  return FPB_OK;
+}
+
+int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
+                                  const int32_t* d_list_ids, const int64_t* d_list_offsets, int64_t max_list_len,
+                                  cudaStream_t st) {
+  if (!((ix->dim == 128 || ix->dim == 64) && (ix->nbits == 4 || ix->nbits == 2))) {
+    fpb_set_error("exhaustive search: unsupported (dim=%d, nbits=%d)", ix->dim, ix->nbits);
+    return FPB_ERR_UNSUPPORTED;
+  }
+  const ExListTable t = ExListTable::at(reinterpret_cast<int32_t*>(ws + X.off_table), X.n_lists, X.B, X.n_rows);
+  int32_t* ids = reinterpret_cast<int32_t*>(ws + X.off_lists);
+  int32_t* count = reinterpret_cast<int32_t*>(ws + X.off_lcount);
+  int32_t* chunk_pfx = reinterpret_cast<int32_t*>(ws + X.off_chunks);
+  // 1. every list sorted and deduplicated: a document bitmap per list, compacted in id order
+  uint32_t* bitmap = reinterpret_cast<uint32_t*>(ws + X.off_bitmap);
+  FPB_TRY(launch_doc_bitmap(ix, d_list_ids, d_list_offsets, max_list_len, X.n_lists, bitmap, X.words, st));
+  FPB_TRY(launch_compact(bitmap, nullptr, X.words, ids, int(X.cap), count, X.n_lists, st));
+  const int dpc = k7_docs_per_chunk(ix, X.list_docs);
+  k7_list_chunks_kernel<<<1, 1024, 0, st>>>(count, t, X.n_lists, dpc, chunk_pfx);
+  FPB_LAUNCH_CHECK("k7_list_chunks");
+  // 2. the query rows, grouped by list
+  const int64_t n16 = int64_t(X.n_rows) * (ix->dim / 8);
+  k7_pack_rows_kernel<<<int((n16 + 255) / 256), 256, 0, st>>>(d_queries, X.B, X.Q, X.Qs, ix->dim, n16, t.grp_query,
+                                                               t.grp_tok, reinterpret_cast<__half*>(ws + X.off_rows));
+  FPB_LAUNCH_CHECK("k7_pack_rows");
+  FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_acc, 0, size_t(X.B) * X.cap * 8, st));
+  FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_counter, 0, sizeof(int), st));
+  // 3. K7 over the lists
+  const K7Lists lst{ids, count, chunk_pfx, t, X.n_lists};
+  int rc;
+  if (ix->dim == 128 && ix->nbits == 4) rc = launch_k7_t<128, 4, K7_ALL, true>(ix, X, ws, dpc, st, lst);
+  else if (ix->dim == 128 && ix->nbits == 2) rc = launch_k7_t<128, 2, K7_ALL, true>(ix, X, ws, dpc, st, lst);
+  else if (ix->dim == 64 && ix->nbits == 4) rc = launch_k7_t<64, 4, K7_ALL, true>(ix, X, ws, dpc, st, lst);
+  else rc = launch_k7_t<64, 2, K7_ALL, true>(ix, X, ws, dpc, st, lst);
+  if (rc != FPB_OK) return rc;
+  // 4. the [B, cap] scores, candidates and counts of the selection
+  const int64_t total = int64_t(X.B) * X.cap;
+  k7_list_finalize_kernel<<<finalize_blocks(ix, total), 256, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(ws + X.off_acc), ix->doc_offsets, ids, count, t.qlist, X.cap, total,
+      X.Q, reinterpret_cast<float*>(ws + X.off_scores), reinterpret_cast<int32_t*>(ws + X.off_cand),
+      reinterpret_cast<int32_t*>(ws + X.off_n_cand));
+  FPB_LAUNCH_CHECK("k7_list_finalize");
   return FPB_OK;
 }

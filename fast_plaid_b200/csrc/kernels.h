@@ -84,16 +84,52 @@ inline int launch_rank(const fpb_index* ix, const Ws& ws, int top_k, int64_t* d_
                      d_out_scores, d_out_counts, st);
 }
 
+// the document bitmap alone of subset_mark_kernel, [n_lists, words]: list l owns d_ids[d_offsets[l] ..
+// d_offsets[l+1]) (global ids; ids outside the index are ignored)
+int launch_doc_bitmap(const fpb_index* ix, const int32_t* d_ids, const int64_t* d_offsets, int64_t max_len,
+                      int n_lists, uint32_t* bitmap, int words, cudaStream_t st);
+
 // Workspace of the exhaustive search (exhaustive.cu).  The selection part (top_k > 0) holds the [B, N] scores that
-// k3b_select reads (every document a candidate) and the [B, top_k] list it writes for k6_rank.
+// k3b_select reads (every document a candidate) and the [B, top_k] list it writes for k6_rank.  A list walk
+// (n_lists > 0, fpb_search_exhaustive_subset) has [B, cap] scores instead, with their candidates, and the lists.
 struct ExLayout {
   int B, Q, Qs, n_rows, top_k, grid;  // Qs = Q rounded up to 16; n_rows = B*Qs rounded up to 128; grid = K7 CTAs
   int64_t off_rows;     // f16 [n_rows, dim] dense query rows
-  int64_t off_acc;      // u64 [B, N] fixed-point score sums
+  int64_t off_acc;      // u64 [B, N] fixed-point score sums ([B, cap] in a list walk)
   int64_t off_carry;    // f32 [grid, n_rows] running maxima of documents that cross a tile boundary
   int64_t off_counter;  // i32 chunk counter
   int64_t off_scores, off_n_rerank, off_rerank, off_rerank_approx;  // selection (top_k > 0)
+  // list walk only (zero bytes otherwise).  n_rows = B*Qs + 48*n_lists rounded up to 128: every list's rows start on
+  // a 64-row boundary.  list_docs = cap x the number of lists some query searches (set per call).
+  int n_lists, words;       // lists; uint32 words of a document bitmap
+  int64_t cap, list_docs;   // positions per list = min(N, max_list_len) (at least 1)
+  int64_t off_bitmap;       // u32 [n_lists, words] documents of every list
+  int64_t off_lists;        // i32 [n_lists, cap] sorted-unique local ids of every list
+  int64_t off_lcount;       // i32 [n_lists] their numbers
+  int64_t off_chunks;       // i32 [n_lists + 1] chunk prefix of the lists
+  int64_t off_table;        // i32 ExListTable, built on the host
+  int64_t off_cand;         // i32 [B, cap] query b's candidates (its list's ids)
+  int64_t off_n_cand;       // i32 [B] their numbers
   int64_t total_bytes;
 };
+
+// The host-built table of a list walk (int32, in the workspace at off_table)
+struct ExListTable {
+  int32_t* row0;       // [n_lists] first query row of every list (64-row aligned)
+  int32_t* row1;       // [n_lists] end of its rows (= row0 for a list no query searches)
+  int32_t* qlist;      // [B] the list every query searches
+  int32_t* grp_query;  // [n_rows / 16] query of every 16-row group of the row array, -1 for padding
+  int32_t* grp_tok;    // [n_rows / 16] token of the group's first row
+  static int64_t ints(int n_lists, int B, int n_rows) { return 2 * int64_t(n_lists) + B + 2 * int64_t(n_rows / 16); }
+  static ExListTable at(int32_t* t, int n_lists, int B, int n_rows) {
+    int32_t* q = t + 2 * int64_t(n_lists);
+    return {t, t + n_lists, q, q + B, q + B + n_rows / 16};
+  }
+};
+
 int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
                              float* d_scores, cudaStream_t st);  // K7 + finalize
+// list walk: canonical lists, K7 over them, and the [B, cap] scores / candidates / counts of the layout
+int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
+                                  const int32_t* d_list_ids, const int64_t* d_list_offsets, int64_t max_list_len,
+                                  cudaStream_t st);

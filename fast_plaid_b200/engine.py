@@ -132,6 +132,8 @@ EXPORTED_SYMBOLS = [
     "fpb_exhaustive_workspace_bytes",
     "fpb_exhaustive_scores",
     "fpb_search_exhaustive",
+    "fpb_exhaustive_subset_workspace_bytes",
+    "fpb_search_exhaustive_subset",
     "fpb_reconstruct",
     "fpb_token_scores",
     "fpb_encode",
@@ -245,6 +247,11 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_exhaustive_scores.argtypes = [vp, vp, i32, i32, vp, sz, vp, vp]
         lib.fpb_search_exhaustive.restype = i32
         lib.fpb_search_exhaustive.argtypes = [vp, vp, i32, i32, i32, vp, sz, vp, vp, vp, vp]
+        lib.fpb_exhaustive_subset_workspace_bytes.restype = i32
+        lib.fpb_exhaustive_subset_workspace_bytes.argtypes = [vp, i32, i32, i32, i32, i64, ctypes.POINTER(sz)]
+        lib.fpb_search_exhaustive_subset.restype = i32
+        lib.fpb_search_exhaustive_subset.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, i64, vp, vp, sz, vp, vp, vp,
+                                                     vp]
         _lib = lib
         return lib
 
@@ -256,6 +263,27 @@ def _check(rc: int) -> None:
     if rc in (FPB_ERR_INVALID, FPB_ERR_NO_IVF, FPB_ERR_UNSUPPORTED):
         raise ValueError(msg)  # anyhow -> PyValueError in the reference (rust/utils/errors.rs:5-7)
     raise RuntimeError(msg)
+
+
+def group_subsets(subset) -> tuple[list, list[int]]:
+    """Per-query id lists -> (distinct lists, the list of every query).  Identical lists become one, so that the
+    queries that share it share one decode of each of its documents: by object identity first (the broadcast
+    ``subset=[ids]`` form in one step), then by equal contents.  An empty list stays a list of its own."""
+    lists: list = []
+    query_list: list[int] = []
+    by_object: dict[int, int] = {}
+    by_contents: dict[tuple, int] = {}
+    for s in subset:
+        l = by_object.get(id(s))  # `subset` keeps every object alive, so an id is not reused during the loop
+        if l is None:
+            key = tuple(int(i) for i in s)
+            l = by_contents.get(key)
+            if l is None:
+                l = by_contents[key] = len(lists)
+                lists.append(s)
+            by_object[id(s)] = l
+        query_list.append(l)
+    return lists, query_list
 
 
 def _require_cuda() -> None:
@@ -756,15 +784,19 @@ class DeviceIndex:
                              f"got {t.dtype} {list(t.shape)} on {t.device}")
         return t.contiguous()
 
-    def _exhaustive_step(self, B: int, Q: int, top_k: int, budget_bytes: int) -> int:
+    def _exhaustive_step(self, B: int, Q: int, top_k: int, budget_bytes: int, workspace_bytes=None) -> int:
         """Most queries per call whose workspace fits the budget (at least one).  The size grows with B but not
-        linearly (query rows are padded to blocks of 128), so the largest fitting call is found by bisection."""
-        if self.exhaustive_workspace_bytes(B, Q, top_k) <= budget_bytes:
+        linearly (query rows are padded to blocks of 128), so the largest fitting call is found by bisection.
+        `workspace_bytes(B)`: the workspace of a call of B queries (default: fpb_search_exhaustive's)."""
+        if workspace_bytes is None:
+            def workspace_bytes(b: int) -> int:
+                return self.exhaustive_workspace_bytes(b, Q, top_k)
+        if workspace_bytes(B) <= budget_bytes:
             return B
         lo, hi = 1, B  # ws(lo) may exceed the budget: one query per call is the floor
         while lo < hi:
             mid = (lo + hi + 1) // 2
-            if self.exhaustive_workspace_bytes(mid, Q, top_k) <= budget_bytes:
+            if workspace_bytes(mid) <= budget_bytes:
                 lo = mid
             else:
                 hi = mid - 1
@@ -788,11 +820,22 @@ class DeviceIndex:
             )
         return scores
 
-    def search_exhaustive(self, queries: torch.Tensor, top_k: int, budget_bytes: int = 6 << 30
-                          ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    def exhaustive_subset_workspace_bytes(self, B: int, Q: int, top_k: int, n_lists: int, max_list_len: int) -> int:
+        """Workspace of fpb_search_exhaustive_subset."""
+        out = ctypes.c_size_t()
+        _check(self._lib.fpb_exhaustive_subset_workspace_bytes(self._handle, B, Q, top_k, n_lists, max_list_len,
+                                                               ctypes.byref(out)))
+        return int(out.value)
+
+    def search_exhaustive(self, queries: torch.Tensor, top_k: int, budget_bytes: int = 6 << 30,
+                          subset: list[list[int]] | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Exact top_k over every document: (ids int64 [B, top_k] global, scores f32 [B, top_k], counts int32 [B]),
         the result contract of `search`.  The batch is split into calls whose workspace fits `budget_bytes`;
-        the result does not depend on the split.  Asynchronous."""
+        the result does not depend on the split.  Asynchronous.
+
+        `subset`: per query a list of GLOBAL doc ids (any order; duplicates and ids outside the index are ignored).
+        Query b is then ranked among the documents of subset[b] only, with counts[b] = min(top_k, #documents), and
+        every score is the one `exhaustive_scores` gives the same document."""
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k = int(top_k)
@@ -800,6 +843,11 @@ class DeviceIndex:
         scores = torch.empty((B, k), dtype=torch.float32, device=self.device)
         counts = torch.empty((B,), dtype=torch.int32, device=self.device)
         if B == 0:
+            return ids, scores, counts
+        if subset is not None:
+            if len(subset) != B:
+                raise ValueError("Subset length must match number of queries.")
+            self._search_exhaustive_subset(queries, k, budget_bytes, subset, ids, scores, counts)
             return ids, scores, counts
         step = self._exhaustive_step(B, Q, k, budget_bytes)
         with self._exclusive(), torch.cuda.device(self.device):
@@ -813,6 +861,37 @@ class DeviceIndex:
                     )
                 )
         return ids, scores, counts
+
+    def _search_exhaustive_subset(self, queries: torch.Tensor, k: int, budget_bytes: int, subset: list,
+                                  ids: torch.Tensor, scores: torch.Tensor, counts: torch.Tensor) -> None:
+        """search_exhaustive with per-query subsets: identical subsets become one list (group_subsets), and each call
+        passes the lists of its own queries."""
+        B, Q, _ = queries.shape
+        lists, query_list = group_subsets(subset)
+        max_len = max(len(x) for x in lists)
+        # a call of b queries has at most min(b, len(lists)) lists, none longer than max_len: its workspace bound
+        step = self._exhaustive_step(B, Q, k, budget_bytes, lambda b: self.exhaustive_subset_workspace_bytes(
+            b, Q, k, min(b, len(lists)), max_len))
+        step = min(step, 65535)  # the library's limit on lists per call
+        keep = []
+        with self._exclusive(), torch.cuda.device(self.device):
+            for s in range(0, B, step):
+                e = min(B, s + step)
+                local: dict[int, int] = {}  # list -> its index in this call, in order of first use
+                call_list = [local.setdefault(l, len(local)) for l in query_list[s:e]]
+                call_lists = [lists[l] for l in local]
+                sid, soff, smax = self._subset_csr(call_lists, 0, len(call_lists))
+                h_list = (ctypes.c_int32 * (e - s))(*call_list)
+                buf = self._buffer(self.exhaustive_subset_workspace_bytes(e - s, Q, k, len(call_lists), smax))
+                _check(
+                    self._lib.fpb_search_exhaustive_subset(
+                        self._handle, queries[s:e].data_ptr(), e - s, Q, k, sid.data_ptr(), soff.data_ptr(),
+                        len(call_lists), smax, h_list, buf.data_ptr(), buf.numel(), ids[s:e].data_ptr(),
+                        scores[s:e].data_ptr(), counts[s:e].data_ptr(), self._stream(),
+                    )
+                )
+                keep.append((sid, soff))
+        self._keepalive = keep  # until the stream has consumed them
 
     def _host_io(self, B: int, Q: int, k: int) -> dict[str, torch.Tensor]:
         """Cached pinned + device staging buffers of the host-buffer path."""

@@ -586,12 +586,12 @@ class FastPlaid:
             out.extend(f.result())
         return out
 
-    def _search_exhaustive_device(self, idx: DeviceIndex, queries: torch.Tensor,
-                                  top_k: int) -> list[list[tuple[int, float]]]:
+    def _search_exhaustive_device(self, idx: DeviceIndex, queries: torch.Tensor, top_k: int,
+                                  subset: list[list[int]] | None = None) -> list[list[tuple[int, float]]]:
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         q16 = queries.to(device=idx.device, dtype=torch.float16)  # the fp16 cast of `search` (fast_plaid.py:241)
-        ids, scores, counts = idx.search_exhaustive(q16, top_k)
+        ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
     @torch.inference_mode()
@@ -599,6 +599,7 @@ class FastPlaid:
         self,
         queries_embeddings: torch.Tensor | list[torch.Tensor],
         top_k: int = 10,
+        subset: list[list[int]] | list[int] | None = None,
     ) -> list[list[tuple[int, float]]]:
         """Exact search: score EVERY document with the exact MaxSim formula of the re-rank stage and return,
         per query, the ``top_k`` best ``(doc_id, score)`` pairs in rank order (score desc, then id asc).
@@ -606,6 +607,14 @@ class FastPlaid:
         No centroid probing and no pruning, so there is no recall loss and no knob to tune; the cost grows
         with the number of documents (see README for measured times).  Works on ``compress_only`` indexes.
         Queries take the forms ``search`` accepts.  ``top_k`` <= 4096.
+
+        ``subset`` restricts each query to a set of documents, in the forms ``search`` accepts: one id, one id list
+        for every query (e.g. the result of ``filtering.where``), or one list per query (e.g. first-stage candidates
+        to re-rank); ``None`` or ``[]`` means no restriction.  Order and duplicates do not matter and unknown ids are
+        ignored.  A query then gets the ``min(top_k, #documents)`` best of its set, each with the score the
+        unrestricted search gives that document: restricting to a subset is the full exhaustive ranking filtered to
+        the subset.  The cost grows with the listed documents rather than the index; queries that share a list share
+        its decode.
 
         A score sums the per-query-token fp16 maxima exactly and rounds once to fp32; ``search`` keeps an fp32
         running sum.  The two agree whenever that running sum is exact (the usual case); otherwise the same
@@ -616,16 +625,17 @@ class FastPlaid:
                 "search_exhaustive on a document-sharded index is not implemented: each rank holds only its "
                 "document range, and the per-shard top-k lists would need a merge across ranks"
             )
-        search_indices, queries, _ = self._prepare_search(queries_embeddings, None)
+        search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
         if len(self.devices) == 1:
-            return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k)
+            return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k, subset)
         # several devices in ONE process hold replicas: the query list is split across them, like `search`
         n = len(self.devices)
         chunk = math.ceil(queries.shape[0] / n)
         chunks = list(torch.split(queries, chunk))
+        sub_chunks = [None] * len(chunks) if subset is None else [subset[i : i + chunk] for i in range(0, len(subset), chunk)]
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
-                ex.submit(self._search_exhaustive_device, search_indices[d], chunks[i], top_k)
+                ex.submit(self._search_exhaustive_device, search_indices[d], chunks[i], top_k, sub_chunks[i])
                 for i, d in enumerate(self.devices)
                 if i < len(chunks)
             ]

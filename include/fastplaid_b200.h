@@ -322,6 +322,31 @@ int fpb_search_exhaustive(const fpb_index* index, const void* d_queries, int B, 
                           size_t workspace_bytes, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
                           void* stream);
 
+/* Exhaustive exact search over document lists: query b is scored against the documents of list h_query_list[b]
+ * only (filtered exact search, exact re-ranking of a candidate list).  Queries that share a list share one decode
+ * of each of its documents.
+ *   d_list_ids      i32 [total]  GLOBAL doc ids, list l owns [d_list_offsets[l], d_list_offsets[l+1]); any order,
+ *                                duplicates count once, ids outside [doc_id_base, doc_id_base + n_docs) are ignored
+ *                                (the convention of fpb_search_batch_subset)
+ *   d_list_offsets  i64 [n_lists + 1]
+ *   max_list_len    at least the length of every list (it sizes the workspace: min(n_docs, max_list_len) positions
+ *                   per list; like max_subset_len)
+ *   h_query_list    HOST i32 [B], the list of every query, each in [0, n_lists); read during the call only
+ * Outputs as fpb_search_exhaustive, over the SET of valid documents of the query's list: global ids in rank order
+ * (score desc, then id asc), d_out_counts[b] = min(top_k, set size) (0 for an empty list), tails id -1 / score -inf.
+ * Every score is bit-identical to fpb_exhaustive_scores' score of the same document: the same decoder, MMA sequence
+ * and exact sum.  The result does not depend on how queries are grouped into lists or on how a batch is split.
+ * Limits as fpb_exhaustive_workspace_bytes (1 <= top_k <= 4096, Q <= 256); 1 <= n_lists <= 65535.  The arguments
+ * are checked in the order shapes, lists, index.  fpb_exhaustive_subset_workspace_bytes: the workspace (256-byte
+ * aligned) of a call with these shapes and lists. */
+int fpb_exhaustive_subset_workspace_bytes(const fpb_index* index, int B, int Q, int top_k, int n_lists,
+                                          int64_t max_list_len, size_t* out);
+int fpb_search_exhaustive_subset(const fpb_index* index, const void* d_queries, int B, int Q, int top_k,
+                                 const int32_t* d_list_ids, const int64_t* d_list_offsets, int n_lists,
+                                 int64_t max_list_len, const int32_t* h_query_list, void* d_workspace,
+                                 size_t workspace_bytes, int64_t* d_out_ids, float* d_out_scores,
+                                 int32_t* d_out_counts, void* stream);
+
 /* ---- by-products of the MaxSim kernel ("next" rows of SURVEY.md 8f-3) ---- */
 /* reconstruct_embeddings (rust/utils/embeddings.rs:12-69): decompressed, normalised
  * fp16 rows of the given local docs, concatenated.  d_out: f16 [sum(len), dim]. */
