@@ -25,6 +25,8 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include <cooperative_groups.h>
+
 #include "kernels.h"
 #include "select.cuh"
 
@@ -32,15 +34,30 @@ namespace {
 
 constexpr int64_t K3_TWO_PASS_MIN_TOKENS = 200000000;  // B * index tokens below which one pass is used by default
 constexpr int K3_THREADS = 256;
-constexpr int K3_DOCS_PER_CHUNK = 64;    // exact pass: work-queue granule
-constexpr int K3A_DOCS_PER_CHUNK = 128;  // bound pass
+constexpr int K3A_DOCS_PER_CHUNK = 128;  // bound pass: documents per chunk
+// exact pass: documents per chunk, at most (the one-pass mode's granule), and the most queries' refine lists the
+// resident CTAs' chunks may span (k3_prefix_kernel).  Smaller chunks only where the lists are short: on clustered
+// corpora, whose long lists gather few distinct rows, chunks below 64 only add queue overhead.
+constexpr int K3_EXACT_MAX_DOCS = 64;
+constexpr int K3_EXACT_QUERIES_IN_FLIGHT = 4;
 // bound pass: per-warp ring of high codes waiting for their gather (a power of two >= one group + one batch)
 constexpr int K3_WQ_FOR(int W, int FLUSH) { int n = 64; while (n < 32 * W + FLUSH) n <<= 1; return n; }
 
-// chunk prefix of the dynamic work queue: work[b] = first chunk of query b, work[B] = total, work[B+1] = counter
-__global__ void k3_prefix_kernel(const int32_t* __restrict__ n_items, int B, int per_chunk,
+// chunk prefix of the dynamic work queue: work[b] = first chunk of query b, work[B] = total, work[B+1] = counter,
+// work[B+2] = documents per chunk.  per_chunk > 0 fixes the granule (the bound pass, the one-pass mode).  per_chunk = 0
+// sizes it for the exact pass's refine lists (`ctas` CTAs resident): the chunks are taken in query order, so the resident CTAs cover about
+// K3_EXACT_QUERIES_IN_FLIGHT queries' documents and what they gather of S stays in L2.  It is a multiple of the warps
+// per CTA, from one document per warp up to K3_EXACT_MAX_DOCS.  pin (such a multiple, 0 = none) overrides it.
+__global__ void k3_prefix_kernel(const int32_t* __restrict__ n_items, int B, int per_chunk, int ctas, int pin,
                                  int32_t* __restrict__ work) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
+    if (per_chunk <= 0) {
+      constexpr int WARPS = K3_THREADS / 32;
+      int64_t total = 0;
+      for (int b = 0; b < B; ++b) total += n_items[b];
+      const int64_t g = K3_EXACT_QUERIES_IN_FLIGHT * total / (int64_t(B) * ctas) / WARPS * WARPS;
+      per_chunk = pin > 0 ? pin : int(g < WARPS ? WARPS : (g > K3_EXACT_MAX_DOCS ? K3_EXACT_MAX_DOCS : g));
+    }
     int acc = 0;
     for (int b = 0; b < B; ++b) {
       work[b] = acc;
@@ -48,6 +65,7 @@ __global__ void k3_prefix_kernel(const int32_t* __restrict__ n_items, int B, int
     }
     work[B] = acc;
     work[B + 1] = 0;
+    work[B + 2] = per_chunk;
   }
 }
 
@@ -239,7 +257,9 @@ __device__ __forceinline__ void load_codes(int (&c)[LPR], const int32_t* p) {
   }
 }
 
-template <int LPR>
+// LIST: the refine-list walk, documents per chunk from work[B+2]; otherwise the one-pass mode over every candidate in
+// chunks of K3_EXACT_MAX_DOCS (a compile-time constant, as the one-pass walk has always been built)
+template <int LPR, bool LIST>
 __global__ void __launch_bounds__(K3_THREADS, K3_EXACT_MINB)
 k3_exact_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* __restrict__ doc_offsets,
                 const int32_t* __restrict__ walk_codes, const int64_t* __restrict__ walk_win,
@@ -256,21 +276,22 @@ k3_exact_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
   const int Ki = int(K);
   const K3Cols empty = K3Cols::empty();
   unsigned long long rows = 0;
+  const int per_chunk = LIST ? work[B + 2] : K3_EXACT_MAX_DOCS;
 
   for (;;) {
     k3_next_chunk(work, B, &s_b, &s_c);
     const int b = s_b;
     if (b < 0) break;
-    const int n = list ? n_list[b] : n_cand[b];
+    const int n = LIST ? n_list[b] : n_cand[b];
     const uint4* Sb = reinterpret_cast<const uint4*>(S + int64_t(b) * K * QP) + sub;
     const int32_t* cb = cand + int64_t(b) * cand_cap;
-    const int32_t* lb = list ? list + int64_t(b) * cand_cap : nullptr;
+    const int32_t* lb = LIST ? list + int64_t(b) * cand_cap : nullptr;
     float* ab = approx + int64_t(b) * cand_cap;
 
-    for (int i = 0; i < K3_DOCS_PER_CHUNK / (K3_THREADS / 32); ++i) {
-      const int j = s_c * K3_DOCS_PER_CHUNK + i * (K3_THREADS / 32) + warp;
+    for (int i = 0; i < per_chunk / (K3_THREADS / 32); ++i) {
+      const int j = s_c * per_chunk + i * (K3_THREADS / 32) + warp;
       if (j >= n) break;
-      const int idx = lb ? lb[j] : j;
+      const int idx = LIST ? lb[j] : j;
       const int d = cb[idx];
       const int64_t o0 = doc_offsets[d];
       const int len = int(doc_offsets[d + 1] - o0);
@@ -742,26 +763,61 @@ k3_bound_kernel(const __half* __restrict__ S, int64_t K, int Q, const int64_t* _
 
 // step 4: per query the pruning threshold T (at least n_dec candidates have lb >= T; found with two levels of
 // 2048 value buckets, so outliers only cost resolution) and the list of unresolved candidates with ub >= T.
-__global__ void __launch_bounds__(1024)
+// One cluster of K3_REFINE_CTAS CTAs per query (one CTA per query would leave half of the GPU idle), each over its
+// own slice of the candidates.  The minimum and maximum, the two histograms and the smallest selected value are
+// merged through distributed shared memory: integer counts, minima and maxima do not depend on how the candidates are
+// split, so every CTA finds the buckets and the T that one CTA over all of them would.  The list is compacted through
+// a counter in the first CTA's shared memory: the set is the same, only its order depends on the schedule.
+constexpr int K3_REFINE_CTAS = 4;
+
+__global__ void __cluster_dims__(K3_REFINE_CTAS, 1, 1) __launch_bounds__(1024, 2)
 k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb, int cand_cap,
                       const int32_t* __restrict__ n_cand, int n_dec, int refine_all, int32_t* __restrict__ list,
                       int32_t* __restrict__ n_list, float* __restrict__ thresh) {
-  __shared__ int hist[SEL_BINS];
+  namespace cg = cooperative_groups;
+  const cg::cluster_group cluster = cg::this_cluster();
+  __shared__ int hist[SEL_BINS];  // this CTA's counts
+  __shared__ int hsum[SEL_BINS];  // the cluster's
   __shared__ float s_red[64];
+  __shared__ float s_part[3];     // this CTA's minimum, maximum and smallest selected value
   __shared__ int s_t, s_need, s_cnt;
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+  const int rank = int(cluster.block_rank());
+  const int b = blockIdx.x / K3_REFINE_CTAS, tid = threadIdx.x, lane = tid & 31;
   const int n = n_cand[b];
+  const int per = (n + K3_REFINE_CTAS - 1) / K3_REFINE_CTAS;
+  const int lo = min(n, rank * per), hi = min(n, lo + per);  // this CTA's slice
   const float* ubb = ub + int64_t(b) * cand_cap;
   const float* lbb = lb + int64_t(b) * cand_cap;
   int32_t* out = list + int64_t(b) * cand_cap;
   constexpr int FV = 8;
+  if (tid == 0) s_cnt = 0;
+  // hsum = the sum of the cluster's hist; afterwards every CTA may clear its hist again
+  auto merge_hist = [&]() {
+    cluster.sync();
+    for (int i = tid; i < SEL_BINS; i += 1024) {
+      int c = 0;
+#pragma unroll
+      for (int r = 0; r < K3_REFINE_CTAS; ++r) c += cluster.map_shared_rank(hist, r)[i];
+      hsum[i] = c;
+    }
+    cluster.sync();
+  };
+  // the minimum (or maximum) of s_part[k] over the cluster, folded into v
+  auto merge_part = [&](int k, float v, bool is_max) {
+#pragma unroll
+    for (int r = 0; r < K3_REFINE_CTAS; ++r) {
+      const float x = cluster.map_shared_rank(s_part, r)[k];
+      v = is_max ? fmaxf(v, x) : fminf(v, x);
+    }
+    return v;
+  };
   float T = -INFINITY;
   if (!refine_all && n > n_dec) {  // n <= n_dec: nothing is pruned (search.rs:605 / :615), every score is needed
     float mn = INFINITY, mx = -INFINITY;
-    for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
+    for (int i0 = lo + tid; i0 < hi; i0 += 1024 * FV) {
       float v[FV];
 #pragma unroll
-      for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? lbb[i0 + u * 1024] : NAN;  // fmin/fmax skip NaN
+      for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < hi) ? lbb[i0 + u * 1024] : NAN;  // fmin/fmax skip NaN
 #pragma unroll
       for (int u = 0; u < FV; ++u) {
         mn = fminf(mn, v[u]);
@@ -769,23 +825,30 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
       }
     }
     block_min_max(mn, mx, s_red);
+    if (tid == 0) {
+      s_part[0] = mn;
+      s_part[1] = mx;
+    }
+    cluster.sync();
+    mn = merge_part(0, mn, false);
+    mx = merge_part(1, mx, true);
     const float range = mx - mn;
     if (range > 0.f && range < 3.0e38f) {
       // level 1: 2048 buckets over [mn, mx]
       const float scale1 = float(SEL_BINS - 1) / range;
       for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
       __syncthreads();
-      for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
+      for (int i0 = lo + tid; i0 < hi; i0 += 1024 * FV) {
         float v[FV];
 #pragma unroll
-        for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? lbb[i0 + u * 1024] : 0.f;
+        for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < hi) ? lbb[i0 + u * 1024] : 0.f;
 #pragma unroll
         for (int u = 0; u < FV; ++u)
-          if (i0 + u * 1024 < n && v[u] == v[u]) atomicAdd(&hist[value_bucket(v[u], mn, scale1)], 1);
+          if (i0 + u * 1024 < hi && v[u] == v[u]) atomicAdd(&hist[value_bucket(v[u], mn, scale1)], 1);
       }
       if (tid == 0) s_t = -1;
-      __syncthreads();
-      if (tid < 32) warp_find_bucket(hist, SEL_BINS, n_dec, &s_t, &s_need);
+      merge_hist();
+      if (tid < 32) warp_find_bucket(hsum, SEL_BINS, n_dec, &s_t, &s_need);
       __syncthreads();
       const int t1 = s_t, need1 = s_need;
       __syncthreads();
@@ -795,27 +858,27 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
         const float scale2 = float(SEL_BINS - 1) * scale1;
         for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
         __syncthreads();
-        for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
+        for (int i0 = lo + tid; i0 < hi; i0 += 1024 * FV) {
           float v[FV];
 #pragma unroll
-          for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? lbb[i0 + u * 1024] : 0.f;
+          for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < hi) ? lbb[i0 + u * 1024] : 0.f;
 #pragma unroll
           for (int u = 0; u < FV; ++u)
-            if (i0 + u * 1024 < n && v[u] == v[u] && value_bucket(v[u], mn, scale1) == t1)
+            if (i0 + u * 1024 < hi && v[u] == v[u] && value_bucket(v[u], mn, scale1) == t1)
               atomicAdd(&hist[value_bucket(v[u], lo1, scale2)], 1);
         }
         if (tid == 0) s_t = -1;
-        __syncthreads();
-        if (tid < 32) warp_find_bucket(hist, SEL_BINS, need1, &s_t, &s_need);
+        merge_hist();
+        if (tid < 32) warp_find_bucket(hsum, SEL_BINS, need1, &s_t, &s_need);
         __syncthreads();
         const int t2 = s_t;
         // T = the smallest value of the selected upper set {b1 > t1} u {b1 == t1, b2 >= t2}: it holds >= n_dec values
         float tmin = INFINITY;
         if (t2 >= 0) {
-          for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
+          for (int i0 = lo + tid; i0 < hi; i0 += 1024 * FV) {
             float v[FV];
 #pragma unroll
-            for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? lbb[i0 + u * 1024] : NAN;
+            for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < hi) ? lbb[i0 + u * 1024] : NAN;
 #pragma unroll
             for (int u = 0; u < FV; ++u) {
               if (v[u] == v[u]) {
@@ -833,42 +896,63 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
         tmin = s_red[lane];
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) tmin = fminf(tmin, __shfl_xor_sync(0xffffffffu, tmin, off));
+        if (tid == 0) s_part[2] = tmin;
+        cluster.sync();
+        tmin = merge_part(2, tmin, false);
         if (t2 >= 0 && tmin < INFINITY) T = tmin;
       }
     } else if (range == 0.f) {
       T = mn;  // every lower bound is the same value: all n > n_dec candidates have lb >= mn
     }
   }
-  if (tid == 0) s_cnt = 0;
-  __syncthreads();
-  const int n_up = (n + 1023) / 1024 * 1024;
-  for (int i = tid; i < n_up; i += 1024) {
+  cluster.sync();  // the first CTA's counter is zero
+  int* cnt = cluster.map_shared_rank(&s_cnt, 0);
+  const int hi_up = lo + (hi - lo + 1023) / 1024 * 1024;
+  for (int i = lo + tid; i < hi_up; i += 1024) {
     bool take = false;
-    if (i < n) {
+    if (i < hi) {
       const float u = ubb[i], l = lbb[i];
       take = (l < u) && (u >= T);
     }
     const unsigned m = __ballot_sync(0xffffffffu, take);
     int base = 0;
-    if (lane == 0 && m) base = atomicAdd(&s_cnt, __popc(m));
+    if (lane == 0 && m) base = atomicAdd(cnt, __popc(m));
     base = __shfl_sync(0xffffffffu, base, 0);
     if (take) out[base + __popc(m & ((1u << lane) - 1u))] = i;
   }
-  __syncthreads();
-  if (tid == 0) {
+  cluster.sync();  // every CTA's count is in
+  if (rank == 0 && tid == 0) {
     n_list[b] = s_cnt;
     thresh[b] = T;
   }
 }
 
-// exact scoring of `list` (NULL: every candidate) into approx
+// exact scoring of `list` (NULL: every candidate) into approx: the work queue over the list lengths (n_cand and
+// K3_EXACT_MAX_DOCS documents per chunk without a list), then the kernel.  FPB_K3_EXACT_DOCS_PER_CHUNK=n (a multiple
+// of the 8 warps of a CTA, up to K3_EXACT_MAX_DOCS) pins the documents per chunk of the refine-list walk; the scores do not depend on it, and the tests
+// use it.  Read at every launch.
 template <int LPR>
 int launch_k3_exact(const fpb_index* ix, const Ws& ws, const int32_t* list, const int32_t* n_list, int32_t* work,
                     cudaStream_t st) {
   const fpb_layout& L = *ws.L;
-  k3_exact_kernel<LPR><<<ix->sm_count * 8, K3_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes,
-                                                                 ix->walk_win, ws.cand(), L.cand_cap, ws.n_cand(), list,
-                                                                 n_list, work, L.B, ws.approx(), ws.stats());
+  static int per_sm = 0;  // resident CTAs per SM: fixed by the kernel's resources, asked once per instantiation
+  if (per_sm == 0) {
+    int n = 0;
+    FPB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k3_exact_kernel<LPR, true>, K3_THREADS, 0));
+    per_sm = n < 1 ? 1 : n;
+  }
+  const char* e = getenv("FPB_K3_EXACT_DOCS_PER_CHUNK");
+  const int pin = e ? atoi(e) : 0;
+  const int pinned = pin >= 1 && pin <= K3_EXACT_MAX_DOCS && pin % (K3_THREADS / 32) == 0 ? pin : 0;
+  // the one-pass mode (no list) keeps K3_EXACT_MAX_DOCS: its candidate lists are long, and the sizing rule is
+  // measured on the refine lists only
+  k3_prefix_kernel<<<1, 32, 0, st>>>(list ? n_list : ws.n_cand(), L.B, list ? 0 : K3_EXACT_MAX_DOCS,
+                                     ix->sm_count * per_sm, pinned, work);
+  FPB_LAUNCH_CHECK("k3_prefix");
+  auto kern = list ? k3_exact_kernel<LPR, true> : k3_exact_kernel<LPR, false>;
+  kern<<<ix->sm_count * 8, K3_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes, ix->walk_win,
+                                                ws.cand(), L.cand_cap, ws.n_cand(), list, n_list, work, L.B,
+                                                ws.approx(), ws.stats());
   FPB_LAUNCH_CHECK("k3_exact");
   return FPB_OK;
 }
@@ -915,8 +999,6 @@ int launch_k3_t(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st) {
   const bool small_job = int64_t(L.B) * ix->E < K3_TWO_PASS_MIN_TOKENS;
   if ((flags & FPB_FLAG_APPROX_DIRECT) || size_t(L.hb_words) * 4 > 96 * 1024 || (!forced && small_job)) {
     FPB_CUDA_CHECK(cudaMemsetAsync(ws.n_refine(), 0, size_t(L.B) * 4, st));  // nothing was re-scored
-    k3_prefix_kernel<<<1, 32, 0, st>>>(ws.n_cand(), L.B, K3_DOCS_PER_CHUNK, ws.work());
-    FPB_LAUNCH_CHECK("k3_prefix");
     return launch_k3_exact<LPR>(ix, ws, nullptr, nullptr, ws.work(), st);
   }
   k3_tau_kernel<LPR><<<L.B, K3_TAU_THREADS, 0, st>>>(ws.S(), ix->K, L.Q, ix->doc_offsets, ix->walk_codes,
@@ -928,7 +1010,7 @@ int launch_k3_t(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st) {
     k3_hibits_kernel<LPR><<<grid, 256, 0, st>>>(ws.S(), ix->K, ws.tau(), ws.hibits(), L.hb_words);
     FPB_LAUNCH_CHECK("k3_hibits");
   }
-  k3_prefix_kernel<<<1, 32, 0, st>>>(ws.n_cand(), L.B, K3A_DOCS_PER_CHUNK, ws.work());
+  k3_prefix_kernel<<<1, 32, 0, st>>>(ws.n_cand(), L.B, K3A_DOCS_PER_CHUNK, 0, 0, ws.work());
   FPB_LAUNCH_CHECK("k3_prefix");
   {
     // windows per group: the index's choice (fpb_index::walk_group), FPB_K3_GROUP overrides it (tuning only: every
@@ -939,12 +1021,10 @@ int launch_k3_t(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st) {
                  : g == 5 ? launch_k3_bound<LPR, 5>(ix, ws, st) : launch_k3_bound<LPR, 6>(ix, ws, st);
     if (rc != FPB_OK) return rc;
   }
-  k3_refine_list_kernel<<<L.B, 1024, 0, st>>>(ws.approx(), ws.lb(), L.cand_cap, ws.n_cand(), L.R,
+  k3_refine_list_kernel<<<L.B * K3_REFINE_CTAS, 1024, 0, st>>>(ws.approx(), ws.lb(), L.cand_cap, ws.n_cand(), L.R,
                                               (flags & FPB_FLAG_APPROX_EXACT_ALL) ? 1 : 0, ws.refine(), ws.n_refine(),
                                               ws.thresh());
   FPB_LAUNCH_CHECK("k3_refine_list");
-  k3_prefix_kernel<<<1, 32, 0, st>>>(ws.n_refine(), L.B, K3_DOCS_PER_CHUNK, ws.work2());
-  FPB_LAUNCH_CHECK("k3_prefix");
   return launch_k3_exact<LPR>(ix, ws, ws.refine(), ws.n_refine(), ws.work2(), st);
 }
 
