@@ -53,6 +53,32 @@ def test_errors_are_reported_not_thrown():
     assert rc == engine.FPB_ERR_INVALID
 
 
+def test_build_kernels_refuse_what_they_do_not_encode():
+    """fpb_encode handles dim 128 with nbits 2 or 4 and the k-means kernels dim 128; the refusal comes before any
+    CUDA call.  Zero tokens or points is a no-op that succeeds and writes nothing (host buffers stand in for device
+    ones: they are never touched)."""
+    lib = engine.load_library()
+    for nbits, dim in ((4, 64), (2, 96), (3, 128), (8, 128)):
+        rc = lib.fpb_encode(0, nbits, dim, 16, None, None, 10, None, None, None, None)
+        assert rc == engine.FPB_ERR_UNSUPPORTED, (nbits, dim)
+        assert b"dim=128 with nbits 2 or 4" in lib.fpb_last_error()
+    assert lib.fpb_kmeans_assign(0, 64, 16, None, None, None, 10, None, None) == engine.FPB_ERR_UNSUPPORTED
+    assert b"dim=128" in lib.fpb_last_error()
+    assert lib.fpb_kmeans_update(0, 256, 16, None, None, None, None, None, None) == engine.FPB_ERR_UNSUPPORTED
+    assert b"dim=128" in lib.fpb_last_error()
+    cent = torch.zeros(16, 128, dtype=torch.float16)
+    cut = torch.zeros(15)
+    codes = torch.full((4,), -7, dtype=torch.int32)
+    res = torch.full((4, 64), 0xA5, dtype=torch.uint8)
+    rc = lib.fpb_encode(0, 4, 128, 16, cent.data_ptr(), cent.data_ptr(), 0, cut.data_ptr(), codes.data_ptr(),
+                        res.data_ptr(), None)
+    assert rc == engine.FPB_OK
+    bias = torch.zeros(16)
+    rc = lib.fpb_kmeans_assign(0, 128, 16, cent.data_ptr(), bias.data_ptr(), cent.data_ptr(), 0, codes.data_ptr(), None)
+    assert rc == engine.FPB_OK
+    assert bool((codes == -7).all()) and bool((res == 0xA5).all())
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
 def test_no_cpu_fallback_without_cuda():
     from fast_plaid_b200.engine import DeviceIndex, EngineUnavailableError, IndexTensors
