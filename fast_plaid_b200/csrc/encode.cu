@@ -301,8 +301,9 @@ extern "C" int fpb_kmeans_update(int device, int dim, int64_t n_centroids, const
 extern "C" int fpb_encode(int device, int nbits, int dim, int64_t n_centroids, const void* d_centroids,
                           const void* d_tokens, int64_t n_tokens, const float* d_cutoffs, int32_t* d_codes,
                           uint8_t* d_residuals, void* stream) {
-  if (dim != 128 || (nbits != 2 && nbits != 4)) {
-    fpb_set_error("fpb_encode: this build encodes dim=128 with nbits 2 or 4 (got dim=%d nbits=%d)", dim, nbits);
+  if (dim != 128 || (nbits != 1 && nbits != 2 && nbits != 4)) {
+    fpb_set_error("fpb_encode: this build encodes dim=128 with nbits 2 or 4, and dim=128 with nbits 1 (got dim=%d nbits=%d)",
+                  dim, nbits);
     return FPB_ERR_UNSUPPORTED;
   }
   if (!d_centroids || !d_tokens || !d_cutoffs || !d_codes || !d_residuals || n_centroids < 1 || n_tokens < 0) {
@@ -321,6 +322,10 @@ extern "C" int fpb_encode(int device, int nbits, int dim, int64_t n_centroids, c
   const int pblocks = int(((total + 255) / 256) < 65535 * 16 ? ((total + 255) / 256) : 65535 * 16);
   if (nbits == 4)
     encode_pack_kernel<4><<<pblocks, 256, 0, st>>>(static_cast<const __half*>(d_tokens),
+                                                   static_cast<const __half*>(d_centroids), d_codes, d_cutoffs,
+                                                   n_tokens, dim, d_residuals);
+  else if (nbits == 1)
+    encode_pack_kernel<1><<<pblocks, 256, 0, st>>>(static_cast<const __half*>(d_tokens),
                                                    static_cast<const __half*>(d_centroids), d_codes, d_cutoffs,
                                                    n_tokens, dim, d_residuals);
   else

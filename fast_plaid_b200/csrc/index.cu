@@ -107,8 +107,14 @@ extern "C" int fpb_index_create(fpb_index** out, int device, int nbits, int dim,
     return FPB_ERR_INVALID;
   }
   *out = nullptr;
-  if (nbits != 2 && nbits != 4) {
-    fpb_set_error("unsupported nbits=%d (2 and 4 are supported)", nbits);
+  if (nbits != 1 && nbits != 2 && nbits != 4) {
+    fpb_set_error("unsupported nbits=%d (this build supports nbits 2 and 4 at dim 64 and 128, nbits 1 at dim 128)",
+                  nbits);
+    return FPB_ERR_UNSUPPORTED;
+  }
+  if (nbits == 1 && dim != 128) {
+    fpb_set_error("unsupported embedding dim=%d with nbits=1: this build supports nbits 2 and 4 at dim 64 and 128, "
+                  "nbits 1 at dim 128", dim);
     return FPB_ERR_UNSUPPORTED;
   }
   const int pd = dim * nbits / 8;

@@ -35,8 +35,7 @@ k5_maxsim_kernel(const __half* __restrict__ C, const int64_t* __restrict__ doc_o
                  const __half* __restrict__ Qpad, int Q, int B, int R, const int32_t* __restrict__ n_rerank,
                  const int32_t* __restrict__ rerank, float* __restrict__ exact) {
   constexpr int LDS = K5Smem<D, QP>::LDS;
-  constexpr int PD = D * NBITS / 8;
-  constexpr int LPT = PD / 16;
+  constexpr int LPT = lanes_per_token<D, NBITS>();
   constexpr int KS = D / 16;
   constexpr int QC = QP < 64 ? QP : 64;
   constexpr int NT = QC / 8;
@@ -147,8 +146,7 @@ k5_reconstruct_kernel(const __half* __restrict__ C, const int64_t* __restrict__ 
                       const __half* __restrict__ norms, WPerm wp,
                       const int32_t* __restrict__ doc_ids, int n, const int64_t* __restrict__ out_offsets,
                       __half* __restrict__ out) {
-  constexpr int PD = D * NBITS / 8;
-  constexpr int LPT = PD / 16;
+  constexpr int LPT = lanes_per_token<D, NBITS>();
   __shared__ uint32_t lut[512];
   Decoder<NBITS>::build(lut, wp, threadIdx.x, K5_THREADS);
   __syncthreads();
@@ -179,8 +177,7 @@ k5_token_scores_kernel(const __half* __restrict__ C, const int64_t* __restrict__
                        const int32_t* __restrict__ doc_ids, int n, int64_t max_len, __half* __restrict__ out) {
   // Simple CUDA-core formulation (this is an off-metric by-product): one token per LPT lanes,
   // the dot products are accumulated in fp32 in index order and rounded once to fp16.
-  constexpr int PD = D * NBITS / 8;
-  constexpr int LPT = PD / 16;
+  constexpr int LPT = lanes_per_token<D, NBITS>();
   constexpr int EPL = D / LPT;
   __shared__ uint32_t lut[512];
   __shared__ __align__(16) __half row[K5_THREADS / LPT][D + 8];
@@ -218,8 +215,7 @@ template <int D, int NBITS>
 __global__ void __launch_bounds__(K5_THREADS)
 k5_token_norms_kernel(const __half* __restrict__ C, const int32_t* __restrict__ codes,
                       const uint8_t* __restrict__ residuals, WPerm wp, int64_t n_tokens, __half* __restrict__ out) {
-  constexpr int PD = D * NBITS / 8;
-  constexpr int LPT = PD / 16;
+  constexpr int LPT = lanes_per_token<D, NBITS>();
   __shared__ uint32_t lut[512];
   Decoder<NBITS>::build(lut, wp, threadIdx.x, K5_THREADS);
   __syncthreads();
@@ -267,6 +263,7 @@ int launch_k5_q(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   else if ((ix)->dim == 128 && (ix)->nbits == 2) { CALL(128, 2) }       \
   else if ((ix)->dim == 64 && (ix)->nbits == 4) { CALL(64, 4) }         \
   else if ((ix)->dim == 64 && (ix)->nbits == 2) { CALL(64, 2) }         \
+  else if ((ix)->dim == 128 && (ix)->nbits == 1) { CALL(128, 1) }       \
   else {                                                                 \
     fpb_set_error("unsupported (dim=%d, nbits=%d)", (ix)->dim, (ix)->nbits); \
     return FPB_ERR_UNSUPPORTED;                                          \
@@ -287,7 +284,8 @@ int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st) {
 
 int launch_maxsim(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   // dim 128, nbits 4: Qp <= 32 -> v4 (register-resident operands, mma.sync), 32 < Qp <= 128 -> v5 (wgmma);
-  // everything else (dim 64, nbits 2, Qp = 256, documents longer than v5's pass table) -> the generic kernel here.
+  // everything else (dim 64, nbits 2 or 1, Qp = 256, documents longer than v5's pass table) -> the generic kernel
+  // here (v4 and v5 return without launching for anything but dim 128 / nbits 4).
   // FPB_K5=v1 pins the generic kernel (the A/B alternative); read at every launch, so one process can switch.
   const char* pin = getenv("FPB_K5");
   const bool generic_only = pin && pin[1] == '1';

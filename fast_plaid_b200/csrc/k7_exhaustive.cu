@@ -13,7 +13,8 @@
 //   * query rows: query b owns rows [b*Qs, b*Qs + Q) of a dense row array (Qs = Q rounded up to 16, so the 16
 //     rows of an MMA warp belong to one query); rows q >= Q are zero and are left out of the sum;
 //   * 256 threads = two warpgroups.  Both decode the tile with the generic path of the shared decoder
-//     (decode.cuh: Decoder, then ehat_chunk per 16-byte SWIZZLE_128B chunk) in v5's 8-token passes: pass p of a
+//     (decode.cuh: Decoder, then ehat_chunk per 16-byte SWIZZLE_128B chunk; at nbits 1 two lanes of 8 packed bytes
+//     per token, as at nbits 2) in v5's 8-token passes: pass p of a
 //     document is its tokens 8p..8p+7, a partial pass repeats the last token (a duplicate cannot change a
 //     maximum), passes of consecutive documents follow each other, and a document is split only where it
 //     crosses a tile boundary.  Then the 128-row A stages are cp.async-loaded one stage ahead, and
@@ -110,7 +111,8 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
                      float* __restrict__ carry_all, int* __restrict__ counter, K7Lists lst) {
   using S = K7Smem<D>;
   constexpr int PD = D * NBITS / 8;
-  constexpr int LPT = PD / 16;           // lanes per token, 16 packed bytes each
+  using Dec = Decoder<NBITS>;
+  constexpr int LPT = PD / Dec::LANE_BYTES;  // lanes per token, LANE_BYTES packed bytes each
   constexpr int EPL = D / LPT;           // elements per lane
   constexpr int NH2 = EPL / 2;
   constexpr int TPR = K7_THREADS / LPT;  // tokens per decode round
@@ -137,7 +139,7 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int c = warp >> 2, w = warp & 3, quad = lane & 3;
   float* carry = carry_all + int64_t(blockIdx.x) * n_rows;
-  Decoder<NBITS>::build(lut, wp, tid, K7_THREADS);
+  Dec::build(lut, wp, tid, K7_THREADS);
   const int64_t n_chunks = LIST ? int64_t(lst.chunk_pfx[lst.n_lists]) : (N + docs_per_chunk - 1) / docs_per_chunk;
   const int n_rb = n_rows / K7_RB;
 
@@ -251,18 +253,18 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
         const int nrow = tp * 8;
         int64_t tok[ROUNDS];
         int code[ROUNDS];
-        uint4 rv[ROUNDS];
+        typename Dec::Raw rv[ROUNDS];
 #pragma unroll
         for (int u = 0; u < ROUNDS; ++u) {  // every load of the tile in flight before the first decode
           const int r = u * TPR + tid / LPT;
           tok[u] = 0;
           code[u] = 0;
-          rv[u] = make_uint4(0u, 0u, 0u, 0u);
+          rv[u] = typename Dec::Raw{};
           if (r < nrow) {
             const int p = r >> 3;
             tok[u] = t_row[p] + min(r & 7, t_nv[p] - 1);
             code[u] = __ldg(codes + tok[u]);
-            rv[u] = ldg_nc_na(reinterpret_cast<const uint4*>(residuals + tok[u] * PD) + sub);
+            rv[u] = Dec::load(residuals + tok[u] * PD, sub);
           }
         }
 #pragma unroll
@@ -270,7 +272,7 @@ k7_exhaustive_kernel(const __half* __restrict__ C, const int64_t* __restrict__ d
           const int r = u * TPR + tid / LPT;
           if (r < nrow) {
             __half2 e[NH2];
-            Decoder<NBITS>::decode16(lut, rv[u], reinterpret_cast<const uint4*>(C + int64_t(code[u]) * D + sub * EPL), e);
+            Dec::decode(lut, rv[u], reinterpret_cast<const uint4*>(C + int64_t(code[u]) * D + sub * EPL), e);
             const float nf = __half2float(norms[tok[u]]);
             const float rc = __frcp_rn(nf);
 #pragma unroll
@@ -556,6 +558,7 @@ int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, c
   else if (ix->dim == 128 && ix->nbits == 2) rc = launch_k7_t<128, 2, K7_ALL>(ix, X, ws, dpc, st);
   else if (ix->dim == 64 && ix->nbits == 4) rc = launch_k7_t<64, 4, K7_ALL>(ix, X, ws, dpc, st);
   else if (ix->dim == 64 && ix->nbits == 2) rc = launch_k7_t<64, 2, K7_ALL>(ix, X, ws, dpc, st);
+  else if (ix->dim == 128 && ix->nbits == 1) rc = launch_k7_t<128, 1, K7_ALL>(ix, X, ws, dpc, st);
   else {
     fpb_set_error("exhaustive search: unsupported (dim=%d, nbits=%d)", ix->dim, ix->nbits);
     return FPB_ERR_UNSUPPORTED;
@@ -571,7 +574,7 @@ int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, c
 int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
                                   const int32_t* d_list_ids, const int64_t* d_list_offsets, int64_t max_list_len,
                                   cudaStream_t st) {
-  if (!((ix->dim == 128 || ix->dim == 64) && (ix->nbits == 4 || ix->nbits == 2))) {
+  if (!((ix->dim == 128 || ix->dim == 64) && (ix->nbits == 4 || ix->nbits == 2)) && !(ix->dim == 128 && ix->nbits == 1)) {
     fpb_set_error("exhaustive search: unsupported (dim=%d, nbits=%d)", ix->dim, ix->nbits);
     return FPB_ERR_UNSUPPORTED;
   }
@@ -599,7 +602,8 @@ int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* 
   if (ix->dim == 128 && ix->nbits == 4) rc = launch_k7_t<128, 4, K7_ALL, true>(ix, X, ws, dpc, st, lst);
   else if (ix->dim == 128 && ix->nbits == 2) rc = launch_k7_t<128, 2, K7_ALL, true>(ix, X, ws, dpc, st, lst);
   else if (ix->dim == 64 && ix->nbits == 4) rc = launch_k7_t<64, 4, K7_ALL, true>(ix, X, ws, dpc, st, lst);
-  else rc = launch_k7_t<64, 2, K7_ALL, true>(ix, X, ws, dpc, st, lst);
+  else if (ix->dim == 64 && ix->nbits == 2) rc = launch_k7_t<64, 2, K7_ALL, true>(ix, X, ws, dpc, st, lst);
+  else rc = launch_k7_t<128, 1, K7_ALL, true>(ix, X, ws, dpc, st, lst);
   if (rc != FPB_OK) return rc;
   // 4. the [B, cap] scores, candidates and counts of the selection
   const int64_t total = int64_t(X.B) * X.cap;

@@ -295,10 +295,13 @@ def _require_cuda() -> None:
 
 def check_supported(dim: int, nbits: int) -> None:
     """The engine's compiled limits (csrc/index.cu fpb_index_create): raise before an index is written."""
-    if int(nbits) not in (2, 4):
-        raise ValueError(f"unsupported nbits={nbits}: the engine supports nbits 2 and 4")
+    if int(nbits) not in (1, 2, 4):
+        raise ValueError(f"unsupported nbits={nbits}: the engine supports nbits 2 and 4 at dim 64 and 128, "
+                         "and nbits 1 at dim 128")
     if int(dim) not in (64, 128):
         raise ValueError(f"unsupported embedding dim={dim}: the engine supports dim 64 and 128")
+    if int(nbits) == 1 and int(dim) != 128:
+        raise ValueError(f"unsupported embedding dim={dim} with nbits=1: the engine supports nbits 1 at dim 128 only")
 
 
 def _ptr(t: torch.Tensor | None) -> int | None:

@@ -209,7 +209,7 @@ def encode(batch: torch.Tensor, centroids: torch.Tensor, centroids_t: torch.Tens
     """One batch of fp16 token rows -> (codes int64, packed residual bytes) (create.rs:404-428).
     On a CUDA device with dim = 128 this is the sm_90a encode kernel pair (wgmma argmax GEMM +
     bucketize/pack, csrc/encode.cu); otherwise dense torch ops."""
-    if batch.is_cuda and batch.shape[1] == 128 and nbits in (2, 4):
+    if batch.is_cuda and batch.shape[1] == 128 and nbits in (1, 2, 4):
         from ..engine import encode_tokens
 
         codes32, packed = encode_tokens(batch, centroids, cutoffs, nbits)

@@ -64,6 +64,10 @@ int fpb_abi_version(void);
  * The two 256-entry LUTs of the reference collapse into one (1<<nbits)-entry permuted
  * weight table w_perm[i] = bucket_weights[bitrev_nbits(i)] built here on the host.
  *
+ * Supported (dim, nbits): nbits 2 and 4 at dim 64 and 128, nbits 1 at dim 128 (16-byte residual rows).  Anything
+ * else, dim 64 with nbits 1 included, returns FPB_ERR_UNSUPPORTED before any CUDA call, with a message naming dim
+ * and nbits.
+ *
  * The handle also allocates and owns one derived device array that fpb_index_destroy frees: the approximate
  * stage's copy of the codes, each document's tokens reordered into whole 32-token windows (4 bytes per token
  * rounded up to a multiple of 32 per document, plus 8 bytes per document).
@@ -314,6 +318,7 @@ int fpb_search_batch_sharded_host(const fpb_index* index, fpb_comm* comm, int n_
  *   fpb_exhaustive_scores  d_queries f16 [B, Q, dim] (16-byte aligned), d_scores f32 [B, n_docs] (local ids)
  *   fpb_search_exhaustive  outputs as fpb_search_batch: global ids in rank order (score desc, then id asc),
  *                          d_out_counts[b] = min(top_k, n_docs), unused tail entries id -1 / score -inf
+ * Every (dim, nbits) that fpb_index_create accepts is searched, nbits 1 at dim 128 included.
  * Deterministic: the same inputs give the same bytes, whatever B and however a batch is split into calls. */
 int fpb_exhaustive_workspace_bytes(const fpb_index* index, int B, int Q, int top_k, size_t* out);
 int fpb_exhaustive_scores(const fpb_index* index, const void* d_queries, int B, int Q, void* d_workspace,
@@ -362,7 +367,9 @@ int fpb_token_scores(const fpb_index* index, const void* d_queries, int Q, const
  * residuals[t] = packed bucket indices of fp16(x_t - c[codes[t]]) against `cutoffs`
  * (bucketize right=false + LSB-first bits + big-endian packbits, create.rs:413-427, :176-184).
  *   d_tokens f16 [n_tokens, dim], d_centroids f16 [n_centroids, dim], d_cutoffs f32 [(1<<nbits)-1]
- *   d_codes i32 [n_tokens], d_residuals u8 [n_tokens, dim*nbits/8] */
+ *   d_codes i32 [n_tokens], d_residuals u8 [n_tokens, dim*nbits/8]
+ * fpb_encode takes dim 128 with nbits 1, 2 or 4 and refuses anything else with FPB_ERR_UNSUPPORTED before any
+ * CUDA call. */
 /* Host utility: round-to-nearest-even fp32 -> fp16 cast of a query batch (the cast search_on_device does
  * on the host, fast_plaid.py:241), single-threaded with F16C.  The _portable variant is the same
  * conversion in plain C, exported so the tests can compare the two. */
