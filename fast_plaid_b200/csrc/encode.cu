@@ -301,7 +301,7 @@ extern "C" int fpb_kmeans_update(int device, int dim, int64_t n_centroids, const
 extern "C" int fpb_encode(int device, int nbits, int dim, int64_t n_centroids, const void* d_centroids,
                           const void* d_tokens, int64_t n_tokens, const float* d_cutoffs, int32_t* d_codes,
                           uint8_t* d_residuals, void* stream) {
-  if (dim != 128 || (nbits != 1 && nbits != 2 && nbits != 4)) {
+  if (dim != 128 || !fpb_codec_supported(dim, nbits)) {
     fpb_set_error("fpb_encode: this build encodes dim=128 with nbits 2 or 4, and dim=128 with nbits 1 (got dim=%d nbits=%d)",
                   dim, nbits);
     return FPB_ERR_UNSUPPORTED;
@@ -320,18 +320,11 @@ extern "C" int fpb_encode(int device, int nbits, int dim, int64_t n_centroids, c
   const int pd = dim * nbits / 8;
   const int64_t total = n_tokens * pd;
   const int pblocks = int(((total + 255) / 256) < 65535 * 16 ? ((total + 255) / 256) : 65535 * 16);
-  if (nbits == 4)
-    encode_pack_kernel<4><<<pblocks, 256, 0, st>>>(static_cast<const __half*>(d_tokens),
-                                                   static_cast<const __half*>(d_centroids), d_codes, d_cutoffs,
-                                                   n_tokens, dim, d_residuals);
-  else if (nbits == 1)
-    encode_pack_kernel<1><<<pblocks, 256, 0, st>>>(static_cast<const __half*>(d_tokens),
-                                                   static_cast<const __half*>(d_centroids), d_codes, d_cutoffs,
-                                                   n_tokens, dim, d_residuals);
-  else
-    encode_pack_kernel<2><<<pblocks, 256, 0, st>>>(static_cast<const __half*>(d_tokens),
-                                                   static_cast<const __half*>(d_centroids), d_codes, d_cutoffs,
-                                                   n_tokens, dim, d_residuals);
-  FPB_LAUNCH_CHECK("encode_pack");
-  return FPB_OK;
+  return fpb_with_codec(dim, nbits, "fpb_encode", [&](auto c) {
+    encode_pack_kernel<c.NBITS><<<pblocks, 256, 0, st>>>(static_cast<const __half*>(d_tokens),
+                                                         static_cast<const __half*>(d_centroids), d_codes, d_cutoffs,
+                                                         n_tokens, dim, d_residuals);
+    FPB_LAUNCH_CHECK("encode_pack");
+    return FPB_OK;
+  });
 }

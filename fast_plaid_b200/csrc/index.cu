@@ -107,21 +107,7 @@ extern "C" int fpb_index_create(fpb_index** out, int device, int nbits, int dim,
     return FPB_ERR_INVALID;
   }
   *out = nullptr;
-  if (nbits != 1 && nbits != 2 && nbits != 4) {
-    fpb_set_error("unsupported nbits=%d (this build supports nbits 2 and 4 at dim 64 and 128, nbits 1 at dim 128)",
-                  nbits);
-    return FPB_ERR_UNSUPPORTED;
-  }
-  if (nbits == 1 && dim != 128) {
-    fpb_set_error("unsupported embedding dim=%d with nbits=1: this build supports nbits 2 and 4 at dim 64 and 128, "
-                  "nbits 1 at dim 128", dim);
-    return FPB_ERR_UNSUPPORTED;
-  }
-  const int pd = dim * nbits / 8;
-  if ((dim != 64 && dim != 128) || (pd != 16 && pd != 32 && pd != 64)) {
-    fpb_set_error("unsupported embedding dim=%d with nbits=%d: this build supports dim 64 and 128", dim, nbits);
-    return FPB_ERR_UNSUPPORTED;
-  }
+  if (!fpb_codec_supported(dim, nbits)) return fpb_codec_error("fpb_index_create", dim, nbits);
   if (n_centroids <= 0 || n_docs < 0 || !d_centroids || !d_bucket_weights || !d_doc_offsets) {
     fpb_set_error("fpb_index_create: bad sizes or NULL codec/offset pointers");
     return FPB_ERR_INVALID;
@@ -137,7 +123,7 @@ extern "C" int fpb_index_create(fpb_index** out, int device, int nbits, int dim,
   ix->device = device;
   ix->nbits = nbits;
   ix->dim = dim;
-  ix->pd = pd;
+  ix->pd = dim * nbits / 8;
   ix->K = n_centroids;
   ix->N = n_docs;
   ix->n_ivf = n_ivf;

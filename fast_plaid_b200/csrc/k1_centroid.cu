@@ -8,8 +8,6 @@
 // as the reference does.  The epilogue writes S in the [b][k][q] layout the approximate stage
 // gathers from (one contiguous Qp*2-byte row per centroid and query) and, per 128-row tile,
 // the column maxima that let K1b find the top-n cells by touching ~n tiles instead of all K.
-#include <stdlib.h>
-
 #include "kernels.h"
 #include "select.cuh"
 
@@ -291,6 +289,15 @@ int launch_k1_d(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   return launch_k1_t<D, 64>(ix, ws, st);  // Qp in {64,128,256}: 64-column chunks
 }
 
+// The K1 variant of a launch, the whole rule: the wgmma kernel (k1_centroid_v2.cu) at dim 128 and Qp <= 128 when
+// the centroid table has a TMA descriptor, unless FPB_K1=v1 pins the mma.sync kernel; the mma.sync kernel with
+// QC = min(Qp, 64) otherwise.
+enum class K1Kernel { wgmma, mma };
+K1Kernel k1_kernel(const fpb_index* ix, const fpb_layout& L) {
+  const bool wgmma = !fpb_env_is("FPB_K1", "v1") && ix->dim == 128 && L.Qp <= 128 && ix->has_tmap;
+  return wgmma ? K1Kernel::wgmma : K1Kernel::mma;
+}
+
 }  // namespace
 
 int launch_pad_queries(const fpb_index* ix, const Ws& ws, const __half* d_queries, cudaStream_t st) {
@@ -303,20 +310,8 @@ int launch_pad_queries(const fpb_index* ix, const Ws& ws, const __half* d_querie
 }
 
 int launch_centroid_scores(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
-  // FPB_K1=v1 pins the mma.sync kernel; default is the wgmma kernel where it applies.  Read at every launch.
-  const char* pin = getenv("FPB_K1");
-  if (!pin || pin[1] != '1') {
-    bool handled = false;
-    const int rc = launch_centroid_scores_v2(ix, ws, st, &handled);
-    if (rc != FPB_OK || handled) return rc;
-  }
-  switch (ix->dim) {
-    case 64: return launch_k1_d<64>(ix, ws, st);
-    case 128: return launch_k1_d<128>(ix, ws, st);
-    default:
-      fpb_set_error("centroid scoring: unsupported dim %d", ix->dim);
-      return FPB_ERR_UNSUPPORTED;
-  }
+  if (k1_kernel(ix, *ws.L) == K1Kernel::wgmma) return launch_centroid_scores_v2(ix, ws, st);
+  return fpb_with_codec(ix->dim, ix->nbits, "centroid scoring", [&](auto c) { return launch_k1_d<c.D>(ix, ws, st); });
 }
 
 int launch_probe(const fpb_index* ix, const Ws& ws, bool subset, cudaStream_t st) {

@@ -167,11 +167,9 @@ k1_centroid_v2_kernel(const __grid_constant__ CUtensorMap tmap_c, int K, const _
 
 }  // namespace
 
-int launch_centroid_scores_v2(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled) {
-  *handled = false;
+// dim 128, Qp <= 128 and a TMA descriptor: k1_centroid.cu's rule launches v2 only there
+int launch_centroid_scores_v2(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   const fpb_layout& L = *ws.L;
-  if (ix->dim != 128 || L.Qp > 128 || !ix->has_tmap) return FPB_OK;
-  *handled = true;
   // opt in on every launch: the attribute is per device and the call costs about a microsecond
   FPB_CUDA_CHECK(cudaFuncSetAttribute(k1_centroid_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G1Smem::bytes));
   const int n_ttiles = (L.B * L.Qp + 127) / 128;

@@ -23,7 +23,6 @@
 //   it cannot enter the pruned list whatever the tie rule, and K3b (which only orders by value) never
 //   selects it.  The pruned list and everything after it are bit-identical to scoring every candidate.
 #include <math.h>
-#include <stdlib.h>
 
 #include <cooperative_groups.h>
 
@@ -928,9 +927,9 @@ k3_refine_list_kernel(const float* __restrict__ ub, const float* __restrict__ lb
 }
 
 // exact scoring of `list` (NULL: every candidate) into approx: the work queue over the list lengths (n_cand and
-// K3_EXACT_MAX_DOCS documents per chunk without a list), then the kernel.  FPB_K3_EXACT_DOCS_PER_CHUNK=n (a multiple
-// of the 8 warps of a CTA, up to K3_EXACT_MAX_DOCS) pins the documents per chunk of the refine-list walk; the scores do not depend on it, and the tests
-// use it.  Read at every launch.
+// K3_EXACT_MAX_DOCS documents per chunk without a list), then the kernel.  FPB_K3_EXACT_DOCS_PER_CHUNK (kernels.h: a
+// multiple of the 8 warps of a CTA, up to K3_EXACT_MAX_DOCS) pins the documents per chunk of the refine-list walk;
+// the scores do not depend on it, and the tests use it.
 template <int LPR>
 int launch_k3_exact(const fpb_index* ix, const Ws& ws, const int32_t* list, const int32_t* n_list, int32_t* work,
                     cudaStream_t st) {
@@ -941,9 +940,8 @@ int launch_k3_exact(const fpb_index* ix, const Ws& ws, const int32_t* list, cons
     FPB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k3_exact_kernel<LPR, true>, K3_THREADS, 0));
     per_sm = n < 1 ? 1 : n;
   }
-  const char* e = getenv("FPB_K3_EXACT_DOCS_PER_CHUNK");
-  const int pin = e ? atoi(e) : 0;
-  const int pinned = pin >= 1 && pin <= K3_EXACT_MAX_DOCS && pin % (K3_THREADS / 32) == 0 ? pin : 0;
+  const int pin = fpb_env_int("FPB_K3_EXACT_DOCS_PER_CHUNK", 1, K3_EXACT_MAX_DOCS);
+  const int pinned = pin % (K3_THREADS / 32) == 0 ? pin : 0;
   // the one-pass mode (no list) keeps K3_EXACT_MAX_DOCS: its candidate lists are long, and the sizing rule is
   // measured on the refine lists only
   k3_prefix_kernel<<<1, 32, 0, st>>>(list ? n_list : ws.n_cand(), L.B, list ? 0 : K3_EXACT_MAX_DOCS,
@@ -959,11 +957,10 @@ int launch_k3_exact(const fpb_index* ix, const Ws& ws, const int32_t* list, cons
 
 // LAMBDA of k3_tau_kernel: the expected number of tokens per candidate and column at or above tau.  A document is
 // resolved when all of its Q columns are, so the useful level grows with log Q: LAMBDA = ln(Q) - 1.45 (2.0 at
-// Q = 32, 2.7 at Q = 64).  FPB_K3_LAMBDA overrides it (tuning only: every value gives the same results); it is read
-// at every launch so that one process can sweep it (tools/profile_approx.py).
+// Q = 32, 2.7 at Q = 64).  FPB_K3_LAMBDA (kernels.h) overrides it (tuning only: every value gives the same results);
+// one process can sweep it (tools/profile_approx.py).
 float k3_tau_lambda(int Q) {
-  const char* e = getenv("FPB_K3_LAMBDA");
-  const float pinned = e ? float(atof(e)) : 0.f;
+  const float pinned = fpb_env_float("FPB_K3_LAMBDA");
   const float x = pinned > 0.f ? pinned : logf(float(Q < 2 ? 2 : Q)) - 1.45f;
   return x < 0.5f ? 0.5f : (x > 64.f ? 64.f : x);
 }
@@ -1013,10 +1010,10 @@ int launch_k3_t(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st) {
   k3_prefix_kernel<<<1, 32, 0, st>>>(ws.n_cand(), L.B, K3A_DOCS_PER_CHUNK, 0, 0, ws.work());
   FPB_LAUNCH_CHECK("k3_prefix");
   {
-    // windows per group: the index's choice (fpb_index::walk_group), FPB_K3_GROUP overrides it (tuning only: every
-    // value gives the same results; read at every launch like FPB_K3_LAMBDA)
-    const char* e = getenv("FPB_K3_GROUP");
-    const int g = e ? atoi(e) : ix->walk_group;
+    // windows per group: the index's choice (fpb_index::walk_group), FPB_K3_GROUP (kernels.h) overrides it (tuning
+    // only: every value gives the same results)
+    const int pin = fpb_env_int("FPB_K3_GROUP", 4, 6);
+    const int g = pin ? pin : ix->walk_group;
     const int rc = g == 4 ? launch_k3_bound<LPR, 4>(ix, ws, st)
                  : g == 5 ? launch_k3_bound<LPR, 5>(ix, ws, st) : launch_k3_bound<LPR, 6>(ix, ws, st);
     if (rc != FPB_OK) return rc;

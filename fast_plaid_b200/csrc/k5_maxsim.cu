@@ -11,8 +11,6 @@
 // (4 B) and the centroid row (L2-resident table).
 //
 // v1 data path: mma.sync m16n8k16 (legacy tensor path) with a CTA of 4 warps per document.
-#include <stdlib.h>
-
 #include "decode.cuh"
 #include "kernels.h"
 
@@ -258,50 +256,38 @@ int launch_k5_q(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   }
 }
 
-#define FPB_DISPATCH_D_NBITS(ix, CALL)                                   \
-  if ((ix)->dim == 128 && (ix)->nbits == 4) { CALL(128, 4) }            \
-  else if ((ix)->dim == 128 && (ix)->nbits == 2) { CALL(128, 2) }       \
-  else if ((ix)->dim == 64 && (ix)->nbits == 4) { CALL(64, 4) }         \
-  else if ((ix)->dim == 64 && (ix)->nbits == 2) { CALL(64, 2) }         \
-  else if ((ix)->dim == 128 && (ix)->nbits == 1) { CALL(128, 1) }       \
-  else {                                                                 \
-    fpb_set_error("unsupported (dim=%d, nbits=%d)", (ix)->dim, (ix)->nbits); \
-    return FPB_ERR_UNSUPPORTED;                                          \
-  }
+// The K5 variant of a launch, the whole rule.  v4 and v5 decode dim 128 / nbits 4 only: v4 (register-resident
+// operands, mma.sync) takes Qp <= 32, v5 (wgmma) 32 < Qp <= 128 when a document's 8-token passes fit its pass table.
+// Everything else (other codecs, Qp = 256, an index whose longest document is empty or longer than the pass table)
+// takes the generic kernel, as does FPB_K5=v1 (the A/B alternative).
+enum class K5Kernel { generic, v4, v5 };
+K5Kernel k5_kernel(const fpb_index* ix, const fpb_layout& L) {
+  if (fpb_env_is("FPB_K5", "v1") || ix->dim != 128 || ix->nbits != 4) return K5Kernel::generic;
+  if (L.Qp <= 32) return K5Kernel::v4;
+  const int64_t passes_per_doc = (ix->max_doc_len + 7) / 8;
+  if (L.Qp <= 128 && passes_per_doc >= 1 && passes_per_doc <= V5_MAX_PASS) return K5Kernel::v5;
+  return K5Kernel::generic;
+}
 
 }  // namespace
 
 int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st) {
   const int blocks = ix->sm_count * 8;
-#define CALL(DD, NB)                                                                                               \
-  k5_token_norms_kernel<DD, NB><<<blocks, K5_THREADS, 0, st>>>(ix->centroids, ix->doc_codes, ix->doc_residuals, \
-                                                               ix->w_perm, ix->E, d_out);
-  FPB_DISPATCH_D_NBITS(ix, CALL)
-#undef CALL
-  FPB_LAUNCH_CHECK("k5_token_norms");
-  return FPB_OK;
+  return fpb_with_codec(ix->dim, ix->nbits, "token norms", [&](auto c) {
+    k5_token_norms_kernel<c.D, c.NBITS><<<blocks, K5_THREADS, 0, st>>>(ix->centroids, ix->doc_codes,
+                                                                       ix->doc_residuals, ix->w_perm, ix->E, d_out);
+    FPB_LAUNCH_CHECK("k5_token_norms");
+    return FPB_OK;
+  });
 }
 
 int launch_maxsim(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
-  // dim 128, nbits 4: Qp <= 32 -> v4 (register-resident operands, mma.sync), 32 < Qp <= 128 -> v5 (wgmma);
-  // everything else (dim 64, nbits 2 or 1, Qp = 256, documents longer than v5's pass table) -> the generic kernel
-  // here (v4 and v5 return without launching for anything but dim 128 / nbits 4).
-  // FPB_K5=v1 pins the generic kernel (the A/B alternative); read at every launch, so one process can switch.
-  const char* pin = getenv("FPB_K5");
-  const bool generic_only = pin && pin[1] == '1';
-  bool handled = false;
-  int rc = FPB_OK;
-  if (!generic_only && ws.L->Qp > 32) {
-    rc = launch_maxsim_v5(ix, ws, st, &handled);
-    if (rc != FPB_OK || handled) return rc;
+  switch (k5_kernel(ix, *ws.L)) {
+    case K5Kernel::v4: return launch_maxsim_v4(ix, ws, st);
+    case K5Kernel::v5: return launch_maxsim_v5(ix, ws, st);
+    case K5Kernel::generic: break;
   }
-  if (!generic_only) {
-    rc = launch_maxsim_v4(ix, ws, st, &handled);
-    if (rc != FPB_OK || handled) return rc;
-  }
-#define CALL(DD, NB) return launch_k5_q<DD, NB>(ix, ws, st);
-  FPB_DISPATCH_D_NBITS(ix, CALL)
-#undef CALL
+  return fpb_with_codec(ix->dim, ix->nbits, "maxsim", [&](auto c) { return launch_k5_q<c.D, c.NBITS>(ix, ws, st); });
 }
 
 extern "C" int fpb_reconstruct(const fpb_index* ix, const int32_t* d_doc_ids, int n,
@@ -313,14 +299,13 @@ extern "C" int fpb_reconstruct(const fpb_index* ix, const int32_t* d_doc_ids, in
   if (n == 0) return FPB_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int blocks = min(n, ix->sm_count * 8);
-#define CALL(DD, NB)                                                                                        \
-  k5_reconstruct_kernel<DD, NB><<<blocks, K5_THREADS, 0, st>>>(ix->centroids, ix->doc_offsets, ix->doc_codes, \
-                                                               ix->doc_residuals, ix->token_norms, ix->w_perm, d_doc_ids, n, \
-                                                               d_out_offsets, static_cast<__half*>(d_out));
-  FPB_DISPATCH_D_NBITS(ix, CALL)
-#undef CALL
-  FPB_LAUNCH_CHECK("k5_reconstruct");
-  return FPB_OK;
+  return fpb_with_codec(ix->dim, ix->nbits, "fpb_reconstruct", [&](auto c) {
+    k5_reconstruct_kernel<c.D, c.NBITS><<<blocks, K5_THREADS, 0, st>>>(
+        ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals, ix->token_norms, ix->w_perm, d_doc_ids, n,
+        d_out_offsets, static_cast<__half*>(d_out));
+    FPB_LAUNCH_CHECK("k5_reconstruct");
+    return FPB_OK;
+  });
 }
 
 extern "C" int fpb_token_scores(const fpb_index* ix, const void* d_queries, int Q, const int32_t* d_query_of,
@@ -332,12 +317,11 @@ extern "C" int fpb_token_scores(const fpb_index* ix, const void* d_queries, int 
   if (n == 0) return FPB_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int blocks = min(n, ix->sm_count * 8);
-#define CALL(DD, NB)                                                                                          \
-  k5_token_scores_kernel<DD, NB><<<blocks, K5_THREADS, 0, st>>>(                                             \
-      ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals, ix->token_norms, ix->w_perm,               \
-      static_cast<const __half*>(d_queries), Q, d_query_of, d_doc_ids, n, max_len, static_cast<__half*>(d_out));
-  FPB_DISPATCH_D_NBITS(ix, CALL)
-#undef CALL
-  FPB_LAUNCH_CHECK("k5_token_scores");
-  return FPB_OK;
+  return fpb_with_codec(ix->dim, ix->nbits, "fpb_token_scores", [&](auto c) {
+    k5_token_scores_kernel<c.D, c.NBITS><<<blocks, K5_THREADS, 0, st>>>(
+        ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals, ix->token_norms, ix->w_perm,
+        static_cast<const __half*>(d_queries), Q, d_query_of, d_doc_ids, n, max_len, static_cast<__half*>(d_out));
+    FPB_LAUNCH_CHECK("k5_token_scores");
+    return FPB_OK;
+  });
 }

@@ -36,9 +36,6 @@
 // list), only the A stages that hold rows of l are streamed, a warpgroup without rows of l runs no MMA, and a row
 // counts only when its query searches l.  Decoder, MMA sequence and fixed-point sum are those of the full scan, so
 // every score is bit-identical to the full scan's score of the same document.
-#include <stdlib.h>
-#include <string.h>
-
 #include "decode.cuh"
 #include "kernels.h"
 #include "wgmma.cuh"
@@ -499,16 +496,22 @@ k7_list_chunks_kernel(const int32_t* __restrict__ count, ExListTable t, int n_li
 }
 
 // documents per chunk: as many as one warp scans, fewer (down to 4, as in v5) when that leaves too few chunks of
-// `n_docs` documents to balance the SMs.  FPB_K7_DOCS_PER_CHUNK=n (1..32) pins it: the result does not depend on it,
-// and the tests use it to run the multi-document chunk walk on small indexes.
+// `n_docs` documents to balance the SMs.  FPB_K7_DOCS_PER_CHUNK (kernels.h) pins it: the result does not depend on
+// it, and the tests use it to run the multi-document chunk walk on small indexes.
 int k7_docs_per_chunk(const fpb_index* ix, int64_t n_docs) {
+  if (const int pin = fpb_env_int("FPB_K7_DOCS_PER_CHUNK", 1, K7_MAX_DOCS)) return pin;
   int dpc = K7_MAX_DOCS;
   while (dpc > 4 && (n_docs + dpc - 1) / dpc < int64_t(ix->sm_count) * 8) dpc >>= 1;
-  if (const char* pin = getenv("FPB_K7_DOCS_PER_CHUNK")) {
-    const int v = atoi(pin);
-    if (v >= 1 && v <= K7_MAX_DOCS) dpc = v;
-  }
   return dpc;
+}
+
+// The K7 variant of a full scan, the whole rule: the timing variant FPB_K7=mma|decode asks for at dim 128 / nbits 4,
+// the product (K7_ALL) otherwise.
+K7Part k7_part(const fpb_index* ix) {
+  if (ix->dim != 128 || ix->nbits != 4) return K7_ALL;
+  if (fpb_env_is("FPB_K7", "mma")) return K7_MMA_ONLY;
+  if (fpb_env_is("FPB_K7", "decode")) return K7_DECODE_ONLY;
+  return K7_ALL;
 }
 
 template <int D, int NBITS, int PART, bool LIST = false>
@@ -547,23 +550,15 @@ int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, c
   FPB_LAUNCH_CHECK("k7_pack_rows");
   FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_acc, 0, size_t(X.B) * ix->N * 8, st));
   FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_counter, 0, sizeof(int), st));
-  // FPB_K7=mma | decode: timing variants of dim 128 / nbits 4 (their scores are meaningless)
-  const char* part = getenv("FPB_K7");
-  const bool mma_only = part && strcmp(part, "mma") == 0, decode_only = part && strcmp(part, "decode") == 0;
+  const K7Part part = k7_part(ix);
   const int dpc = k7_docs_per_chunk(ix, ix->N);
-  int rc;
-  if (ix->dim == 128 && ix->nbits == 4 && mma_only) rc = launch_k7_t<128, 4, K7_MMA_ONLY>(ix, X, ws, dpc, st);
-  else if (ix->dim == 128 && ix->nbits == 4 && decode_only) rc = launch_k7_t<128, 4, K7_DECODE_ONLY>(ix, X, ws, dpc, st);
-  else if (ix->dim == 128 && ix->nbits == 4) rc = launch_k7_t<128, 4, K7_ALL>(ix, X, ws, dpc, st);
-  else if (ix->dim == 128 && ix->nbits == 2) rc = launch_k7_t<128, 2, K7_ALL>(ix, X, ws, dpc, st);
-  else if (ix->dim == 64 && ix->nbits == 4) rc = launch_k7_t<64, 4, K7_ALL>(ix, X, ws, dpc, st);
-  else if (ix->dim == 64 && ix->nbits == 2) rc = launch_k7_t<64, 2, K7_ALL>(ix, X, ws, dpc, st);
-  else if (ix->dim == 128 && ix->nbits == 1) rc = launch_k7_t<128, 1, K7_ALL>(ix, X, ws, dpc, st);
-  else {
-    fpb_set_error("exhaustive search: unsupported (dim=%d, nbits=%d)", ix->dim, ix->nbits);
-    return FPB_ERR_UNSUPPORTED;
-  }
-  if (rc != FPB_OK) return rc;
+  FPB_TRY(fpb_with_codec(ix->dim, ix->nbits, "exhaustive search", [&](auto c) {
+    if constexpr (c.D == 128 && c.NBITS == 4) {  // the timing variants exist at this codec only
+      if (part == K7_MMA_ONLY) return launch_k7_t<128, 4, K7_MMA_ONLY>(ix, X, ws, dpc, st);
+      if (part == K7_DECODE_ONLY) return launch_k7_t<128, 4, K7_DECODE_ONLY>(ix, X, ws, dpc, st);
+    }
+    return launch_k7_t<c.D, c.NBITS, K7_ALL>(ix, X, ws, dpc, st);
+  }));
   const int64_t total = int64_t(X.B) * ix->N;
   k7_finalize_kernel<<<finalize_blocks(ix, total), 256, 0, st>>>(
       reinterpret_cast<const unsigned long long*>(ws + X.off_acc), ix->doc_offsets, ix->N, total, X.Q, d_scores);
@@ -574,10 +569,6 @@ int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, c
 int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
                                   const int32_t* d_list_ids, const int64_t* d_list_offsets, int64_t max_list_len,
                                   cudaStream_t st) {
-  if (!((ix->dim == 128 || ix->dim == 64) && (ix->nbits == 4 || ix->nbits == 2)) && !(ix->dim == 128 && ix->nbits == 1)) {
-    fpb_set_error("exhaustive search: unsupported (dim=%d, nbits=%d)", ix->dim, ix->nbits);
-    return FPB_ERR_UNSUPPORTED;
-  }
   const ExListTable t = ExListTable::at(reinterpret_cast<int32_t*>(ws + X.off_table), X.n_lists, X.B, X.n_rows);
   int32_t* ids = reinterpret_cast<int32_t*>(ws + X.off_lists);
   int32_t* count = reinterpret_cast<int32_t*>(ws + X.off_lcount);
@@ -598,13 +589,8 @@ int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* 
   FPB_CUDA_CHECK(cudaMemsetAsync(ws + X.off_counter, 0, sizeof(int), st));
   // 3. K7 over the lists
   const K7Lists lst{ids, count, chunk_pfx, t, X.n_lists};
-  int rc;
-  if (ix->dim == 128 && ix->nbits == 4) rc = launch_k7_t<128, 4, K7_ALL, true>(ix, X, ws, dpc, st, lst);
-  else if (ix->dim == 128 && ix->nbits == 2) rc = launch_k7_t<128, 2, K7_ALL, true>(ix, X, ws, dpc, st, lst);
-  else if (ix->dim == 64 && ix->nbits == 4) rc = launch_k7_t<64, 4, K7_ALL, true>(ix, X, ws, dpc, st, lst);
-  else if (ix->dim == 64 && ix->nbits == 2) rc = launch_k7_t<64, 2, K7_ALL, true>(ix, X, ws, dpc, st, lst);
-  else rc = launch_k7_t<128, 1, K7_ALL, true>(ix, X, ws, dpc, st, lst);
-  if (rc != FPB_OK) return rc;
+  FPB_TRY(fpb_with_codec(ix->dim, ix->nbits, "exhaustive search",
+                         [&](auto c) { return launch_k7_t<c.D, c.NBITS, K7_ALL, true>(ix, X, ws, dpc, st, lst); }));
   // 4. the [B, cap] scores, candidates and counts of the selection
   const int64_t total = int64_t(X.B) * X.cap;
   k7_list_finalize_kernel<<<finalize_blocks(ix, total), 256, 0, st>>>(

@@ -1,6 +1,78 @@
 // Internal launchers (one per pipeline stage).  All are asynchronous on `stream`.
 #pragma once
+#include <stdlib.h>
+#include <string.h>
+
 #include "common.cuh"
+
+// ---- Residual codecs: the (dim, nbits) pairs an index may have ----------------------------------------------------
+template <int D_, int NBITS_>
+struct Codec {
+  static constexpr int D = D_, NBITS = NBITS_;
+};
+// The one list of them, nbits 2 and 4 at dim 64 and 128, nbits 1 at dim 128: f(Codec<D, NBITS>{}) for each in turn
+// until one returns true.
+template <class F>
+constexpr bool fpb_any_codec(F&& f) {
+  return f(Codec<128, 4>{}) || f(Codec<128, 2>{}) || f(Codec<64, 4>{}) || f(Codec<64, 2>{}) || f(Codec<128, 1>{});
+}
+constexpr bool fpb_codec_supported(int dim, int nbits) {
+  return fpb_any_codec([=](auto c) { return c.D == dim && c.NBITS == nbits; });
+}
+// sets the error "<who>: unsupported embedding dim=.. with nbits=..", naming the supported pairs
+inline int fpb_codec_error(const char* who, int dim, int nbits) {
+  fpb_set_error("%s: unsupported embedding dim=%d with nbits=%d: this build supports nbits 2 and 4 at dim 64 and 128, "
+                "nbits 1 at dim 128", who, dim, nbits);
+  return FPB_ERR_UNSUPPORTED;
+}
+// f(Codec<dim, nbits>{}), an FPB_* status, or the codec error.  f is instantiated at every supported pair: a launch
+// that exists at some pairs only selects them with `if constexpr`.
+template <class F>
+int fpb_with_codec(int dim, int nbits, const char* who, F&& f) {
+  int rc = FPB_OK;
+  const bool found = fpb_any_codec([&](auto c) {
+    if (c.D != dim || c.NBITS != nbits) return false;
+    rc = f(c);
+    return true;
+  });
+  return found ? rc : fpb_codec_error(who, dim, nbits);
+}
+
+// ---- Tuning pins: environment variables that pin a choice the engine otherwise makes, for A/B timing and tests ----
+// Each is read at every launch, so one process can switch.  A value not listed is ignored, as if the variable were
+// unset.  Apart from FPB_K7, none changes a result.
+//   FPB_K1=v1                      K1 on the mma.sync kernel, not wgmma
+//   FPB_K5=v1                      the generic K5, not v4 or v5
+//   FPB_K5_DOCS_PER_CHUNK=1..32    v5's documents per chunk, still capped by its pass table
+//   FPB_K7=mma|decode              K7's timing variants at dim 128 / nbits 4 (their scores are meaningless)
+//   FPB_K7_DOCS_PER_CHUNK=1..32    K7's documents per chunk
+//   FPB_K3_EXACT_DOCS_PER_CHUNK=n  the exact pass's documents per chunk of a refine list, n = 8, 16, .., 64
+//   FPB_K3_LAMBDA=x                x > 0, clamped to [0.5, 64]: the bound pass's tau level (k3_tau_lambda)
+//   FPB_K3_GROUP=4|5|6             the bound pass's windows per group, instead of fpb_index::walk_group
+inline const char* fpb_env(const char* name) {  // NULL when unset or empty
+  const char* e = getenv(name);
+  return e && *e ? e : nullptr;
+}
+inline bool fpb_env_is(const char* name, const char* value) {
+  const char* e = fpb_env(name);
+  return e && strcmp(e, value) == 0;
+}
+// the integer value of `name`; 0 when it is unset, not an integer or outside [lo, hi]
+inline int fpb_env_int(const char* name, int lo, int hi) {
+  const char* e = fpb_env(name);
+  if (!e) return 0;
+  char* end;
+  const long v = strtol(e, &end, 10);
+  return *end == '\0' && v >= lo && v <= hi ? int(v) : 0;
+}
+// the float value of `name`; 0 when it is unset or not a number
+inline float fpb_env_float(const char* name) {
+  const char* e = fpb_env(name);
+  if (!e) return 0.f;
+  char* end;
+  const float v = strtof(e, &end);
+  return *end == '\0' ? v : 0.f;
+}
 
 struct Ws {
   const fpb_layout* L;
@@ -34,7 +106,7 @@ struct Ws {
 
 int launch_pad_queries(const fpb_index* ix, const Ws& ws, const __half* d_queries, cudaStream_t st);
 int launch_centroid_scores(const fpb_index* ix, const Ws& ws, cudaStream_t st);   // K1 (dispatch)
-int launch_centroid_scores_v2(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K1 on wgmma
+int launch_centroid_scores_v2(const fpb_index* ix, const Ws& ws, cudaStream_t st);  // K1 on wgmma
 int launch_probe(const fpb_index* ix, const Ws& ws, bool subset, cudaStream_t st);       // K1b
 int launch_candidates(const fpb_index* ix, const Ws& ws, bool subset, cudaStream_t st);  // K2
 int launch_subset_mark(const fpb_index* ix, const Ws& ws, const int32_t* d_ids, const int64_t* d_offsets,
@@ -55,8 +127,10 @@ int launch_select(const float* scores, const int32_t* cand, const int32_t* n_can
                   int32_t* rerank, float* rerank_scores, int32_t* n_rerank, cudaStream_t st);
 int launch_maxsim(const fpb_index* ix, const Ws& ws, cudaStream_t st);            // K5 (dispatch)
 int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st);      // per-token fp16 norms (index load)
-int launch_maxsim_v4(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K5 v4 (register operands)
-int launch_maxsim_v5(const fpb_index* ix, const Ws& ws, cudaStream_t st, bool* handled);  // K5 v5 (wgmma, 16 decode warps)
+int launch_maxsim_v4(const fpb_index* ix, const Ws& ws, cudaStream_t st);  // K5 v4 (register operands)
+int launch_maxsim_v5(const fpb_index* ix, const Ws& ws, cudaStream_t st);  // K5 v5 (wgmma, 16 decode warps)
+// 8-token passes per v5 chunk: a document of more passes than this goes to the generic kernel
+constexpr int V5_MAX_PASS = 2048;
 // K6: per query b the top_k of the n[b] (score, id) pairs in row b of scores / ids (row stride R) in the canonical
 // order, ids offset by doc_id_base
 int launch_rank(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,

@@ -381,10 +381,14 @@ def _kernels(fn) -> str:
     (128, 4, 64, (3, 16385, 9), None, "k5_maxsim_kernel"),
     (128, 2, 64, LENGTHS, None, "k5_maxsim_kernel"),
     (64, 2, 32, LENGTHS, None, "k5_maxsim_kernel"),
+    (128, 1, 16, LENGTHS, None, "k5_maxsim_kernel"),
+    (128, 1, 64, LENGTHS, None, "k5_maxsim_kernel"),
+    (128, 1, 128, LENGTHS, None, "k5_maxsim_kernel"),
+    (128, 4, 32, LENGTHS, "", "k5_maxsim_v4_kernel"),  # only FPB_K5=v1 pins
 ])
 def test_maxsim_dispatch(dim, nbits, Q, lengths, pin, kernel, cuda_device, monkeypatch):
     """The cells above reach the kernel they are meant to test."""
-    if pin:
+    if pin is not None:
         monkeypatch.setenv("FPB_K5", pin)
     else:
         monkeypatch.delenv("FPB_K5", raising=False)
@@ -403,11 +407,12 @@ def test_maxsim_dispatch(dim, nbits, Q, lengths, pin, kernel, cuda_device, monke
     (128, 256, None, "k1_centroid_scores_kernel"),
     (128, 32, "v1", "k1_centroid_scores_kernel"),
     (64, 64, None, "k1_centroid_scores_kernel"),
+    (128, 32, "", "k1_centroid_v2_kernel"),  # only FPB_K1=v1 pins
 ])
 def test_centroid_scores_dispatch(dim, Q, pin, kernel, cuda_device, monkeypatch):
     from fast_plaid_b200.engine import DeviceIndex
 
-    if pin:
+    if pin is not None:
         monkeypatch.setenv("FPB_K1", pin)
     else:
         monkeypatch.delenv("FPB_K1", raising=False)

@@ -378,6 +378,20 @@ def test_check_supported():
         with pytest.raises(ValueError) as e:
             engine.check_supported(dim, nbits)
         assert all(w in str(e.value) for w in words), (dim, nbits, str(e.value))
+    # the Python copy of the supported set is the library's: with NULL pointers fpb_index_create refuses an unsupported
+    # pair and stops at the pointers for a supported one, both before any CUDA call
+    lib = engine.load_library()
+    handle = ctypes.c_void_p()
+    for dim in (32, 64, 96, 128, 256):
+        for nbits in (0, 1, 2, 3, 4, 8):
+            try:
+                engine.check_supported(dim, nbits)
+                refused = False
+            except ValueError:
+                refused = True
+            rc = lib.fpb_index_create(ctypes.byref(handle), 0, nbits, dim, 16, None, None, 0, None, None, None, None,
+                                      None, None, 0, 0, 0)
+            assert rc == (engine.FPB_ERR_UNSUPPORTED if refused else engine.FPB_ERR_INVALID), (dim, nbits, rc)
 
 
 def test_cabi_refuses_dim_64_at_nbits_1_before_any_cuda_call():
