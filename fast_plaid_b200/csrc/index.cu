@@ -227,8 +227,8 @@ extern "C" int fpb_workspace_layout(const fpb_index* ix, int B, int Q, const fpb
     fpb_set_error("queries with more than 256 tokens are not supported (Q=%d)", Q);
     return FPB_ERR_UNSUPPORTED;
   }
-  if (p->n_ivf_probe < 1 || p->n_ivf_probe > 32) {
-    fpb_set_error("n_ivf_probe=%d outside the supported range [1,32]", p->n_ivf_probe);
+  if (p->n_ivf_probe < 1 || p->n_ivf_probe > FPB_MAX_PROBE) {
+    fpb_set_error("n_ivf_probe=%d outside the supported range [1,%d]", p->n_ivf_probe, FPB_MAX_PROBE);
     return FPB_ERR_UNSUPPORTED;
   }
   if (p->n_full_scores < 1 || p->top_k < 1) {
@@ -261,7 +261,9 @@ extern "C" int fpb_workspace_layout(const fpb_index* ix, int B, int Q, const fpb
   L->off_queries = take(int64_t(B) * Qp * ix->dim * 2);
   L->off_S = take(int64_t(B) * ix->K * Qp * 2);
   L->off_tmax = take(int64_t(B) * Qp * L->n_tiles * 2);
-  L->off_cells = take(int64_t(B) * Q * L->n_probe * 4);
+  L->cbitmap_words = int((ix->K + 31) / 32) + 1;
+  // a wide probe's centroid bitmap follows the cells (kernels.h)
+  L->off_cells = take(fpb_align256(fpb_cells_bytes(*L)) + fpb_probe_bitmap_bytes(*L));
   L->off_bitmap = take(int64_t(B) * L->bitmap_words * 4);
   L->off_n_cand = take(int64_t(B) * 4);
   L->off_cand = take(int64_t(B) * L->cand_cap * 4);
@@ -272,7 +274,6 @@ extern "C" int fpb_workspace_layout(const fpb_index* ix, int B, int Q, const fpb
   L->off_rerank_approx = take(int64_t(B) * R * 4);
   L->off_exact = take(int64_t(B) * R * 4);
   const bool sub = (p->flags & FPB_FLAG_SUBSET) != 0;
-  L->cbitmap_words = int((ix->K + 31) / 32) + 1;
   L->off_cbitmap = take(sub ? int64_t(B) * L->cbitmap_words * 4 : 0);
   L->off_clist = take(sub ? int64_t(B) * ix->K * 4 : 0);
   L->off_n_clist = take(sub ? int64_t(B) * 4 : 0);

@@ -247,6 +247,197 @@ k1b_probe_subset_kernel(const __half* __restrict__ S, int K, int B, int Q, int Q
   }
 }
 
+// ---- wide probe (FPB_WARP_PROBE < n <= FPB_MAX_PROBE): one 1024-thread CTA per (query, query token) -------------
+// The n best keys are found by an exact threshold on the 16-bit value key (two levels of 256-bucket histograms and
+// warp_find_bucket), then every key above the threshold and the first keys at it in id order are gathered and
+// block_sort_desc puts them in rank order.  Items are visited in warp groups of 32 consecutive ones, so that a source
+// can skip a whole group by a bound on its keys (the rows of one tile by the tile maximum).
+struct WideSmem {
+  uint64_t keys[FPB_MAX_PROBE];
+  int hist[256];
+  int wsum[32];
+  int sel[2];  // threshold bucket (-1: fewer keys than needed) and the entries still to take from it
+  int n_out;
+};
+
+// The tile maxima of one S column
+struct TileItems {
+  const uint16_t* tm;
+  int n_tiles;
+  __device__ int count() const { return n_tiles; }
+  __device__ bool live(int, uint32_t) const { return true; }
+  __device__ uint32_t key(int i) const { return f16_key(tm[i]); }
+};
+// The rows of one S column; the 32-row group starting at g lies in tile g / K1_ROWS
+struct RowItems {
+  const uint16_t* col;
+  const uint16_t* tm;
+  int K, Qp;
+  __device__ int count() const { return K; }
+  __device__ bool live(int g, uint32_t floor) const { return f16_key(tm[g / K1_ROWS]) >= floor; }
+  __device__ uint32_t key(int i) const { return f16_key(col[int64_t(i) * Qp]); }
+  __device__ uint32_t id(int i) const { return uint32_t(i); }
+};
+// The rows of one S column named by an ascending centroid list
+struct ListItems {
+  const uint16_t* col;
+  const int32_t* cl;
+  int nc, Qp;
+  __device__ int count() const { return nc; }
+  __device__ bool live(int, uint32_t) const { return true; }
+  __device__ uint32_t key(int i) const { return f16_key(col[int64_t(cl[i]) * Qp]); }
+  __device__ uint32_t id(int i) const { return uint32_t(cl[i]); }
+};
+
+// f(key, i) for every item i whose key is >= floor
+template <class Items, class F>
+__device__ __forceinline__ void wide_for_each(const Items& it, uint32_t floor, F f) {
+  const int n = it.count(), lane = threadIdx.x & 31;
+  for (int g = (threadIdx.x >> 5) * 32; g < n; g += SEL_THREADS) {
+    if (!it.live(g, floor)) continue;  // warp-uniform
+    const int i = g + lane;
+    if (i < n) {
+      const uint32_t k = it.key(i);
+      if (k >= floor) f(k, i);
+    }
+  }
+}
+
+// The threshold T of the `need` (>= 1) best keys >= floor: count(key > T) < need <= count(key >= T), with
+// *rest = need - count(key > T) and *ties = count(key == T).  False, in every thread, when fewer than `need` keys
+// are >= floor.
+template <class Items>
+__device__ bool wide_threshold(const Items& it, uint32_t floor, int need, WideSmem& s, uint32_t* T, int* rest,
+                               int* ties) {
+  const int tid = threadIdx.x;
+  int hi = 0;
+  for (int level = 0; level < 2; ++level) {
+    for (int i = tid; i < 256; i += SEL_THREADS) s.hist[i] = 0;
+    if (tid == 0) s.sel[0] = -1;
+    __syncthreads();
+    if (level == 0) {
+      wide_for_each(it, floor, [&](uint32_t k, int) { atomicAdd(&s.hist[k >> 8], 1); });
+    } else {
+      wide_for_each(it, max(floor, uint32_t(hi) << 8), [&](uint32_t k, int) {
+        if (int(k >> 8) == hi) atomicAdd(&s.hist[k & 255], 1);
+      });
+    }
+    __syncthreads();
+    if (tid < 32) {
+      int t, r;
+      if (warp_find_bucket(s.hist, 256, need, &t, &r)) {
+        s.sel[0] = t;
+        s.sel[1] = r;
+      }
+    }
+    __syncthreads();
+    const int t = s.sel[0], r = s.sel[1];
+    if (t < 0) return false;
+    if (level == 0) {
+      hi = t;
+      need = r;
+    } else {
+      *T = (uint32_t(hi) << 8) | uint32_t(t);
+      *rest = r;
+      *ties = s.hist[t];
+    }
+    __syncthreads();  // everyone has read hist and sel
+  }
+  return true;
+}
+
+// s.keys[0, s.n_out) = the keys above T and the first `rest` items at T in item order (all of them when there are
+// `ties` == rest), as 64-bit rank keys.  Items must be in ascending id order.
+template <class Items>
+__device__ void wide_gather(const Items& it, uint32_t T, int rest, int ties, WideSmem& s) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) s.n_out = 0;
+  __syncthreads();
+  auto push = [&](uint32_t k, int i) { s.keys[atomicAdd(&s.n_out, 1)] = rank_key(k, it.id(i)); };
+  if (ties == rest) {
+    wide_for_each(it, T, push);
+    __syncthreads();
+    return;
+  }
+  wide_for_each(it, T + 1, push);
+  // the ties in item order: 1024-item chunks and a block-wide count of the ties before each item
+  const int n = it.count();
+  int base = 0;
+  for (int c0 = 0; c0 < n && base < rest; c0 += SEL_THREADS) {
+    const int i = c0 + tid;
+    bool tie = false;
+    if (i < n && it.live(i & ~31, T)) tie = it.key(i) == T;
+    const unsigned bal = __ballot_sync(0xffffffffu, tie);
+    __syncthreads();  // the previous chunk is done with wsum
+    if (lane == 0) s.wsum[warp] = __popc(bal);
+    __syncthreads();
+    int before = base + __popc(bal & ((1u << lane) - 1u)), total = 0;
+    for (int w = 0; w < 32; ++w) {
+      const int c = s.wsum[w];
+      if (w < warp) before += c;
+      total += c;
+    }
+    if (tie && before < rest) s.keys[atomicAdd(&s.n_out, 1)] = rank_key(T, it.id(i));
+    base += total;
+  }
+  __syncthreads();
+}
+
+// The `need` best items in s.keys[0, s.n_out) (every item >= floor when fewer), in no particular order
+template <class Items>
+__device__ void wide_select(const Items& it, uint32_t floor, int need, WideSmem& s) {
+  uint32_t T;
+  int rest, ties;
+  if (need <= 0) {
+    if (threadIdx.x == 0) s.n_out = 0;
+    __syncthreads();
+  } else if (wide_threshold(it, floor, need, s, &T, &rest, &ties)) {
+    wide_gather(it, T, rest, ties, s);
+  } else {
+    wide_gather(it, floor, 0, 0, s);
+  }
+}
+
+// out[0, n_probe) = the ids of s.keys[0, s.n_out) in rank order, then -1
+__device__ void wide_write_cells(WideSmem& s, int n_probe, int32_t* out) {
+  const int m = s.n_out;
+  int P = 1;
+  while (P < m) P <<= 1;
+  for (int i = m + threadIdx.x; i < P; i += SEL_THREADS) s.keys[i] = 0;
+  __syncthreads();
+  block_sort_desc(s.keys, P);
+  for (int i = threadIdx.x; i < n_probe; i += SEL_THREADS) out[i] = i < m ? int32_t(rank_key_id(s.keys[i])) : -1;
+}
+
+// grid B*Q.  The tile pruning of k1b_probe_kernel: tau = the n-th best tile maximum bounds the n-th best score from
+// below, so only the rows of tiles whose maximum is >= tau are read (all of them when there are fewer than n tiles).
+__global__ void __launch_bounds__(SEL_THREADS)
+k1b_probe_wide_kernel(const __half* __restrict__ S, const __half* __restrict__ tmax, int K, int Q, int Qp,
+                      int n_tiles, int n_probe, int32_t* __restrict__ cells) {
+  __shared__ WideSmem s;
+  const int b = blockIdx.x / Q, q = blockIdx.x % Q;
+  const uint16_t* tm = reinterpret_cast<const uint16_t*>(tmax) + (int64_t(b) * Qp + q) * n_tiles;
+  const uint16_t* col = reinterpret_cast<const uint16_t*>(S) + int64_t(b) * K * Qp + q;
+  uint32_t tau = 0, T;
+  int rest, ties;
+  if (wide_threshold(TileItems{tm, n_tiles}, 0u, n_probe, s, &T, &rest, &ties)) tau = T;
+  wide_select(RowItems{col, tm, K, Qp}, tau, n_probe, s);
+  wide_write_cells(s, n_probe, cells + int64_t(blockIdx.x) * n_probe);
+}
+
+// grid B*Q.  The subset probe of k1b_probe_subset_kernel: n = min(n_probe, #centroids of the subset's documents).
+__global__ void __launch_bounds__(SEL_THREADS)
+k1b_probe_subset_wide_kernel(const __half* __restrict__ S, int K, int Q, int Qp, int n_probe,
+                             const int32_t* __restrict__ clist, const int32_t* __restrict__ n_clist,
+                             int32_t* __restrict__ cells) {
+  __shared__ WideSmem s;
+  const int b = blockIdx.x / Q, q = blockIdx.x % Q;
+  const int nc = n_clist[b];
+  const uint16_t* col = reinterpret_cast<const uint16_t*>(S) + int64_t(b) * K * Qp + q;
+  wide_select(ListItems{col, clist + int64_t(b) * K, nc, Qp}, 0u, min(n_probe, nc), s);
+  wide_write_cells(s, n_probe, cells + int64_t(blockIdx.x) * n_probe);
+}
+
 __global__ void pad_queries_kernel(const __half* __restrict__ q, __half* __restrict__ out, int B, int Q,
                                    int Qp, int D) {
   const int64_t n8 = int64_t(B) * Qp * (D / 8);
@@ -316,6 +507,18 @@ int launch_centroid_scores(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
 
 int launch_probe(const fpb_index* ix, const Ws& ws, bool subset, cudaStream_t st) {
   const fpb_layout& L = *ws.L;
+  if (L.n_probe > FPB_WARP_PROBE) {
+    if (subset) {
+      k1b_probe_subset_wide_kernel<<<L.B * L.Q, SEL_THREADS, 0, st>>>(ws.S(), int(ix->K), L.Q, L.Qp, L.n_probe,
+                                                                      ws.clist(), ws.n_clist(), ws.cells());
+      FPB_LAUNCH_CHECK("k1b_probe_subset_wide");
+      return FPB_OK;
+    }
+    k1b_probe_wide_kernel<<<L.B * L.Q, SEL_THREADS, 0, st>>>(ws.S(), ws.tmax(), int(ix->K), L.Q, L.Qp, L.n_tiles,
+                                                             L.n_probe, ws.cells());
+    FPB_LAUNCH_CHECK("k1b_probe_wide");
+    return FPB_OK;
+  }
   const int warps = L.B * L.Q;
   const int blocks = (warps + 7) / 8;
   if (subset) {

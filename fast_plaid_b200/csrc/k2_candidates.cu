@@ -28,6 +28,31 @@ k2_mark_kernel(const int32_t* __restrict__ cells, int slots, const int64_t* __re
   }
 }
 
+// A wide probe (n_probe > FPB_WARP_PROBE): grid (ceil(slots / 8), B), one warp per probe slot.  The slot that sets
+// its cell's bit in the query's centroid bitmap walks the cell's IVF list; every other slot of that cell stops there.
+__global__ void __launch_bounds__(256)
+k2_mark_wide_kernel(const int32_t* __restrict__ cells, int slots, const int64_t* __restrict__ ivf_offsets,
+                    const int32_t* __restrict__ ivf_pids, uint32_t* __restrict__ cell_bitmap, int cell_words,
+                    uint32_t* __restrict__ bitmap, int bitmap_words) {
+  const int b = blockIdx.y, lane = threadIdx.x & 31;
+  const int s = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (s >= slots) return;
+  const int32_t c = cells[int64_t(b) * slots + s];
+  if (c < 0) return;
+  int first = 0;
+  if (lane == 0) {
+    const uint32_t bit = 1u << (c & 31);
+    first = (atomicOr(cell_bitmap + int64_t(b) * cell_words + (c >> 5), bit) & bit) == 0;
+  }
+  if (!__shfl_sync(0xffffffffu, first, 0)) return;
+  const int64_t o0 = ivf_offsets[c], o1 = ivf_offsets[c + 1];
+  uint32_t* bm = bitmap + int64_t(b) * bitmap_words;
+  for (int64_t i = o0 + lane; i < o1; i += 32) {
+    const int32_t pid = __ldg(ivf_pids + i);
+    atomicOr(bm + (pid >> 5), 1u << (pid & 31));
+  }
+}
+
 // one CTA per query: ordered compaction of the bitmap into cand[b][0..n_cand[b])
 __global__ void __launch_bounds__(1024)
 k2_compact_kernel(const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ mask, int bitmap_words,
@@ -183,10 +208,18 @@ int launch_candidates(const fpb_index* ix, const Ws& ws, bool subset, cudaStream
   const fpb_layout& L = *ws.L;
   FPB_CUDA_CHECK(cudaMemsetAsync(ws.bitmap(), 0, size_t(L.B) * L.bitmap_words * 4, st));
   const int slots = L.Q * L.n_probe;
-  dim3 grid(slots, L.B);
-  k2_mark_kernel<<<grid, 128, 0, st>>>(ws.cells(), slots, ix->ivf_offsets, ix->ivf_pids, ws.bitmap(),
-                                       L.bitmap_words);
-  FPB_LAUNCH_CHECK("k2_mark");
+  if (L.n_probe > FPB_WARP_PROBE) {
+    FPB_CUDA_CHECK(cudaMemsetAsync(ws.probe_bitmap(), 0, fpb_probe_bitmap_bytes(L), st));
+    dim3 grid((slots + 7) / 8, L.B);
+    k2_mark_wide_kernel<<<grid, 256, 0, st>>>(ws.cells(), slots, ix->ivf_offsets, ix->ivf_pids, ws.probe_bitmap(),
+                                              L.cbitmap_words, ws.bitmap(), L.bitmap_words);
+    FPB_LAUNCH_CHECK("k2_mark_wide");
+  } else {
+    dim3 grid(slots, L.B);
+    k2_mark_kernel<<<grid, 128, 0, st>>>(ws.cells(), slots, ix->ivf_offsets, ix->ivf_pids, ws.bitmap(),
+                                         L.bitmap_words);
+    FPB_LAUNCH_CHECK("k2_mark");
+  }
   return launch_compact(ws.bitmap(), subset ? ws.sbitmap() : nullptr, L.bitmap_words, ws.cand(), L.cand_cap,
                         ws.n_cand(), L.B, st);
 }

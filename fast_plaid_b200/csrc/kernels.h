@@ -74,6 +74,17 @@ inline float fpb_env_float(const char* name) {
   return *end == '\0' ? v : 0.f;
 }
 
+// ---- The probe: n_ivf_probe in [1, FPB_MAX_PROBE] cells per query token ------------------------------------------
+// Up to FPB_WARP_PROBE cells, K1b keeps a warp-held list and K2 drops a repeated cell by scanning the query's earlier
+// probe slots.  Above it, K1b selects block-wide and K2 drops repeats with a per-query bitmap over the centroids
+// ([B, cbitmap_words] u32), stored in the cells' region after the [B, Q, n_probe] cells.
+constexpr int FPB_WARP_PROBE = 32;
+constexpr int FPB_MAX_PROBE = 4096;
+inline int64_t fpb_cells_bytes(const fpb_layout& L) { return int64_t(L.B) * L.Q * L.n_probe * 4; }
+inline int64_t fpb_probe_bitmap_bytes(const fpb_layout& L) {
+  return L.n_probe > FPB_WARP_PROBE ? int64_t(L.B) * L.cbitmap_words * 4 : 0;
+}
+
 struct Ws {
   const fpb_layout* L;
   char* base;
@@ -81,6 +92,9 @@ struct Ws {
   __half* S() const { return reinterpret_cast<__half*>(base + L->off_S); }
   __half* tmax() const { return reinterpret_cast<__half*>(base + L->off_tmax); }
   int32_t* cells() const { return reinterpret_cast<int32_t*>(base + L->off_cells); }
+  uint32_t* probe_bitmap() const {  // n_probe > FPB_WARP_PROBE only
+    return reinterpret_cast<uint32_t*>(base + L->off_cells + fpb_align256(fpb_cells_bytes(*L)));
+  }
   uint32_t* bitmap() const { return reinterpret_cast<uint32_t*>(base + L->off_bitmap); }
   int32_t* n_cand() const { return reinterpret_cast<int32_t*>(base + L->off_n_cand); }
   int32_t* cand() const { return reinterpret_cast<int32_t*>(base + L->off_cand); }

@@ -88,7 +88,7 @@ int fpb_index_walk_layout(const fpb_index* index, int64_t* n_windows, int32_t* d
  * `batch_size` (document batch of the approximate stage) only bounds memory in the
  * reference and does not change values (search.rs:558-586); it is accepted and ignored. */
 typedef struct fpb_params {
-  int32_t n_ivf_probe;   /* search.rs:185, default 8    */
+  int32_t n_ivf_probe;   /* search.rs:185, default 8; 1..4096 (n >= K probes every centroid) */
   int32_t n_full_scores; /* search.rs:179, default 4096 */
   int32_t top_k;         /* search.rs:182               */
   int32_t batch_size;    /* search.rs:176, ignored      */
