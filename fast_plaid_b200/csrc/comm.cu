@@ -210,6 +210,69 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
   return FPB_OK;
 }
 
+// Exhaustive search on the same grid: each rank selects the top_k of its documents for the queries of its group
+// (fpb_shard_exhaustive_records), one ncclAllGather of the [b_local, top_k] records, one merge of every query.
+// The records carry approx = exact = the K7 score, so the merge's "R best by approx" with R = top_k is the global
+// top_k, and its order is the canonical one of fpb_search_exhaustive.
+extern "C" int fpb_search_exhaustive_sharded(const fpb_index* ix, fpb_comm* comm, int n_query_groups,
+                                             const void* d_queries, int B, int Q, int top_k, void* d_ws,
+                                             size_t ws_bytes, void* d_scratch, size_t scratch_bytes,
+                                             int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
+                                             void* stream) {
+  // every refusal comes before the collective and depends only on arguments every rank has in common (the
+  // workspace and the scratch are sized per rank by the caller): shapes, pointers, grid, merge limit
+  if (top_k < 1) {
+    fpb_set_error("fpb_search_exhaustive_sharded: top_k=%d must be >= 1", top_k);
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(check_exhaustive_shapes(B, Q, top_k));
+  if (n_query_groups < 1) {
+    fpb_set_error("fpb_search_exhaustive_sharded: n_query_groups=%d must be >= 1", n_query_groups);
+    return FPB_ERR_INVALID;
+  }
+  if (!ix || !comm || !d_queries || !d_ws || !d_scratch || !d_out_ids || !d_out_scores || !d_out_counts) {
+    fpb_set_error("fpb_search_exhaustive_sharded: NULL argument");
+    return FPB_ERR_INVALID;
+  }
+  if (comm->nranks % n_query_groups != 0) {
+    fpb_set_error("fpb_search_exhaustive_sharded: %d query groups do not divide %d ranks", n_query_groups,
+                  comm->nranks);
+    return FPB_ERR_INVALID;
+  }
+  const int n_shards = comm->nranks / n_query_groups;
+  const int group = comm->rank / n_shards;
+  const int b_local = (B + n_query_groups - 1) / n_query_groups;
+  const int q0 = group * b_local;
+  const int nb = B - q0 < 0 ? 0 : (B - q0 < b_local ? B - q0 : b_local);
+  FPB_TRY(check_merge_records("fpb_search_exhaustive_sharded", n_shards, top_k));
+  size_t ws_need = 0;
+  FPB_TRY(fpb_exhaustive_workspace_bytes(ix, b_local, Q, top_k, &ws_need));
+  FPB_TRY(fpb_require_bytes("workspace", int64_t(ws_need), ws_bytes));
+  FPB_TRY(fpb_require_bytes("scratch", fpb_sharded_scratch_bytes(b_local, top_k, comm->nranks), scratch_bytes));
+  FPB_TRY(fpb_require_aligned("workspace", d_ws));
+  FPB_TRY(fpb_require_aligned("scratch", d_scratch));
+  if ((reinterpret_cast<uintptr_t>(d_queries) & 15u) != 0) {
+    fpb_set_error("fpb_search_exhaustive_sharded: queries must be 16-byte aligned");
+    return FPB_ERR_INVALID;
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  FPB_CUDA_CHECK(cudaSetDevice(ix->device));
+  // the record blocks of fpb_sharded_scratch_bytes (its key blocks are not used here)
+  const int64_t per_rank = int64_t(b_local) * top_k;
+  char* sc = static_cast<char*>(d_scratch) + fpb_align256(per_rank * 8) + fpb_align256(per_rank * 8 * comm->nranks);
+  fpb_record* recs = reinterpret_cast<fpb_record*>(sc);
+  fpb_record* all_recs = reinterpret_cast<fpb_record*>(sc + fpb_align256(per_rank * 16));
+  // slots of this group that hold no query (ragged last group): record id -1 is the padding value
+  if (nb < b_local) FPB_CUDA_CHECK(cudaMemsetAsync(recs, 0xFF, size_t(per_rank) * 16, st));
+  if (nb > 0) {
+    FPB_TRY(fpb_shard_exhaustive_records(ix, static_cast<const __half*>(d_queries) + int64_t(q0) * Q * ix->dim, nb,
+                                         Q, top_k, d_ws, ws_bytes, recs, st));
+  }
+  FPB_NCCL_CHECK(nccl().AllGather(recs, all_recs, size_t(per_rank) * 16, ncclUint8, comm->comm, st));
+  FPB_TRY(launch_merge(all_recs, n_shards, b_local, B, top_k, top_k, d_out_ids, d_out_scores, d_out_counts, st));
+  return FPB_OK;
+}
+
 extern "C" int fpb_search_batch_sharded_host(const fpb_index* ix, fpb_comm* comm, int n_query_groups,
                                              const void* h_queries, int B, int Q, const fpb_params* p, void* d_ws,
                                              size_t ws_bytes, void* d_scratch, size_t scratch_bytes,

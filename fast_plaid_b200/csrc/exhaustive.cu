@@ -6,11 +6,7 @@
 
 #include "kernels.h"
 
-namespace {
-
-constexpr int EX_MAX_TOP_K = 4096;  // the k6_rank bound (one shared-memory bitonic sort per query)
-
-int check_shapes(int B, int Q, int top_k) {
+int check_exhaustive_shapes(int B, int Q, int top_k) {
   if (B <= 0 || Q <= 0 || top_k < 0) {
     fpb_set_error("exhaustive search: B=%d Q=%d top_k=%d must be positive", B, Q, top_k);
     return FPB_ERR_INVALID;
@@ -19,18 +15,20 @@ int check_shapes(int B, int Q, int top_k) {
     fpb_set_error("queries with more than 256 tokens are not supported (Q=%d)", Q);
     return FPB_ERR_UNSUPPORTED;
   }
-  if (top_k > EX_MAX_TOP_K) {
-    fpb_set_error("exhaustive search: top_k=%d exceeds the supported maximum of %d", top_k, EX_MAX_TOP_K);
+  if (top_k > FPB_EX_MAX_TOP_K) {
+    fpb_set_error("exhaustive search: top_k=%d exceeds the supported maximum of %d", top_k, FPB_EX_MAX_TOP_K);
     return FPB_ERR_UNSUPPORTED;
   }
   return FPB_OK;
 }
 
+namespace {
+
 // n_lists = 0: the full scan.  n_lists > 0: a list walk over lists of at most max_list_len ids.
 int exhaustive_layout(const fpb_index* ix, int B, int Q, int top_k, ExLayout* X, int n_lists = 0,
                       int64_t max_list_len = 0) {
   // the shape limits first: they do not depend on the index
-  FPB_TRY(check_shapes(B, Q, top_k));
+  FPB_TRY(check_exhaustive_shapes(B, Q, top_k));
   if (!ix) {
     fpb_set_error("exhaustive search: NULL index");
     return FPB_ERR_INVALID;
@@ -142,38 +140,68 @@ extern "C" int fpb_exhaustive_scores(const fpb_index* ix, const void* d_queries,
                                   static_cast<cudaStream_t>(stream));
 }
 
-extern "C" int fpb_search_exhaustive(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k, void* d_ws,
-                                     size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
-                                     void* stream) {
+namespace {
+
+// The selected lists of a full scan, in the workspace: per query the n_sel[b] best local documents (ids, scores)
+// by (score desc, id asc), rows of stride top_k.
+struct ExSelected {
+  int32_t* n_sel;
+  int32_t* ids;
+  float* scores;
+};
+
+// The checks and the whole computation of a full-scan search up to its selected lists: K7 scores every document,
+// k3b_select keeps the top_k of each query with every document a candidate.
+int exhaustive_select(const char* who, const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
+                      void* d_ws, size_t ws_bytes, bool outputs_ok, cudaStream_t st, ExSelected* out) {
   if (top_k < 1) {
-    fpb_set_error("fpb_search_exhaustive: top_k=%d must be >= 1", top_k);
+    fpb_set_error("%s: top_k=%d must be >= 1", who, top_k);
     return FPB_ERR_INVALID;
   }
   ExLayout X;
   FPB_TRY(exhaustive_layout(ix, B, Q, top_k, &X));
   FPB_TRY(check_workspace(X, d_ws, ws_bytes));
-  if (!d_queries || !d_out_ids || !d_out_scores || !d_out_counts) {
-    fpb_set_error("fpb_search_exhaustive: NULL query or output pointer");
+  if (!d_queries || !outputs_ok) {
+    fpb_set_error("%s: NULL query or output pointer", who);
     return FPB_ERR_INVALID;
   }
   if ((reinterpret_cast<uintptr_t>(d_queries) & 15u) != 0) {
-    fpb_set_error("fpb_search_exhaustive: queries must be 16-byte aligned");
+    fpb_set_error("%s: queries must be 16-byte aligned", who);
     return FPB_ERR_INVALID;
   }
   FPB_CUDA_CHECK(cudaSetDevice(ix->device));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   char* base = static_cast<char*>(d_ws);
   float* scores = reinterpret_cast<float*>(base + X.off_scores);
-  int32_t* n_sel = reinterpret_cast<int32_t*>(base + X.off_n_rerank);
-  int32_t* sel_ids = reinterpret_cast<int32_t*>(base + X.off_rerank);
-  float* sel_scores = reinterpret_cast<float*>(base + X.off_rerank_approx);
+  out->n_sel = reinterpret_cast<int32_t*>(base + X.off_n_rerank);
+  out->ids = reinterpret_cast<int32_t*>(base + X.off_rerank);
+  out->scores = reinterpret_cast<float*>(base + X.off_rerank_approx);
   FPB_TRY(launch_exhaustive_scores(ix, X, base, static_cast<const __half*>(d_queries), scores, st));
   // every document is a candidate, and its "approximate" score is its exact one: the selected list holds the exact
   // scores that k6_rank orders
-  FPB_TRY(launch_select(scores, nullptr, nullptr, int(ix->N), B, top_k, sel_ids, sel_scores, n_sel, st));
-  FPB_TRY(launch_rank(sel_scores, sel_ids, n_sel, top_k, B, top_k, ix->doc_id_base, d_out_ids, d_out_scores,
-                      d_out_counts, st));
-  return FPB_OK;
+  return launch_select(scores, nullptr, nullptr, int(ix->N), B, top_k, out->ids, out->scores, out->n_sel, st);
+}
+
+}  // namespace
+
+extern "C" int fpb_search_exhaustive(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k, void* d_ws,
+                                     size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
+                                     void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ExSelected sel;
+  FPB_TRY(exhaustive_select("fpb_search_exhaustive", ix, d_queries, B, Q, top_k, d_ws, ws_bytes,
+                            d_out_ids && d_out_scores && d_out_counts, st, &sel));
+  return launch_rank(sel.scores, sel.ids, sel.n_sel, top_k, B, top_k, ix->doc_id_base, d_out_ids, d_out_scores,
+                     d_out_counts, st);
+}
+
+extern "C" int fpb_shard_exhaustive_records(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
+                                            void* d_ws, size_t ws_bytes, fpb_record* d_records, void* stream) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  ExSelected sel;
+  FPB_TRY(exhaustive_select("fpb_shard_exhaustive_records", ix, d_queries, B, Q, top_k, d_ws, ws_bytes,
+                            d_records != nullptr, st, &sel));
+  // approx = exact = the score: the merge's "R best by approx" is then the global top_k, ordered by the same score
+  return launch_emit_records(sel.scores, sel.scores, sel.ids, sel.n_sel, B, top_k, ix->doc_id_base, d_records, st);
 }
 
 extern "C" int fpb_exhaustive_subset_workspace_bytes(const fpb_index* ix, int B, int Q, int top_k, int n_lists,
@@ -186,7 +214,7 @@ extern "C" int fpb_exhaustive_subset_workspace_bytes(const fpb_index* ix, int B,
     fpb_set_error("fpb_exhaustive_subset_workspace_bytes: top_k=%d must be >= 1", top_k);
     return FPB_ERR_INVALID;
   }
-  FPB_TRY(check_shapes(B, Q, top_k));
+  FPB_TRY(check_exhaustive_shapes(B, Q, top_k));
   FPB_TRY(check_lists(n_lists, max_list_len));
   ExLayout X;
   FPB_TRY(exhaustive_layout(ix, B, Q, top_k, &X, n_lists, max_list_len));
@@ -204,7 +232,7 @@ extern "C" int fpb_search_exhaustive_subset(const fpb_index* ix, const void* d_q
     fpb_set_error("fpb_search_exhaustive_subset: top_k=%d must be >= 1", top_k);
     return FPB_ERR_INVALID;
   }
-  FPB_TRY(check_shapes(B, Q, top_k));
+  FPB_TRY(check_exhaustive_shapes(B, Q, top_k));
   FPB_TRY(check_lists(n_lists, max_list_len));
   if (!h_query_list) {
     fpb_set_error("fpb_search_exhaustive_subset: NULL h_query_list");

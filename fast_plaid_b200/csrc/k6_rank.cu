@@ -480,11 +480,10 @@ int launch_rank(const float* scores, const int32_t* ids, const int32_t* n, int R
   return FPB_OK;
 }
 
-int launch_emit_records(const fpb_index* ix, const Ws& ws, fpb_record* d_records, cudaStream_t st) {
-  const fpb_layout& L = *ws.L;
-  const int64_t n = int64_t(L.B) * L.R;
-  emit_records_kernel<<<int((n + 255) / 256), 256, 0, st>>>(ws.exact(), ws.rerank_approx(), ws.rerank(),
-                                                           ws.n_rerank(), L.B, L.R, ix->doc_id_base, d_records);
+int launch_emit_records(const float* exact, const float* approx, const int32_t* ids, const int32_t* n_sel, int B,
+                        int R, int64_t doc_id_base, fpb_record* d_records, cudaStream_t st) {
+  const int64_t n = int64_t(B) * R;
+  emit_records_kernel<<<int((n + 255) / 256), 256, 0, st>>>(exact, approx, ids, n_sel, B, R, doc_id_base, d_records);
   FPB_LAUNCH_CHECK("emit_records");
   return FPB_OK;
 }

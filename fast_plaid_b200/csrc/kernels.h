@@ -159,7 +159,10 @@ int launch_apply_threshold(const Ws& ws, const uint64_t* d_all_keys, int n_shard
                            int b_stride = 0);
 int launch_merge(const fpb_record* d_all_records, int n_shards, int b_stride, int n_queries, int R, int top_k,
                  int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t stream);
-int launch_emit_records(const fpb_index* ix, const Ws& ws, fpb_record* d_records, cudaStream_t st);
+// per query b the records of the n_sel[b] selected documents in row b of exact / approx / ids (row stride R):
+// (approx, exact, doc_id_base + id), then padding records (-inf, -inf, -1) up to R
+int launch_emit_records(const float* exact, const float* approx, const int32_t* ids, const int32_t* n_sel, int B,
+                        int R, int64_t doc_id_base, fpb_record* d_records, cudaStream_t st);
 
 // K3b and K6 of the search: select by the candidates' approximate scores, rank by the exact ones
 inline int launch_select(const Ws& ws, cudaStream_t st) {
@@ -171,11 +174,21 @@ inline int launch_rank(const fpb_index* ix, const Ws& ws, int top_k, int64_t* d_
   return launch_rank(ws.exact(), ws.rerank(), ws.n_rerank(), ws.L->R, ws.L->B, top_k, ix->doc_id_base, d_out_ids,
                      d_out_scores, d_out_counts, st);
 }
+// the records of the search's re-ranked list, for the shard merge
+inline int launch_emit_records(const fpb_index* ix, const Ws& ws, fpb_record* d_records, cudaStream_t st) {
+  return launch_emit_records(ws.exact(), ws.rerank_approx(), ws.rerank(), ws.n_rerank(), ws.L->B, ws.L->R,
+                             ix->doc_id_base, d_records, st);
+}
 
 // the document bitmap alone of subset_mark_kernel, [n_lists, words]: list l owns d_ids[d_offsets[l] ..
 // d_offsets[l+1]) (global ids; ids outside the index are ignored)
 int launch_doc_bitmap(const fpb_index* ix, const int32_t* d_ids, const int64_t* d_offsets, int64_t max_len,
                       int n_lists, uint32_t* bitmap, int words, cudaStream_t st);
+
+// The shape limits of the exhaustive search: B >= 1, 1 <= Q <= 256, 0 <= top_k <= FPB_EX_MAX_TOP_K (top_k = 0: the
+// scores alone).  Sets the error and returns FPB_ERR_INVALID / FPB_ERR_UNSUPPORTED outside them.
+constexpr int FPB_EX_MAX_TOP_K = 4096;  // the k6_rank bound (one shared-memory bitonic sort per query)
+int check_exhaustive_shapes(int B, int Q, int top_k);
 
 // Workspace of the exhaustive search (exhaustive.cu).  The selection part (top_k > 0) holds the [B, N] scores that
 // k3b_select reads (every document a candidate) and the [B, top_k] list it writes for k6_rank.  A list walk

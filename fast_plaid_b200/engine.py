@@ -134,6 +134,8 @@ EXPORTED_SYMBOLS = [
     "fpb_search_exhaustive",
     "fpb_exhaustive_subset_workspace_bytes",
     "fpb_search_exhaustive_subset",
+    "fpb_shard_exhaustive_records",
+    "fpb_search_exhaustive_sharded",
     "fpb_reconstruct",
     "fpb_token_scores",
     "fpb_encode",
@@ -252,6 +254,10 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_search_exhaustive_subset.restype = i32
         lib.fpb_search_exhaustive_subset.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, i64, vp, vp, sz, vp, vp, vp,
                                                      vp]
+        lib.fpb_shard_exhaustive_records.restype = i32
+        lib.fpb_shard_exhaustive_records.argtypes = [vp, vp, i32, i32, i32, vp, sz, vp, vp]
+        lib.fpb_search_exhaustive_sharded.restype = i32
+        lib.fpb_search_exhaustive_sharded.argtypes = [vp, vp, i32, vp, i32, i32, i32, vp, sz, vp, sz, vp, vp, vp, vp]
         _lib = lib
         return lib
 
@@ -530,13 +536,22 @@ def shard_grid(rank: int, world: int, n_query_groups: int) -> tuple[int, int, in
 MERGE_MAX_RECORDS = 16384
 
 
+def _check_merge(n_shards: int, R: int, what: str) -> None:
+    if n_shards * R > MERGE_MAX_RECORDS:
+        raise ValueError(f"{what} over {n_shards} document shards: {n_shards}*{R} records per query exceed the "
+                         f"{MERGE_MAX_RECORDS} the shard merge supports")
+
+
 def check_merge_records(n_shards: int, n_full_scores: int) -> None:
     """Raise ValueError when a document-sharded search over `n_shards` shards cannot merge its records, the rule
     fpb_merge_shards and fpb_search_batch_sharded apply, so that a search is refused before any collective."""
-    R = max(int(n_full_scores) // 4, 1)
-    if n_shards * R > MERGE_MAX_RECORDS:
-        raise ValueError(f"n_full_scores={n_full_scores} over {n_shards} document shards: {n_shards}*{R} records per "
-                         f"query exceed the {MERGE_MAX_RECORDS} the shard merge supports")
+    _check_merge(n_shards, max(int(n_full_scores) // 4, 1), f"n_full_scores={n_full_scores}")
+
+
+def check_exhaustive_merge_records(n_shards: int, top_k: int) -> None:
+    """The same rule for the document-sharded exhaustive search, whose shards send top_k records per query
+    (fpb_search_exhaustive_sharded): n_shards * top_k <= MERGE_MAX_RECORDS."""
+    _check_merge(n_shards, int(top_k), f"top_k={top_k}")
 
 
 class DeviceIndex:
@@ -895,6 +910,61 @@ class DeviceIndex:
                 )
                 keep.append((sid, soff))
         self._keepalive = keep  # until the stream has consumed them
+
+    # -- document-sharded exhaustive search ------------------------------------------------------
+    def shard_exhaustive_records(self, queries: torch.Tensor, top_k: int) -> torch.Tensor:
+        """Step-wise sharded exhaustive search, local half: uint8 [B, top_k, 16] records (score f32 twice, global
+        doc id i64) of this shard's top_k documents per query, padded with (-inf, -inf, -1).  The shards' records,
+        all-gathered, go to `merge_records(all_records, top_k)`.  Asynchronous."""
+        queries = self._check_queries(queries)
+        B, Q, _ = queries.shape
+        k = int(top_k)
+        rec = torch.empty((B, max(k, 0), 16), dtype=torch.uint8, device=self.device)
+        if B == 0:
+            return rec
+        with self._exclusive(), torch.cuda.device(self.device):
+            buf = self._buffer(self.exhaustive_workspace_bytes(B, Q, k))
+            _check(self._lib.fpb_shard_exhaustive_records(self._handle, queries.data_ptr(), B, Q, k, buf.data_ptr(),
+                                                          buf.numel(), rec.data_ptr(), self._stream()))
+        return rec
+
+    def exhaustive_sharded_step(self, n_query_groups: int, B: int, Q: int, top_k: int,
+                                budget_bytes: int = 6 << 30) -> int:
+        """Most queries per `search_exhaustive_sharded` call whose workspace on this rank, that of
+        ceil(step / n_query_groups) queries, fits `budget_bytes`.  It depends on this shard's document count, so the
+        ranks must agree on one step (the smallest of theirs) before the first collective call."""
+        G = max(int(n_query_groups), 1)
+        return min(B, self._exhaustive_step(-(-B // G), Q, top_k, budget_bytes) * G)
+
+    def search_exhaustive_sharded(self, comm: ShardComm, n_query_groups: int, queries: torch.Tensor, top_k: int,
+                                  step: int | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Exhaustive search of a document-sharded index (fpb_search_exhaustive_sharded): queries fp16 [B, Q, D] on
+        this device, the SAME batch on every rank of `comm` (collective call).  Returns device tensors (ids, scores,
+        counts) for all B queries, the bytes `search_exhaustive` gives on one GPU holding the whole index.
+        `step`: queries per collective call, the same on every rank (default: the whole batch in one call;
+        `exhaustive_sharded_step` gives this rank's largest within a memory budget).  Asynchronous."""
+        queries = self._check_queries(queries)
+        B, Q, _ = queries.shape
+        k, G = int(top_k), int(n_query_groups)
+        ids = torch.empty((B, max(k, 0)), dtype=torch.int64, device=self.device)
+        scores = torch.empty((B, max(k, 0)), dtype=torch.float32, device=self.device)
+        counts = torch.empty((B,), dtype=torch.int32, device=self.device)
+        if B == 0:
+            return ids, scores, counts
+        step = B if step is None else max(1, int(step))
+        with self._exclusive(), torch.cuda.device(self.device):
+            for s in range(0, B, step):
+                e = min(B, s + step)
+                b_local = -(-(e - s) // max(G, 1))
+                buf = self._buffer(self.exhaustive_workspace_bytes(b_local, Q, k))
+                need = max(1, int(self._lib.fpb_sharded_scratch_bytes(b_local, k, comm.nranks)))
+                if getattr(self, "_scratch", None) is None or self._scratch.numel() < need:
+                    self._scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+                _check(self._lib.fpb_search_exhaustive_sharded(
+                    self._handle, comm._handle, G, queries[s:e].data_ptr(), e - s, Q, k, buf.data_ptr(), buf.numel(),
+                    self._scratch.data_ptr(), self._scratch.numel(), ids[s:e].data_ptr(), scores[s:e].data_ptr(),
+                    counts[s:e].data_ptr(), self._stream()))
+        return ids, scores, counts
 
     def _host_io(self, B: int, Q: int, k: int) -> dict[str, torch.Tensor]:
         """Cached pinned + device staging buffers of the host-buffer path."""

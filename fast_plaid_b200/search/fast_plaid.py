@@ -594,6 +594,40 @@ class FastPlaid:
         ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
+    def _exhaustive_sharded_step(self, idx: DeviceIndex, B: int, Q: int, top_k: int, budget_bytes: int) -> int:
+        """Queries per collective call of the sharded exhaustive search, the same on every rank.  Each rank's largest
+        step within the budget depends on its own document count, and shards differ by up to one document: two
+        ranks at a budget boundary would split the batch differently, make different numbers of collective calls
+        and hang.  Every rank takes the smallest of the ranks' steps (one all-reduce on the process group)."""
+        step = idx.exhaustive_sharded_step(self.query_groups, B, Q, top_k, budget_bytes)
+        if self.shard[1] > 1:
+            import torch.distributed as dist
+
+            dev = idx.device if dist.get_backend() == "nccl" else torch.device("cpu")
+            t = torch.tensor([step], dtype=torch.int64, device=dev)
+            dist.all_reduce(t, op=dist.ReduceOp.MIN)
+            step = int(t.item())
+        return step
+
+    def _search_exhaustive_sharded(self, idx: DeviceIndex, queries: torch.Tensor, top_k: int,
+                                   budget_bytes: int = 6 << 30) -> list[list[tuple[int, float]]]:
+        """Document-sharded exhaustive search: per-shard top_k records -> NCCL all-gather -> merge, in one C-ABI call
+        per step of the batch (csrc/comm.cu).  `budget_bytes` bounds each rank's workspace."""
+        if queries.dim() != 3:
+            raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
+        rank, world = self.shard
+        _, _, n_shards = _engine.shard_grid(rank, world, self.query_groups)
+        # refused before the communicator or any collective exists
+        _engine.check_exhaustive_merge_records(n_shards, top_k)
+        comm = self._shard_comm(idx)
+        q16 = queries.to(device=idx.device, dtype=torch.float16)  # the fp16 cast of `search` (fast_plaid.py:241)
+        B, Q, _ = q16.shape
+        if B == 0:
+            return []
+        step = self._exhaustive_sharded_step(idx, B, Q, int(top_k), budget_bytes)
+        ids, scores, counts = idx.search_exhaustive_sharded(comm, self.query_groups, q16, top_k, step=step)
+        return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
+
     @torch.inference_mode()
     def search_exhaustive(
         self,
@@ -616,16 +650,34 @@ class FastPlaid:
         the subset.  The cost grows with the listed documents rather than the index; queries that share a list share
         its decode.
 
+        On a document-sharded index (``shard=``) the call is collective, like ``search``: every rank passes the same
+        queries, scores its own documents for the queries of its query group, and gets every query's result, the
+        same bytes as on one GPU holding the whole index.  There ``top_k`` times the number of document shards may
+        not exceed 16384, ``subset`` is not supported, and several ranks need an initialised ``torch.distributed``
+        process group (the communicator is made, and the ranks agree on how to split the batch, through it).
+
         A score sums the per-query-token fp16 maxima exactly and rounds once to fp32; ``search`` keeps an fp32
         running sum.  The two agree whenever that running sum is exact (the usual case); otherwise the same
         document's score can differ in the last bit between ``search`` and ``search_exhaustive``.  In exchange the
         result is the same bytes however the work is ordered or the batch is split."""
-        if self.shard is not None:
+        if self.shard is not None and not (subset is None or (isinstance(subset, list) and not subset)):
             raise NotImplementedError(
-                "search_exhaustive on a document-sharded index is not implemented: each rank holds only its "
-                "document range, and the per-shard top-k lists would need a merge across ranks"
+                "search_exhaustive with subset= on a document-sharded index is not implemented: each rank would "
+                "have to walk the subset documents of its own range"
             )
+        if self.shard is not None and self.shard[1] > 1:
+            import torch.distributed as dist
+
+            if not dist.is_initialized():
+                # the NCCL communicator is bootstrapped, and the ranks agree on the batch step, through the process
+                # group; other bootstraps exist only at the C ABI (fpb_comm_unique_id / fpb_comm_create)
+                raise NotImplementedError(
+                    f"search_exhaustive on a document-sharded index of {self.shard[1]} ranks needs an initialised "
+                    "torch.distributed process group: FastPlaid exchanges the shards' results over no other channel"
+                )
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
+        if self.shard is not None:
+            return self._search_exhaustive_sharded(search_indices[self.devices[0]], queries, top_k)
         if len(self.devices) == 1:
             return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k, subset)
         # several devices in ONE process hold replicas: the query list is split across them, like `search`

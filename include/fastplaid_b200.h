@@ -352,6 +352,33 @@ int fpb_search_exhaustive_subset(const fpb_index* index, const void* d_queries, 
                                  size_t workspace_bytes, int64_t* d_out_ids, float* d_out_scores,
                                  int32_t* d_out_counts, void* stream);
 
+/* Exhaustive search on a document-sharded index: the result of fpb_search_exhaustive on one GPU holding the whole
+ * index, byte for byte (global ids in rank order, counts = min(top_k, total documents), tails id -1 / score -inf).
+ * K7's scores do not depend on how the documents are split, so only the top-k lists have to be combined.
+ *   fpb_shard_exhaustive_records : the step-wise form.  Runs fpb_search_exhaustive's scan and selection on this
+ *       shard and writes, per query, one fpb_record per selected document (approx = exact = its score, global id
+ *       doc_id_base + local id), then padding records (-inf, -inf, -1) up to top_k.  d_records [B, top_k];
+ *       workspace of fpb_exhaustive_workspace_bytes(index, B, Q, top_k).  The shards' records, all-gathered to
+ *       [n_shards, B, top_k], go to fpb_merge_shards(..., n_shards, B, R = top_k, top_k, ...): with approx equal
+ *       to exact, its "keep the R best by approx, order them by exact" is the global top_k.
+ *   fpb_search_exhaustive_sharded : the whole exchange in one call on `stream`, on the grid of
+ *       fpb_search_batch_sharded (rank r holds document shard r % n_shards and searches the queries of group
+ *       r / n_shards); one ncclAllGather of [ceil(B / n_query_groups), top_k] records, then every rank merges every
+ *       query.  Collective: every rank passes the same batch and gets every query's result.
+ *         d_ws       fpb_exhaustive_workspace_bytes(index, ceil(B / n_query_groups), Q, top_k) bytes
+ *         d_scratch  fpb_sharded_scratch_bytes(ceil(B / n_query_groups), top_k, nranks) bytes
+ * Limits: those of fpb_search_exhaustive (1 <= top_k <= 4096, Q <= 256) and the merge limit of fpb_merge_shards,
+ * n_shards * top_k <= 16384 with n_shards = nranks / n_query_groups.  fpb_search_exhaustive_sharded refuses a call
+ * outside them, NULL arguments and a query-group count that does not divide the ranks on every rank before the
+ * all-gather, with the shapes checked first. */
+int fpb_shard_exhaustive_records(const fpb_index* index, const void* d_queries, int B, int Q, int top_k,
+                                 void* d_workspace, size_t workspace_bytes, fpb_record* d_records /* [B, top_k] */,
+                                 void* stream);
+int fpb_search_exhaustive_sharded(const fpb_index* index, fpb_comm* comm, int n_query_groups, const void* d_queries,
+                                  int B, int Q, int top_k, void* d_workspace, size_t workspace_bytes, void* d_scratch,
+                                  size_t scratch_bytes, int64_t* d_out_ids, float* d_out_scores,
+                                  int32_t* d_out_counts, void* stream);
+
 /* ---- by-products of the MaxSim kernel ("next" rows of SURVEY.md 8f-3) ---- */
 /* reconstruct_embeddings (rust/utils/embeddings.rs:12-69): decompressed, normalised
  * fp16 rows of the given local docs, concatenated.  d_out: f16 [sum(len), dim]. */
