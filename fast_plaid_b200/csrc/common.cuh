@@ -5,10 +5,25 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+#include <mutex>
+
 #include "../../include/fastplaid_b200.h"
 
 struct WPerm {
   uint16_t v[16];
+};
+
+// The walk layout's two growable buffers (fpb_buffer_*), shared by an index and every index appended to it
+// (fpb_index_append): a handle covers the first N + 1 entries of win and the windows they name, and the last
+// fpb_index_destroy frees them.  n_docs is the number of documents laid out so far: only a handle over all of them
+// may append, so that two appends never write the same windows.
+struct fpb_walk {
+  std::atomic<int> refs;
+  std::mutex mu;  // held by an append
+  fpb_buffer* codes;
+  fpb_buffer* win;
+  int64_t n_docs;
 };
 
 // Immutable index handle (replaces LoadedIndex, rust/search/load.rs:50-56).  Holds only
@@ -33,17 +48,21 @@ struct fpb_index {
   // It is a property of the token, not of the (query, document) pair: the MaxSim kernels read it (2 B/token)
   // instead of re-deriving it for every pair.  Caller-owned buffer filled by fpb_index_create.
   const __half* token_norms;
-  // derived at load time, owned by the handle: the approximate stage's copy of the codes (k3_approx.cu).  Document
+  // derived at load time, shared through `walk` (refcounted): the approximate stage's copy of the codes (k3_approx.cu).  Document
   // d owns the 32-token windows walk_win[d] .. walk_win[d+1] - 1 (ceil(len/32) of them) of walk_codes; its codes
   // are dealt over them so that the bitmap words they test in shared memory spread over the 32 banks, and empty
   // slots hold padding codes >= K (fpb_walk_pad_code).  A max over a document's tokens does not depend on their
   // order, so every approximate score is unchanged.
   int32_t* walk_codes;  // [32 * walk_win[N]]
   int64_t* walk_win;    // [N + 1]
+  fpb_walk* walk;       // the buffers behind walk_codes / walk_win
   // windows per group of the bound pass (4, 5 or 6), chosen at load: the group count of a document is rounded up to
   // whole groups, and the windows past its end still cost their bit tests, so the width that wastes the fewest
   // window slots over the index is taken (every 300-token document is 10 windows: 5; 1024 tokens: 4)
   int walk_group;
+  // window slots of the whole index at groups of 4, 5 and 6 windows, from which walk_group is chosen: sums over the
+  // documents, so an append adds its documents' slots
+  int64_t walk_slots[3];
   const int64_t* ivf_offsets;  // nullptr => compress_only
   const int32_t* ivf_pids;
   // w_perm[i] = bucket_weights[bitrev_nbits(i)]  (closed form of the two LUTs of

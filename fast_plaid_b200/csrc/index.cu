@@ -37,18 +37,18 @@ static int make_centroid_tmap(fpb_index* ix) {
   return 0;
 }
 
-// The approximate stage's walk layout (common.cuh, k3_approx.cu): window starts on the host from the document
-// offsets, then the codes dealt on the device.  Owned by the handle (fpb_index_destroy frees it).
-static int make_walk_layout(fpb_index* ix) {
-  const int64_t N = ix->N;
-  int64_t* offs = new int64_t[N + 1];
-  int64_t* win = new int64_t[N + 1];
-  offs[0] = 0;
-  cudaError_t e = N > 0 ? cudaMemcpy(offs, ix->doc_offsets, sizeof(int64_t) * (N + 1), cudaMemcpyDeviceToHost)
-                        : cudaSuccess;
+// The approximate stage's walk layout (common.cuh, k3_approx.cu) of documents [d0, N): window starts on the host
+// from the document offsets, then the codes dealt on the device, into ix->walk's buffers grown to N documents.
+// walk_group is re-chosen from the slot sums of all N documents.  The caller holds ix->walk->mu.
+int fpb_extend_walk_layout(fpb_index* ix, int64_t d0) {
+  const int64_t N = ix->N, n = N - d0;
+  int64_t* offs = new int64_t[n + 1];
+  int64_t* win = new int64_t[n + 1];
+  cudaError_t e = cudaMemcpy(offs, ix->doc_offsets + d0, sizeof(int64_t) * (n + 1), cudaMemcpyDeviceToHost);
   win[0] = 0;
-  int64_t slots[3] = {0, 0, 0};  // window slots the bound pass walks with groups of 4, 5, 6 windows
-  for (int64_t d = 0; d < N; ++d) {
+  if (e == cudaSuccess && d0 > 0) e = cudaMemcpy(win, ix->walk_win + d0, sizeof(int64_t), cudaMemcpyDeviceToHost);
+  int64_t* slots = ix->walk_slots;  // window slots the bound pass walks with groups of 4, 5, 6 windows
+  for (int64_t d = 0; d < n; ++d) {
     const int64_t nw = (offs[d + 1] - offs[d] + 31) / 32;
     win[d + 1] = win[d] + nw;
     for (int g = 4; g <= 6; ++g) slots[g - 4] += (nw > g ? (nw + g - 1) / g : 1) * g;
@@ -56,24 +56,42 @@ static int make_walk_layout(fpb_index* ix) {
   ix->walk_group = 6;  // on a tie the widest group: more code loads in flight
   for (int g = 5; g >= 4; --g)
     if (slots[g - 4] < slots[ix->walk_group - 4]) ix->walk_group = g;
-  const int64_t n_win = win[N];
-  if (e == cudaSuccess) e = cudaMalloc(&ix->walk_win, sizeof(int64_t) * (N + 1));
-  if (e == cudaSuccess) e = cudaMemcpy(ix->walk_win, win, sizeof(int64_t) * (N + 1), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMalloc(&ix->walk_codes, sizeof(int32_t) * 32 * (n_win > 0 ? n_win : 1));
+  const int64_t n_win = win[n];
+  int rc = FPB_OK;
+  if (e == cudaSuccess) rc = fpb_buffer_commit(ix->walk->win, sizeof(int64_t) * (N + 1));
+  if (e == cudaSuccess && rc == FPB_OK)
+    rc = fpb_buffer_commit(ix->walk->codes, sizeof(int32_t) * 32 * (n_win > 0 ? n_win : 1));
+  if (e == cudaSuccess && rc == FPB_OK)
+    e = cudaMemcpy(ix->walk_win + d0, win, sizeof(int64_t) * (n + 1), cudaMemcpyHostToDevice);
   delete[] offs;
   delete[] win;
+  if (rc != FPB_OK) return rc;
   if (e != cudaSuccess) {
     fpb_set_error("walk layout: %s", cudaGetErrorString(e));
     return FPB_ERR_CUDA;
   }
-  if (n_win == 0) return FPB_OK;
-  const int rc = launch_walk_layout(ix, nullptr);
-  if (rc != FPB_OK) return rc;
+  if (n == 0) return FPB_OK;
+  FPB_TRY(launch_walk_layout(ix, d0, nullptr));
   e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
     fpb_set_error("walk layout kernel failed: %s", cudaGetErrorString(e));
     return FPB_ERR_CUDA;
   }
+  return FPB_OK;
+}
+
+static int make_walk_layout(fpb_index* ix) {
+  fpb_walk* w = new fpb_walk();
+  w->refs = 1;
+  w->codes = w->win = nullptr;
+  w->n_docs = 0;
+  ix->walk = w;
+  FPB_TRY(fpb_buffer_reserve(&w->codes, ix->device, 0));
+  FPB_TRY(fpb_buffer_reserve(&w->win, ix->device, 0));
+  ix->walk_codes = static_cast<int32_t*>(fpb_buffer_ptr(w->codes));
+  ix->walk_win = static_cast<int64_t*>(fpb_buffer_ptr(w->win));
+  FPB_TRY(fpb_extend_walk_layout(ix, 0));
+  w->n_docs = ix->N;
   return FPB_OK;
 }
 
@@ -169,7 +187,7 @@ extern "C" int fpb_index_create(fpb_index** out, int device, int nbits, int dim,
     return FPB_ERR_INVALID;
   }
   if (n_tokens > 0) {  // derive the per-token norms once (default stream, synchronous: creation is not a hot path)
-    const int rc = launch_token_norms(ix, static_cast<__half*>(d_token_norms), nullptr);
+    const int rc = launch_token_norms(ix, static_cast<__half*>(d_token_norms), 0, nullptr);
     e = rc == FPB_OK ? cudaDeviceSynchronize() : cudaSuccess;
     if (rc != FPB_OK || e != cudaSuccess) {
       delete ix;
@@ -189,16 +207,16 @@ extern "C" int fpb_index_create(fpb_index** out, int device, int nbits, int dim,
 
 extern "C" void fpb_index_destroy(fpb_index* index) {
   if (!index) return;
-  if (index->walk_codes || index->walk_win) {
-    int prev = -1;
-    const bool have_prev = cudaGetDevice(&prev) == cudaSuccess;
-    cudaSetDevice(index->device);
-    cudaFree(index->walk_codes);
-    cudaFree(index->walk_win);
-    if (have_prev) cudaSetDevice(prev);
+  fpb_walk* w = index->walk;
+  if (w && --w->refs == 0) {
+    fpb_buffer_destroy(w->codes);
+    fpb_buffer_destroy(w->win);
+    delete w;
   }
   delete index;
 }
+
+extern "C" int fpb_index_walk_group(const fpb_index* ix) { return ix ? ix->walk_group : -1; }
 
 extern "C" int fpb_index_walk_layout(const fpb_index* ix, int64_t* n_windows, int32_t* d_codes, int64_t* d_win) {
   if (!ix || !n_windows) {

@@ -1041,13 +1041,15 @@ int launch_approx(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st)
   }
 }
 
-int launch_walk_layout(const fpb_index* ix, cudaStream_t st) {
-  if (ix->N == 0) return FPB_OK;
+int launch_walk_layout(const fpb_index* ix, int64_t d0, cudaStream_t st) {
+  const int64_t n = ix->N - d0;
+  if (n <= 0) return FPB_OK;
   const int64_t warps = K3_WALK_THREADS / 32;
-  const int64_t need = (ix->N + warps - 1) / warps;
+  const int64_t need = (n + warps - 1) / warps;
   const int blocks = int(need < int64_t(ix->sm_count) * 16 ? need : int64_t(ix->sm_count) * 16);
-  k3_walk_layout_kernel<<<blocks, K3_WALK_THREADS, 0, st>>>(ix->doc_offsets, ix->doc_codes, ix->walk_win, ix->N,
-                                                            fpb_hb_words(ix->K), ix->walk_codes);
+  // the kernel indexes codes and windows by absolute offsets, so documents [d0, N) are the arrays' suffixes
+  k3_walk_layout_kernel<<<blocks, K3_WALK_THREADS, 0, st>>>(ix->doc_offsets + d0, ix->doc_codes, ix->walk_win + d0,
+                                                            n, fpb_hb_words(ix->K), ix->walk_codes);
   FPB_LAUNCH_CHECK("k3_walk_layout");
   return FPB_OK;
 }

@@ -271,11 +271,12 @@ K5Kernel k5_kernel(const fpb_index* ix, const fpb_layout& L) {
 
 }  // namespace
 
-int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st) {
+int launch_token_norms(const fpb_index* ix, __half* d_out, int64_t t0, cudaStream_t st) {
+  if (ix->E <= t0) return FPB_OK;
   const int blocks = ix->sm_count * 8;
   return fpb_with_codec(ix->dim, ix->nbits, "token norms", [&](auto c) {
-    k5_token_norms_kernel<c.D, c.NBITS><<<blocks, K5_THREADS, 0, st>>>(ix->centroids, ix->doc_codes,
-                                                                       ix->doc_residuals, ix->w_perm, ix->E, d_out);
+    k5_token_norms_kernel<c.D, c.NBITS><<<blocks, K5_THREADS, 0, st>>>(
+        ix->centroids, ix->doc_codes + t0, ix->doc_residuals + t0 * ix->pd, ix->w_perm, ix->E - t0, d_out + t0);
     FPB_LAUNCH_CHECK("k5_token_norms");
     return FPB_OK;
   });

@@ -132,7 +132,9 @@ int launch_subset(const fpb_index* ix, const Ws& ws, const int32_t* d_ids, const
 int launch_compact(const uint32_t* bitmap, const uint32_t* mask, int words, int32_t* out, int cap, int32_t* n_out,
                    int B, cudaStream_t st);
 int launch_approx(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st); // K3 (flags: FPB_FLAG_APPROX_*)
-int launch_walk_layout(const fpb_index* ix, cudaStream_t st);                     // K3's walk_codes (index load)
+int launch_walk_layout(const fpb_index* ix, int64_t d0, cudaStream_t st);  // K3's walk_codes of documents [d0, N)
+// the walk layout of documents [d0, N) in ix->walk's buffers, and walk_group (index.cu)
+int fpb_extend_walk_layout(fpb_index* ix, int64_t d0);
 // K3b: per query b the R best of the n_cand[b] scores in row b of `scores` (row stride `stride`) by (score desc,
 // candidate index asc); their ids (cand[b, i], or i itself when cand is NULL: then every one of the `stride` entries
 // of a row is a candidate and n_cand is not read), their scores and their count go to rerank, rerank_scores [B, R]
@@ -140,7 +142,8 @@ int launch_walk_layout(const fpb_index* ix, cudaStream_t st);                   
 int launch_select(const float* scores, const int32_t* cand, const int32_t* n_cand, int stride, int B, int R,
                   int32_t* rerank, float* rerank_scores, int32_t* n_rerank, cudaStream_t st);
 int launch_maxsim(const fpb_index* ix, const Ws& ws, cudaStream_t st);            // K5 (dispatch)
-int launch_token_norms(const fpb_index* ix, __half* d_out, cudaStream_t st);      // per-token fp16 norms (index load)
+// per-token fp16 norms of tokens [t0, E) into d_out[t0, E) (index load and append)
+int launch_token_norms(const fpb_index* ix, __half* d_out, int64_t t0, cudaStream_t st);
 int launch_maxsim_v4(const fpb_index* ix, const Ws& ws, cudaStream_t st);  // K5 v4 (register operands)
 int launch_maxsim_v5(const fpb_index* ix, const Ws& ws, cudaStream_t st);  // K5 v5 (wgmma, 16 decode warps)
 // 8-token passes per v5 chunk: a document of more passes than this goes to the generic kernel

@@ -101,6 +101,14 @@ EXPORTED_SYMBOLS = [
     "fpb_index_create",
     "fpb_index_destroy",
     "fpb_index_walk_layout",
+    "fpb_index_walk_group",
+    "fpb_index_append",
+    "fpb_ivf_append",
+    "fpb_buffer_reserve",
+    "fpb_buffer_commit",
+    "fpb_buffer_ptr",
+    "fpb_buffer_mapped_bytes",
+    "fpb_buffer_destroy",
     "fpb_workspace_layout",
     "fpb_search_batch",
     "fpb_search_batch_subset",
@@ -174,6 +182,22 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_index_destroy.argtypes = [vp]
         lib.fpb_index_walk_layout.restype = i32
         lib.fpb_index_walk_layout.argtypes = [vp, ctypes.POINTER(i64), vp, vp]
+        lib.fpb_index_walk_group.restype = i32
+        lib.fpb_index_walk_group.argtypes = [vp]
+        lib.fpb_index_append.restype = i32
+        lib.fpb_index_append.argtypes = [ctypes.POINTER(vp), vp, i64, i64, vp, vp, vp, vp, vp, vp, i64, i64]
+        lib.fpb_ivf_append.restype = i32
+        lib.fpb_ivf_append.argtypes = [i32, i64, vp, vp, i64, i64, vp, vp, vp, vp, i64, ctypes.POINTER(i64), vp]
+        lib.fpb_buffer_reserve.restype = i32
+        lib.fpb_buffer_reserve.argtypes = [ctypes.POINTER(vp), i32, sz]
+        lib.fpb_buffer_commit.restype = i32
+        lib.fpb_buffer_commit.argtypes = [vp, sz]
+        lib.fpb_buffer_ptr.restype = vp
+        lib.fpb_buffer_ptr.argtypes = [vp]
+        lib.fpb_buffer_mapped_bytes.restype = sz
+        lib.fpb_buffer_mapped_bytes.argtypes = [vp]
+        lib.fpb_buffer_destroy.restype = None
+        lib.fpb_buffer_destroy.argtypes = [vp]
         lib.fpb_workspace_layout.restype = i32
         lib.fpb_workspace_layout.argtypes = [vp, i32, i32, ctypes.POINTER(FpbParams), ctypes.POINTER(FpbLayout)]
         lib.fpb_search_batch.restype = i32
@@ -332,6 +356,9 @@ class IndexTensors:
     ivf_lengths: torch.Tensor | None  # [K] int
     avg_residual: torch.Tensor | None = None  # unused at search time (load.rs:146)
     bucket_cutoffs: torch.Tensor | None = None  # unused at search time (load.rs:148)
+    # the GrowableArrays whose buffers hold doc_codes / doc_residuals from their start (the loader's fast path):
+    # DeviceIndex then adopts them, so that an append grows them in place
+    growable: Any = None
 
     @property
     def num_documents(self) -> int:
@@ -554,6 +581,89 @@ def check_exhaustive_merge_records(n_shards: int, top_k: int) -> None:
     _check_merge(n_shards, int(top_k), f"top_k={top_k}")
 
 
+class GrowableBuffer:
+    """One growable device buffer (fpb_buffer_*): address space reserved up to the device's memory, physical memory
+    mapped in 2 MB granules as `commit` asks for it.  Its address never changes, so tensors viewing its start stay
+    valid while it grows.  The views (`view`) keep this object alive, and it frees the memory when the last of them
+    and the last owner are gone."""
+
+    _TYPESTR = {torch.int32: "<i4", torch.int64: "<i8", torch.uint8: "|u1", torch.float16: "<f2"}
+
+    def __init__(self, device: torch.device) -> None:
+        self._lib = load_library()
+        self.device = torch.device(device)
+        handle = ctypes.c_void_p()
+        with torch.cuda.device(self.device):
+            _check(self._lib.fpb_buffer_reserve(ctypes.byref(handle), self.device.index, 0))
+        self._handle = handle
+        self.ptr = int(self._lib.fpb_buffer_ptr(handle))
+
+    def commit(self, nbytes: int) -> None:
+        _check(self._lib.fpb_buffer_commit(self._handle, max(int(nbytes), 1)))
+
+    @property
+    def mapped_bytes(self) -> int:
+        return int(self._lib.fpb_buffer_mapped_bytes(self._handle))
+
+    def view(self, dtype: torch.dtype, shape: tuple[int, ...]) -> torch.Tensor:
+        """A tensor over the buffer's first bytes (committed here first)."""
+        n = 1
+        for d in shape:
+            n *= int(d)
+        self.commit(n * torch.empty((), dtype=dtype).element_size())
+        return torch.as_tensor(_BufferView(self, shape, self._TYPESTR[dtype]), device=self.device)
+
+    def __del__(self) -> None:  # pragma: no cover
+        h = getattr(self, "_handle", None)
+        if h is not None and h.value:
+            try:
+                torch.cuda.synchronize(self.device)  # kernels still reading the buffer
+            except Exception:
+                pass
+            self._lib.fpb_buffer_destroy(h)
+            self._handle = ctypes.c_void_p()
+
+
+class _BufferView:
+    """__cuda_array_interface__ of a GrowableBuffer's start; the tensor made from it holds this object, and this
+    object holds the buffer."""
+
+    def __init__(self, buf: GrowableBuffer, shape: tuple[int, ...], typestr: str) -> None:
+        self.buf = buf
+        self.__cuda_array_interface__ = {"shape": tuple(int(d) for d in shape), "typestr": typestr,
+                                         "data": (buf.ptr, False), "version": 2}
+
+
+class GrowableArrays:
+    """The per-token arrays of an index (codes, residuals, token norms) and its document offsets in growable
+    buffers, shared by a DeviceIndex and every DeviceIndex appended to it.  `n_docs` / `n_tokens` count what has
+    been written: only the DeviceIndex that covers all of it may append, so that appends never overwrite rows
+    another index uses."""
+
+    def __init__(self, device: torch.device, pd: int) -> None:
+        self.device = torch.device(device)
+        self.pd = int(pd)
+        self.codes = GrowableBuffer(self.device)
+        self.residuals = GrowableBuffer(self.device)
+        self.norms = GrowableBuffer(self.device)
+        self.offsets = GrowableBuffer(self.device)
+        self.n_docs = 0
+        self.n_tokens = 0
+        self.lock = threading.Lock()
+
+    def views(self, n_docs: int, n_tokens: int) -> dict[str, torch.Tensor]:
+        """Tensors over the first n_docs + 1 offsets and n_tokens rows (at least one row, as DeviceIndex keeps)."""
+        rows = max(int(n_tokens), 1)
+        return {"offsets": self.offsets.view(torch.int64, (int(n_docs) + 1,)),
+                "codes": self.codes.view(torch.int32, (rows,)),
+                "residuals": self.residuals.view(torch.uint8, (rows, self.pd)),
+                "norms": self.norms.view(torch.float16, (rows,))}
+
+    @property
+    def mapped_bytes(self) -> int:
+        return sum(b.mapped_bytes for b in (self.codes, self.residuals, self.norms, self.offsets))
+
+
 class DeviceIndex:
     """One index (or shard) resident in HBM + its ``fpb_index`` handle."""
 
@@ -579,13 +689,35 @@ class DeviceIndex:
             offs = torch.zeros(self.num_documents + 1, dtype=torch.int64)
             offs[1:] = lens.cpu().cumsum(0)
             self.num_tokens = int(offs[-1])
-            self.doc_offsets = offs.to(dev)
-            # rows past the last document (the reference's tail padding, load.py:298-300) are dropped
-            self.doc_codes = upload_narrow(data.doc_codes[: self.num_tokens], dev, torch.int32)
-            self.doc_residuals = upload_narrow(data.doc_residuals[: self.num_tokens], dev, torch.uint8)
-            if self.doc_codes.numel() == 0:
-                self.doc_codes = torch.zeros(1, dtype=torch.int32, device=dev)
-                self.doc_residuals = torch.zeros((1, self.dim * self.nbits // 8), dtype=torch.uint8, device=dev)
+            E = self.num_tokens
+            # Codes, residuals, norms and offsets go to growable buffers (appends then grow them in place): the
+            # loader's, or new ones for host tensors.  Device tensors outside them are used where they are, and the
+            # first append copies them (`append`).
+            arrays = data.growable
+            if arrays is None and data.doc_codes.device.type == "cpu":
+                arrays = GrowableArrays(dev, self.dim * self.nbits // 8)
+            if arrays is not None:
+                v = arrays.views(self.num_documents, E)
+                v["offsets"].copy_(offs)
+                if data.growable is None and E > 0:
+                    # rows past the last document (the reference's tail padding, load.py:298-300) are dropped
+                    upload_narrow(data.doc_codes[:E], dev, torch.int32, out=v["codes"][:E])
+                    upload_narrow(data.doc_residuals[:E], dev, torch.uint8, out=v["residuals"][:E])
+                elif data.growable is not None and data.doc_codes.data_ptr() != arrays.codes.ptr:
+                    raise ValueError("IndexTensors.growable must hold doc_codes and doc_residuals from its start")
+                if E == 0:
+                    v["codes"].zero_()
+                    v["residuals"].zero_()
+                arrays.n_docs, arrays.n_tokens = self.num_documents, E
+                self.doc_offsets, self.doc_codes, self.doc_residuals = v["offsets"], v["codes"], v["residuals"]
+            else:
+                self.doc_offsets = offs.to(dev)
+                self.doc_codes = upload_narrow(data.doc_codes[:E], dev, torch.int32)
+                self.doc_residuals = upload_narrow(data.doc_residuals[:E], dev, torch.uint8)
+                if self.doc_codes.numel() == 0:
+                    self.doc_codes = torch.zeros(1, dtype=torch.int32, device=dev)
+                    self.doc_residuals = torch.zeros((1, self.dim * self.nbits // 8), dtype=torch.uint8, device=dev)
+            self._arrays = arrays
             self.num_centroids = int(self.centroids.shape[0])
             if data.ivf is not None and data.ivf_lengths is not None:
                 il = data.ivf_lengths.to(torch.int64).cpu()
@@ -603,7 +735,10 @@ class DeviceIndex:
                 self.ivf_pids = None
                 n_ivf = 0
             # derived at load: the fp16 norm of every decompressed token (2 B/token), filled by fpb_index_create
-            self.token_norms = torch.empty(max(self.num_tokens, 1), dtype=torch.float16, device=dev)
+            if arrays is not None:
+                self.token_norms = v["norms"]
+            else:
+                self.token_norms = torch.empty(max(self.num_tokens, 1), dtype=torch.float16, device=dev)
             handle = ctypes.c_void_p()
             _check(
                 self._lib.fpb_index_create(
@@ -614,6 +749,9 @@ class DeviceIndex:
                 )
             )
         self._handle = handle
+        self._init_state()
+
+    def _init_state(self) -> None:
         self._ws: dict[tuple, FpbLayout] = {}
         self._buf: torch.Tensor | None = None
         self._io: dict[tuple, dict[str, torch.Tensor]] = {}
@@ -663,6 +801,103 @@ class DeviceIndex:
     @property
     def has_ivf(self) -> bool:
         return self.ivf_offsets is not None
+
+    @property
+    def walk_group(self) -> int:
+        """Windows per group of the approximate stage's bound pass, chosen from the walk layout (fpb_index_walk_group)."""
+        return int(self._lib.fpb_index_walk_group(self._handle))
+
+    @property
+    def growable(self) -> "GrowableArrays | None":
+        """The growable buffers this index's arrays live in (None until the first append for an index built from
+        device tensors)."""
+        return self._arrays
+
+    # -- growth --------------------------------------------------------------------------
+    def _copy_to_growable(self) -> GrowableArrays:
+        """The one copy of an index built from device tensors: its arrays in new growable buffers."""
+        N, E = self.num_documents, self.num_tokens
+        arrays = GrowableArrays(self.device, self.dim * self.nbits // 8)
+        v = arrays.views(N, E)
+        v["offsets"].copy_(self.doc_offsets)
+        for name, t in (("codes", self.doc_codes), ("residuals", self.doc_residuals), ("norms", self.token_norms)):
+            v[name][:E].copy_(t[:E])
+        arrays.n_docs, arrays.n_tokens = N, E
+        return arrays
+
+    @torch.inference_mode()
+    def append(self, codes: torch.Tensor, residuals: torch.Tensor, doc_lengths: torch.Tensor) -> "DeviceIndex":
+        """A new DeviceIndex over this index's documents followed by new ones, given by their codes [n_tokens],
+        packed residuals [n_tokens, dim*nbits/8] and lengths [n_docs] (any device).  It shares this index's memory:
+        the new rows are written after the old ones in the growable buffers, the token norms and the approximate
+        stage's walk layout are computed for the new tokens and documents only (fpb_index_append), and the inverted
+        file is merged on the device into a new array (fpb_ivf_append), the one copy of existing data an append
+        makes (4 bytes per posting).  The result equals a DeviceIndex built from scratch over all the documents.
+
+        This index stays valid and searchable, and its results do not change.  Only the newest index of a chain of
+        appends may be appended to.  An index whose arrays are not in growable buffers (built from device tensors,
+        as ``FastPlaid.from_tensors`` and ``bench.py`` do) first copies its codes, residuals, norms and offsets into
+        them, once: that first append briefly holds those arrays twice."""
+        dev = self.device
+        lens = doc_lengths.to(torch.int64).cpu().reshape(-1)
+        n_new, e_new = int(lens.shape[0]), int(lens.sum())
+        pd = self.dim * self.nbits // 8
+        codes = codes.reshape(-1)
+        if bool((lens < 0).any()) or codes.shape[0] != e_new or tuple(residuals.shape) != (e_new, pd):
+            raise ValueError(f"append: {n_new} documents of {e_new} tokens need codes [{e_new}] and residuals "
+                             f"[{e_new}, {pd}], got {tuple(codes.shape)} and {tuple(residuals.shape)}")
+        N, E = self.num_documents, self.num_tokens
+        N1, E1 = N + n_new, E + e_new
+        with torch.cuda.device(dev):
+            if getattr(self, "_handle", None) is None or not self._handle.value:
+                raise RuntimeError("this DeviceIndex has been closed")
+            with self._lock:
+                arrays = self._arrays
+                if arrays is None:
+                    arrays = self._arrays = self._copy_to_growable()
+            with arrays.lock:  # appends to one chain, one at a time
+                if arrays.n_docs != N or arrays.n_tokens != E:
+                    raise ValueError(f"append: this index of {N} documents is not the newest of its chain "
+                                     f"({arrays.n_docs} documents are laid out); append to the newest one")
+                v = arrays.views(N1, E1)
+                if e_new > 0:
+                    v["codes"][E:E1].copy_(codes.to(dev, torch.int32))
+                    v["residuals"][E:E1].copy_(residuals.to(dev, torch.uint8))
+                new_offs = torch.zeros(n_new + 1, dtype=torch.int64)
+                new_offs[1:] = lens.cumsum(0)
+                v["offsets"][N + 1 :].copy_(new_offs[1:] + E)
+                ivf_offsets = ivf_pids = None
+                n_ivf = ctypes.c_int64(0)
+                st = self._stream()
+                if self.has_ivf:
+                    n_cells = int(self.ivf_offsets.shape[0]) - 1
+                    ivf_offsets = torch.empty(n_cells + 1, dtype=torch.int64, device=dev)
+                    local = new_offs.to(dev)
+                    new_codes = v["codes"].data_ptr() + 4 * E
+                    args = (dev.index, n_cells, self.ivf_offsets.data_ptr(), self.ivf_pids.data_ptr(), N, n_new,
+                            local.data_ptr(), new_codes, ivf_offsets.data_ptr())
+                    _check(self._lib.fpb_ivf_append(*args, None, 0, ctypes.byref(n_ivf), st))  # sizes the output
+                    ivf_pids = torch.zeros(max(n_ivf.value, 1), dtype=torch.int32, device=dev)
+                    _check(self._lib.fpb_ivf_append(*args, ivf_pids.data_ptr(), ivf_pids.numel(), ctypes.byref(n_ivf), st))
+                torch.cuda.current_stream(dev).synchronize()  # fpb_index_append works on the legacy default stream
+                max_len = max(self.max_doc_len, int(lens.max()) if n_new > 0 else 0)
+                handle = ctypes.c_void_p()
+                _check(self._lib.fpb_index_append(
+                    ctypes.byref(handle), self._handle, N1, E1, v["offsets"].data_ptr(), v["codes"].data_ptr(),
+                    v["residuals"].data_ptr(), v["norms"].data_ptr(), _ptr(ivf_offsets), _ptr(ivf_pids), n_ivf.value,
+                    max_len))
+                arrays.n_docs, arrays.n_tokens = N1, E1
+        new = DeviceIndex.__new__(DeviceIndex)
+        for name in ("_lib", "device", "nbits", "dim", "doc_id_base", "centroids", "bucket_weights", "num_centroids"):
+            setattr(new, name, getattr(self, name))
+        new.num_documents, new.num_tokens, new.max_doc_len = N1, E1, max_len
+        new.doc_offsets, new.doc_codes, new.doc_residuals, new.token_norms = (
+            v["offsets"], v["codes"], v["residuals"], v["norms"])
+        new.ivf_offsets, new.ivf_pids = ivf_offsets, ivf_pids
+        new._arrays = arrays
+        new._handle = handle
+        new._init_state()
+        return new
 
     # -- helpers -------------------------------------------------------------------------
     @staticmethod

@@ -99,7 +99,7 @@ def read_index_to_device(index_path: str, device: str | torch.device,
     contiguous document range; default: all) are read; the int64 codes are narrowed to int32 by the staging pass.
     A shard's inverted file is rebuilt on the GPU from its own codes (ids local to the shard) instead of filtering
     the global ``ivf.npy`` on the host.  Returns (tensors with the big arrays on `device`, doc_id_base)."""
-    from ..engine import upload_narrow
+    from ..engine import GrowableArrays, upload_narrow
     from .layout import build_ivf
 
     meta = read_metadata(index_path)
@@ -126,10 +126,12 @@ def read_index_to_device(index_path: str, device: str | torch.device,
     offs = torch.zeros(n_docs + 1, dtype=torch.int64)
     offs[1:] = all_lens.cumsum(0)
     t0, t1 = int(offs[lo]), int(offs[hi])
-    codes = torch.empty((max(t1 - t0, 0),), dtype=torch.int32, device=dev)
-    residuals = torch.empty((max(t1 - t0, 0), pd), dtype=torch.uint8, device=dev)
     c0 = 0  # first token of the chunk in the whole index
     with torch.cuda.device(dev), warnings.catch_warnings():
+        # codes and residuals go straight into growable buffers, which DeviceIndex adopts and appends grow in place
+        arrays = GrowableArrays(dev, pd)
+        views = arrays.views(max(hi - lo, 0), t1 - t0)
+        codes, residuals = views["codes"][: max(t1 - t0, 0)], views["residuals"][: max(t1 - t0, 0)]
         warnings.simplefilter("ignore", UserWarning)  # read-only memory maps are only ever read here
         for i in range(num_chunks):
             n_tok = int(sum(chunk_lens[i]))
@@ -155,7 +157,7 @@ def read_index_to_device(index_path: str, device: str | torch.device,
                 del ivf64
         torch.cuda.synchronize(dev)
     data = IndexTensors(nbits=nbits, centroids=centroids, bucket_weights=weights, doc_lengths=all_lens[lo:hi],
-                        doc_codes=codes, doc_residuals=residuals, ivf=ivf, ivf_lengths=ivf_lengths)
+                        doc_codes=codes, doc_residuals=residuals, ivf=ivf, ivf_lengths=ivf_lengths, growable=arrays)
     return data, lo
 
 

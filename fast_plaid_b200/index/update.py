@@ -27,13 +27,16 @@ def _load_raw(path: str) -> list[torch.Tensor]:
 
 def process_update(fp: Any, docs: list[torch.Tensor], metadata: list[dict] | None, batch_size: int,
                    kmeans_niters: int, max_points_per_centroid: int, n_samples_kmeans: int | None, seed: int,
-                   start_from_scratch: int) -> None:
+                   start_from_scratch: int, loaded: dict[str, Any] | None = None) -> dict[str, Any] | None:
+    """Add `docs` to the index directory.  `loaded` (device -> DeviceIndex of the directory as it is on disk) asks
+    for the appended documents to be added to those indexes in place as well; the grown indexes are returned when
+    that happened, None when the caller has to load the directory again."""
     index_path = fp.index
     meta = store.read_metadata(index_path)
     if meta is None:  # update.py:271-290
         fp.create(docs, kmeans_niters=kmeans_niters, max_points_per_centroid=max_points_per_centroid,
                   n_samples_kmeans=n_samples_kmeans, batch_size=batch_size, seed=seed, metadata=metadata)
-        return
+        return None
     n_old = int(meta.get("num_documents", 0))
     emb_path = os.path.join(index_path, "embeddings.npy")
     db = os.path.join(index_path, "metadata.db")
@@ -65,13 +68,19 @@ def process_update(fp: Any, docs: list[torch.Tensor], metadata: list[dict] | Non
                 os.replace(db + ".keep", db)
         if len(old) + len(docs) > start_from_scratch and os.path.exists(emb_path):
             os.remove(emb_path)
-        return
-    append_documents(index_path, docs, batch_size=batch_size, device=fp.devices[0])
+        return None
+    return append_documents(index_path, docs, batch_size=batch_size, device=fp.devices[0], loaded=loaded)
 
 
 @torch.inference_mode()
-def append_documents(index_path: str, docs: list[torch.Tensor], batch_size: int, device: str) -> None:
-    """Encode with the codec on disk and append as new chunk(s) (update.rs:30-473)."""
+def append_documents(index_path: str, docs: list[torch.Tensor], batch_size: int, device: str,
+                     loaded: dict[str, Any] | None = None) -> dict[str, Any] | None:
+    """Encode with the codec on disk and append as new chunk(s) (update.rs:30-473).
+
+    With `loaded` (device -> the DeviceIndex of the directory before this call), the new documents are also
+    appended to each of those indexes (DeviceIndex.append) and the grown indexes are returned; the inverted file
+    written to disk is then the one merged on the device, the same bytes a rebuild from the chunk files gives.  If
+    an append fails the inverted file is rebuilt from the chunk files and None is returned."""
     meta = store.read_metadata(index_path)
     nbits = int(meta["nbits"])
     dev = torch.device(device)
@@ -83,6 +92,9 @@ def append_documents(index_path: str, docs: list[torch.Tensor], batch_size: int,
     emb_offset = int(meta["num_embeddings"])
     n_docs = int(meta["num_documents"])
     per_chunk = max(1, int(batch_size))
+    new_codes: list[torch.Tensor] = []
+    new_res: list[torch.Tensor] = []
+    new_lens: list[int] = []
     for s in range(0, len(docs), per_chunk):
         chunk_docs = docs[s : s + per_chunk]
         lens = [int(d.shape[0]) for d in chunk_docs]
@@ -90,20 +102,51 @@ def append_documents(index_path: str, docs: list[torch.Tensor], batch_size: int,
         codes_parts, res_parts = [], []
         for r in range(0, flat.shape[0], max(1, batch_size)):
             c, rr = build.encode(flat[r : r + batch_size], cent, cent_t, cutoffs, nbits)
-            codes_parts.append(c.cpu())
-            res_parts.append(rr.cpu())
-        codes = torch.cat(codes_parts) if codes_parts else torch.empty(0, dtype=torch.int64)
-        res = torch.cat(res_parts) if res_parts else torch.empty((0, dim * nbits // 8), dtype=torch.uint8)
+            codes_parts.append(c)
+            res_parts.append(rr)
+        codes = torch.cat(codes_parts) if codes_parts else torch.empty(0, dtype=torch.int64, device=dev)
+        res = torch.cat(res_parts) if res_parts else torch.empty((0, dim * nbits // 8), dtype=torch.uint8, device=dev)
         store.write_chunk(index_path, n_chunks, codes, res, lens, emb_offset)
+        if loaded is not None:
+            new_codes.append(codes.to(torch.int32))
+            new_res.append(res)
+            new_lens.extend(lens)
         n_chunks += 1
         emb_offset += int(codes.shape[0])
         n_docs += len(lens)
     compress_only = bool(meta.get("compress_only", False))
+    n_cells = int(meta.get("num_partitions", cent.shape[0]))
+    grown = None
+    if loaded is not None:
+        codes = torch.cat(new_codes) if new_codes else torch.empty(0, dtype=torch.int32, device=dev)
+        res = torch.cat(new_res) if new_res else torch.empty((0, dim * nbits // 8), dtype=torch.uint8, device=dev)
+        lens_t = torch.tensor(new_lens, dtype=torch.int64)
+        try:
+            grown = {d: idx.append(codes, res, lens_t) for d, idx in loaded.items()}
+        except Exception as e:
+            print(f"Warning: appending in place failed, the index will be loaded again: {e}")
+            grown = None
+        del codes, res
     if not compress_only:
-        _rebuild_ivf(index_path, n_chunks, int(meta.get("num_partitions", cent.shape[0])), dev)
-    store.write_metadata(index_path, num_chunks=n_chunks, nbits=nbits,
-                         num_partitions=int(meta.get("num_partitions", cent.shape[0])),
+        if grown is not None:
+            _write_merged_ivf(index_path, grown[device], n_cells)
+        else:
+            _rebuild_ivf(index_path, n_chunks, n_cells, dev)
+    store.write_metadata(index_path, num_chunks=n_chunks, nbits=nbits, num_partitions=n_cells,
                          num_embeddings=emb_offset, num_documents=n_docs, compress_only=compress_only)
+    return grown
+
+
+def _write_merged_ivf(index_path: str, idx: Any, n_cells: int) -> None:
+    """ivf.npy / ivf_lengths.npy of a DeviceIndex's inverted file, as build_ivf writes them: one length per cell up
+    to max(n_cells, the last non-empty cell + 1)."""
+    offs = idx.ivf_offsets.cpu()
+    lengths = offs[1:] - offs[:-1]
+    nz = torch.nonzero(lengths).flatten()
+    n = max(n_cells, int(nz[-1]) + 1 if nz.numel() else 0)
+    if n > lengths.shape[0]:
+        lengths = torch.cat([lengths, torch.zeros(n - lengths.shape[0], dtype=lengths.dtype)])
+    store.write_ivf(index_path, idx.ivf_pids[: int(offs[-1])], lengths[:n])
 
 
 def _rebuild_ivf(index_path: str, n_chunks: int, n_cells: int, dev: torch.device) -> None:

@@ -372,6 +372,12 @@ class FastPlaid:
         reference's centroid-expansion buffer (update.py:65-203) is an index-mutation policy
         outside the search hot path and is not reproduced: appended documents always use the
         existing centroids.
+
+        Appended documents are added to the index already in HBM, in place (``DeviceIndex.append``): the cost is the
+        new documents' data plus a new copy of the inverted file (4 bytes per posting), not a second copy of the
+        index, and searches running meanwhile keep their results.  The index is loaded again from the directory
+        instead when it is sharded, rebuilt from scratch, not loaded on every device, changed on disk by another
+        process since it was loaded, or when the append fails.
         """
         from ..index import update as _update
 
@@ -379,10 +385,33 @@ class FastPlaid:
             docs = self._format_embeddings(documents_embeddings)
             if isinstance(docs, torch.Tensor):
                 docs = list(docs) if docs.dim() == 3 else [docs]
-            _update.process_update(self, docs, metadata, batch_size, kmeans_niters, max_points_per_centroid,
-                                   n_samples_kmeans, seed, start_from_scratch)
-            self._swap_in_fresh()
+            grown = _update.process_update(self, docs, metadata, batch_size, kmeans_niters, max_points_per_centroid,
+                                           n_samples_kmeans, seed, start_from_scratch, loaded=self._appendable())
+            if grown is None:
+                self._swap_in_fresh()
+            else:
+                with self._index_swap_lock:
+                    old = self.indices
+                    self.indices = grown
+                    self._update_mtime()
+                    self._cpu_loaded = True
+                self._retire(old)
         return self
+
+    def _appendable(self) -> dict[str, DeviceIndex] | None:
+        """The loaded indexes an update may append to in place, or None when it must load the directory again: a
+        sharded index (the shards' document ranges move when the index grows), a device without a loaded index, or
+        a directory that another process changed since it was loaded."""
+        meta_path = os.path.join(self.index, "metadata.json")
+        if self.shard is not None or not os.path.exists(meta_path):
+            return None
+        with self._index_swap_lock:
+            if Path(meta_path).stat().st_mtime != self._last_known_mtime:
+                return None
+            snapshot = dict(self.indices)
+        if not snapshot or any(d == "cpu" or snapshot.get(d) is None for d in self.devices):
+            return None
+        return snapshot
 
     @torch.inference_mode()
     def delete(self, subset: list[int], _delete_metadata: bool = True, _delete_buffer: bool = True) -> "FastPlaid":  # noqa: ARG002

@@ -68,9 +68,10 @@ int fpb_abi_version(void);
  * else, dim 64 with nbits 1 included, returns FPB_ERR_UNSUPPORTED before any CUDA call, with a message naming dim
  * and nbits.
  *
- * The handle also allocates and owns one derived device array that fpb_index_destroy frees: the approximate
- * stage's copy of the codes, each document's tokens reordered into whole 32-token windows (4 bytes per token
- * rounded up to a multiple of 32 per document, plus 8 bytes per document).
+ * The handle also allocates one derived device array, in growable buffers it shares with the handles appended to
+ * it (fpb_index_append) and that the last fpb_index_destroy frees: the approximate stage's copy of the codes, each
+ * document's tokens reordered into whole 32-token windows (4 bytes per token rounded up to a multiple of 32 per
+ * document, plus 8 bytes per document).
  */
 int fpb_index_create(fpb_index** out, int device, int nbits, int dim, int64_t n_centroids,
                      const void* d_centroids, const void* d_bucket_weights, int64_t n_docs,
@@ -83,6 +84,57 @@ void fpb_index_destroy(fpb_index* index);
  * (i32 [32 * n_windows]) and d_win (i64 [n_docs + 1], first window of each document) receive device copies.
  * Synchronous. */
 int fpb_index_walk_layout(const fpb_index* index, int64_t* n_windows, int32_t* d_codes, int64_t* d_win);
+/* Windows per group of the approximate stage's bound pass (4, 5 or 6), chosen from the walk layout; -1 on NULL. */
+int fpb_index_walk_group(const fpb_index* index);
+
+/*
+ * Growable device buffers: address space reserved once on `device` (max_bytes, or the device's memory when 0),
+ * backed by physical memory mapped in 2 MB granules as it is committed (the driver's virtual memory management).
+ * fpb_buffer_ptr never changes, so an index's arrays can grow in place while a handle over their first bytes stays
+ * valid.  fpb_buffer_commit(b, bytes) maps up to at least `bytes` from the start (a no-op when already mapped) and
+ * leaves the mapped contents as they are; it is synchronous.  fpb_buffer_destroy unmaps and frees everything: no
+ * work may still read the buffer, and no handle may still use it.
+ */
+typedef struct fpb_buffer fpb_buffer;
+int fpb_buffer_reserve(fpb_buffer** out, int device, size_t max_bytes);
+int fpb_buffer_commit(fpb_buffer* buffer, size_t bytes);
+void* fpb_buffer_ptr(const fpb_buffer* buffer);
+size_t fpb_buffer_mapped_bytes(const fpb_buffer* buffer);
+void fpb_buffer_destroy(fpb_buffer* buffer);
+
+/*
+ * fpb_index_append -- a new handle over `index` grown to n_docs >= N documents and n_tokens >= E tokens.  The
+ * caller has appended the new documents' data: d_doc_offsets (i64 [n_docs + 1]) starts with the old handle's N + 1
+ * offsets, and d_doc_codes / d_doc_residuals hold the old handle's E tokens followed by the new ones.  The arrays may
+ * be the old handle's own buffers grown in place (fpb_buffer_*) or copies.  d_token_norms holds the old handle's
+ * E norms; the norms of tokens [E, n_tokens) are computed here.  The walk layout is extended for the new documents
+ * only, in the old handle's shared buffers, and walk_group is re-chosen: both equal what fpb_index_create builds for
+ * the grown index.  d_ivf_offsets / d_ivf_pids / n_ivf are the grown index's inverted file (fpb_ivf_append), NULL /
+ * 0 for a compress_only index exactly when the old one has none; max_doc_len is the grown index's.
+ *
+ * The old handle stays valid and unchanged, so searches on it may continue.  Only a handle over all the documents
+ * laid out so far may append (appending twice to the same handle is refused).  Bad sizes, NULL pointers and an IVF
+ * that differs in kind from the old handle's are refused before any CUDA call; an offsets array whose entry N is not
+ * E, or whose entry n_docs is not n_tokens, is refused before any kernel.  Synchronous.
+ */
+int fpb_index_append(fpb_index** out, const fpb_index* index, int64_t n_docs, int64_t n_tokens,
+                     const int64_t* d_doc_offsets, const int32_t* d_doc_codes, const uint8_t* d_doc_residuals,
+                     void* d_token_norms, const int64_t* d_ivf_offsets, const int32_t* d_ivf_pids, int64_t n_ivf,
+                     int64_t max_doc_len);
+
+/*
+ * fpb_ivf_append -- the inverted file of an index of n_old_docs documents grown by n_new_docs documents (ids
+ * n_old_docs ..): for every one of the n_cells cells, its old list (d_ivf_offsets i64 [n_cells + 1] into d_ivf_pids)
+ * followed by the ascending ids of the new documents with a token in that cell.  The new documents' codes are
+ * d_new_codes (i32, d_new_offsets i64 [n_new_docs + 1] from 0).  Writes d_out_offsets (i64 [n_cells + 1]), sets
+ * *h_n_ivf to the number of postings and, unless d_out_pids is NULL (a call that sizes the output), writes them to
+ * d_out_pids (i32, room for out_capacity ids).  A code outside [0, n_cells) is refused.  Equal to building the
+ * inverted file of the whole index from scratch.  Synchronous on `stream`.
+ */
+int fpb_ivf_append(int device, int64_t n_cells, const int64_t* d_ivf_offsets, const int32_t* d_ivf_pids,
+                   int64_t n_old_docs, int64_t n_new_docs, const int64_t* d_new_offsets, const int32_t* d_new_codes,
+                   int64_t* d_out_offsets, int32_t* d_out_pids, int64_t out_capacity, int64_t* h_n_ivf,
+                   void* stream);
 
 /* Search parameters -- mirrors `SearchParameters` (rust/search/search.rs:171-200).
  * `batch_size` (document batch of the approximate stage) only bounds memory in the
