@@ -57,51 +57,6 @@ ivf_slab_kernel(const uint32_t* __restrict__ bitmap, int words, int64_t n_cells,
   }
 }
 
-// One block: out[c + 1] = old[c + 1] + (new postings of cells <= c), out[0] = 0, and cursor[c] = where the new ids of
-// cell c go, after its shifted old list.
-__global__ void __launch_bounds__(1024)
-ivf_offsets_kernel(const int64_t* __restrict__ old_offsets, const int64_t* __restrict__ count, int64_t n_cells,
-                   int64_t* __restrict__ out, int64_t* __restrict__ cursor) {
-  __shared__ int64_t s_warp[32];
-  __shared__ int64_t s_carry;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) {
-    s_carry = 0;
-    out[0] = 0;
-  }
-  __syncthreads();
-  for (int64_t c0 = 0; c0 < n_cells; c0 += 1024) {
-    const int64_t c = c0 + threadIdx.x;
-    const int64_t v = c < n_cells ? count[c] : 0;
-    int64_t incl = v;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int64_t u = __shfl_up_sync(0xffffffffu, incl, off);
-      if (lane >= off) incl += u;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      int64_t w = s_warp[lane];
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int64_t u = __shfl_up_sync(0xffffffffu, w, off);
-        if (lane >= off) w += u;
-      }
-      s_warp[lane] = w;
-    }
-    __syncthreads();
-    const int64_t before = s_carry + (warp > 0 ? s_warp[warp - 1] : 0) + incl - v;  // new postings of cells < c
-    if (c < n_cells) {
-      out[c + 1] = old_offsets[c + 1] + before + v;
-      cursor[c] = old_offsets[c + 1] + before;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) s_carry += s_warp[31];
-    __syncthreads();
-  }
-}
-
 // The old lists in their shifted places: posting i of cell c moves by out[c] - old[c].
 __global__ void __launch_bounds__(IVF_THREADS)
 ivf_shift_kernel(const int64_t* __restrict__ old_offsets, const int32_t* __restrict__ old_pids, int64_t n_cells,
@@ -115,12 +70,6 @@ ivf_shift_kernel(const int64_t* __restrict__ old_offsets, const int32_t* __restr
     }
     out_pids[i + out_offsets[lo] - old_offsets[lo]] = old_pids[i];
   }
-}
-
-int grid_for(int64_t items, int per_block, int sm_count) {
-  const int64_t need = (items + per_block - 1) / per_block;
-  const int64_t cap = int64_t(sm_count) * 16;
-  return int(need < 1 ? 1 : (need < cap ? need : cap));
 }
 
 }  // namespace
@@ -163,15 +112,15 @@ extern "C" int fpb_ivf_append(int device, int64_t n_cells, const int64_t* d_ivf_
   int64_t* count = reinterpret_cast<int64_t*>(scratch + bitmap_bytes);
   int64_t* cursor = reinterpret_cast<int64_t*>(scratch + bitmap_bytes + vec_bytes);
   int* bad = reinterpret_cast<int*>(scratch + bitmap_bytes + 2 * vec_bytes);
-  const int cell_grid = grid_for(n_cells, IVF_THREADS, sm_count);
+  const int cell_grid = fpb_grid_for(n_cells, IVF_THREADS, sm_count);
   auto run = [&]() -> int {
     FPB_CUDA_CHECK(cudaMemsetAsync(count, 0, n_cells * 8, st));
     FPB_CUDA_CHECK(cudaMemsetAsync(bad, 0, sizeof(int), st));
     // pass 1 counts each cell's new postings, pass 2 writes them; both rebuild every slab's bitmap
     for (int pass = 0; pass < 2; ++pass) {
       if (pass == 1) {
-        ivf_offsets_kernel<<<1, 1024, 0, st>>>(d_ivf_offsets, count, n_cells, d_out_offsets, cursor);
-        FPB_LAUNCH_CHECK("ivf_offsets");
+        // the new offsets, and cursor[c] = where the new ids of cell c go, after its shifted old list
+        FPB_TRY(launch_offsets_scan(d_ivf_offsets, count, n_cells, d_out_offsets, cursor, st));
         int64_t total = 0;
         int flag = 0;
         FPB_CUDA_CHECK(cudaMemcpyAsync(&total, d_out_offsets + n_cells, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
@@ -188,7 +137,7 @@ extern "C" int fpb_ivf_append(int device, int64_t n_cells, const int64_t* d_ivf_
           return FPB_ERR_INVALID;
         }
         if (n_old > 0) {
-          ivf_shift_kernel<<<grid_for(n_old, IVF_THREADS, sm_count), IVF_THREADS, 0, st>>>(
+          ivf_shift_kernel<<<fpb_grid_for(n_old, IVF_THREADS, sm_count), IVF_THREADS, 0, st>>>(
               d_ivf_offsets, d_ivf_pids, n_cells, n_old, d_out_offsets, d_out_pids);
           FPB_LAUNCH_CHECK("ivf_shift");
         }
@@ -196,7 +145,7 @@ extern "C" int fpb_ivf_append(int device, int64_t n_cells, const int64_t* d_ivf_
       for (int64_t d0 = 0; d0 < n_new_docs; d0 += slab) {
         const int64_t d1 = d0 + slab < n_new_docs ? d0 + slab : n_new_docs;
         FPB_CUDA_CHECK(cudaMemsetAsync(bitmap, 0, int64_t(words) * n_cells * 4, st));
-        ivf_mark_kernel<<<grid_for((d1 - d0) * 32, IVF_THREADS, sm_count), IVF_THREADS, 0, st>>>(
+        ivf_mark_kernel<<<fpb_grid_for((d1 - d0) * 32, IVF_THREADS, sm_count), IVF_THREADS, 0, st>>>(
             d_new_offsets, d_new_codes, d0, d1, n_cells, bitmap, bad);
         FPB_LAUNCH_CHECK("ivf_mark");
         ivf_slab_kernel<<<cell_grid, IVF_THREADS, 0, st>>>(bitmap, words, n_cells, n_old_docs + d0,

@@ -132,6 +132,17 @@ int launch_subset(const fpb_index* ix, const Ws& ws, const int32_t* d_ids, const
 int launch_compact(const uint32_t* bitmap, const uint32_t* mask, int words, int32_t* out, int cap, int32_t* n_out,
                    int B, cudaStream_t st);
 int launch_approx(const fpb_index* ix, const Ws& ws, int flags, cudaStream_t st); // K3 (flags: FPB_FLAG_APPROX_*)
+// One block scans count [n] (i64): out[0] = 0, out[c + 1] = old[c + 1] + count[0..c], and, when cursor is not NULL,
+// cursor[c] = out[c + 1] - count[c].  old == NULL reads as zeros.  The inverted file's new offsets (append, delete)
+// and the delete's rank tables (scan.cu).
+int launch_offsets_scan(const int64_t* old_offsets, const int64_t* count, int64_t n, int64_t* out, int64_t* cursor,
+                        cudaStream_t st);
+// blocks of a grid-stride loop over `items` items at `per_block` per block: at most 16 per SM, at least 1
+inline int fpb_grid_for(int64_t items, int per_block, int sm_count) {
+  const int64_t need = (items + per_block - 1) / per_block;
+  const int64_t cap = int64_t(sm_count) * 16;
+  return int(need < 1 ? 1 : (need < cap ? need : cap));
+}
 int launch_walk_layout(const fpb_index* ix, int64_t d0, cudaStream_t st);  // K3's walk_codes of documents [d0, N)
 // the walk layout of documents [d0, N) in ix->walk's buffers, and walk_group (index.cu)
 int fpb_extend_walk_layout(fpb_index* ix, int64_t d0);

@@ -104,6 +104,8 @@ EXPORTED_SYMBOLS = [
     "fpb_index_walk_group",
     "fpb_index_append",
     "fpb_ivf_append",
+    "fpb_docs_compact",
+    "fpb_ivf_delete",
     "fpb_buffer_reserve",
     "fpb_buffer_commit",
     "fpb_buffer_ptr",
@@ -188,6 +190,11 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_index_append.argtypes = [ctypes.POINTER(vp), vp, i64, i64, vp, vp, vp, vp, vp, vp, i64, i64]
         lib.fpb_ivf_append.restype = i32
         lib.fpb_ivf_append.argtypes = [i32, i64, vp, vp, i64, i64, vp, vp, vp, vp, i64, ctypes.POINTER(i64), vp]
+        lib.fpb_docs_compact.restype = i32
+        lib.fpb_docs_compact.argtypes = [i32, i64, vp, vp, vp, vp, i32, vp, i64, vp, vp, vp, vp, i64,
+                                         ctypes.POINTER(i64), vp]
+        lib.fpb_ivf_delete.restype = i32
+        lib.fpb_ivf_delete.argtypes = [i32, i64, vp, vp, i64, vp, i64, vp, vp, i64, ctypes.POINTER(i64), vp]
         lib.fpb_buffer_reserve.restype = i32
         lib.fpb_buffer_reserve.argtypes = [ctypes.POINTER(vp), i32, sz]
         lib.fpb_buffer_commit.restype = i32
@@ -887,10 +894,15 @@ class DeviceIndex:
                     v["residuals"].data_ptr(), v["norms"].data_ptr(), _ptr(ivf_offsets), _ptr(ivf_pids), n_ivf.value,
                     max_len))
                 arrays.n_docs, arrays.n_tokens = N1, E1
+        return self._successor(arrays, v, N1, E1, max_len, ivf_offsets, ivf_pids, handle)
+
+    def _successor(self, arrays: GrowableArrays, v: dict, n_docs: int, n_tokens: int, max_len: int,
+                   ivf_offsets: torch.Tensor | None, ivf_pids: torch.Tensor | None, handle) -> "DeviceIndex":
+        """A DeviceIndex with this one's codec over the arrays `v` of `arrays` and the fpb_index `handle`."""
         new = DeviceIndex.__new__(DeviceIndex)
         for name in ("_lib", "device", "nbits", "dim", "doc_id_base", "centroids", "bucket_weights", "num_centroids"):
             setattr(new, name, getattr(self, name))
-        new.num_documents, new.num_tokens, new.max_doc_len = N1, E1, max_len
+        new.num_documents, new.num_tokens, new.max_doc_len = n_docs, n_tokens, max_len
         new.doc_offsets, new.doc_codes, new.doc_residuals, new.token_norms = (
             v["offsets"], v["codes"], v["residuals"], v["norms"])
         new.ivf_offsets, new.ivf_pids = ivf_offsets, ivf_pids
@@ -898,6 +910,66 @@ class DeviceIndex:
         new._handle = handle
         new._init_state()
         return new
+
+    @torch.inference_mode()
+    def delete(self, doc_ids) -> "DeviceIndex":
+        """A new DeviceIndex over this index's documents without `doc_ids` (this index's ids; duplicates, negative
+        ids and ids >= num_documents are ignored), the rest renumbered in order, as ``delete_from_index`` leaves a
+        directory.  The kept documents' offsets and rows are compacted on the device into new growable buffers
+        (fpb_docs_compact), so the result can be appended to, and the inverted file of the kept documents is built
+        from this one's (fpb_ivf_delete); fpb_index_create then derives the token norms and the walk layout.  The
+        result equals a DeviceIndex loaded from the directory after the delete.
+
+        Nothing this index reads is written: it stays valid and searchable, and its results do not change.  Until it
+        is released both copies of the kept data are in memory.  A document shard (doc_id_base != 0) is refused."""
+        if self.doc_id_base != 0:
+            raise ValueError("delete: a document shard cannot delete in place (its range moves when the index "
+                             "shrinks); load the directory again instead")
+        dev, N = self.device, self.num_documents
+        ids = torch.as_tensor(list(doc_ids) if not isinstance(doc_ids, torch.Tensor) else doc_ids,
+                              dtype=torch.int64).reshape(-1).cpu()
+        drop = torch.unique(ids[(ids >= 0) & (ids < N)])  # sorted
+        n_drop, n_keep = int(drop.shape[0]), N - int(drop.shape[0])
+        pd = self.dim * self.nbits // 8
+        with torch.cuda.device(dev):
+            if getattr(self, "_handle", None) is None or not self._handle.value:
+                raise RuntimeError("this DeviceIndex has been closed")
+            d_drop = drop.to(dev, torch.int32) if n_drop else None
+            st = self._stream()
+            arrays = GrowableArrays(dev, pd)
+            offsets = arrays.offsets.view(torch.int64, (n_keep + 1,))
+            n_tok = ctypes.c_int64(0)
+            args = (dev.index, N, self.doc_offsets.data_ptr(), self.doc_codes.data_ptr(),
+                    self.doc_residuals.data_ptr(), None, pd, _ptr(d_drop), n_drop, offsets.data_ptr())
+            _check(self._lib.fpb_docs_compact(*args, None, None, None, 0, ctypes.byref(n_tok), st))  # sizes the rows
+            E1 = n_tok.value
+            v = arrays.views(n_keep, E1)
+            if E1 > 0:
+                _check(self._lib.fpb_docs_compact(*args, v["codes"].data_ptr(), v["residuals"].data_ptr(), None, E1,
+                                                  ctypes.byref(n_tok), st))
+            else:
+                v["codes"].zero_()
+                v["residuals"].zero_()
+            ivf_offsets = ivf_pids = None
+            n_ivf = ctypes.c_int64(0)
+            if self.has_ivf:
+                n_cells = int(self.ivf_offsets.shape[0]) - 1
+                ivf_offsets = torch.empty(n_cells + 1, dtype=torch.int64, device=dev)
+                args = (dev.index, n_cells, self.ivf_offsets.data_ptr(), self.ivf_pids.data_ptr(), N, _ptr(d_drop),
+                        n_drop, ivf_offsets.data_ptr())
+                _check(self._lib.fpb_ivf_delete(*args, None, 0, ctypes.byref(n_ivf), st))  # sizes the output
+                ivf_pids = torch.zeros(max(n_ivf.value, 1), dtype=torch.int32, device=dev)
+                _check(self._lib.fpb_ivf_delete(*args, ivf_pids.data_ptr(), ivf_pids.numel(), ctypes.byref(n_ivf), st))
+            max_len = int((v["offsets"][1:] - v["offsets"][:-1]).max()) if n_keep > 0 else 0
+            torch.cuda.current_stream(dev).synchronize()  # fpb_index_create works on the legacy default stream
+            handle = ctypes.c_void_p()
+            _check(self._lib.fpb_index_create(
+                ctypes.byref(handle), dev.index, self.nbits, self.dim, self.num_centroids, _ptr(self.centroids),
+                _ptr(self.bucket_weights), n_keep, v["offsets"].data_ptr(), v["codes"].data_ptr(),
+                v["residuals"].data_ptr(), v["norms"].data_ptr(), _ptr(ivf_offsets), _ptr(ivf_pids), n_ivf.value,
+                max_len, 0))
+            arrays.n_docs, arrays.n_tokens = n_keep, E1
+        return self._successor(arrays, v, n_keep, E1, max_len, ivf_offsets, ivf_pids, handle)
 
     # -- helpers -------------------------------------------------------------------------
     @staticmethod

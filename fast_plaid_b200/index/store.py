@@ -178,9 +178,15 @@ def write_chunk(index_path: str, chunk_index: int, codes: torch.Tensor, residual
     np.save(os.path.join(index_path, f"{chunk_index}.residuals.npy"), residuals.cpu().to(torch.uint8).numpy())
     with open(os.path.join(index_path, f"doclens.{chunk_index}.json"), "w") as f:
         json.dump([int(x) for x in doclens], f)
+    write_chunk_metadata(index_path, chunk_index, len(doclens), int(codes.shape[0]), embedding_offset)
+
+
+def write_chunk_metadata(index_path: str, chunk_index: int, num_documents: int, num_embeddings: int,
+                         embedding_offset: int) -> None:
+    """{i}.metadata.json of a chunk (create.rs:503-523)."""
     with open(os.path.join(index_path, f"{chunk_index}.metadata.json"), "w") as f:
         json.dump(
-            {"num_documents": len(doclens), "num_embeddings": int(codes.shape[0]),
+            {"num_documents": int(num_documents), "num_embeddings": int(num_embeddings),
              "embedding_offset": int(embedding_offset)},
             f, indent=2,
         )

@@ -162,6 +162,65 @@ def _rebuild_ivf(index_path: str, n_chunks: int, n_cells: int, dev: torch.device
 
 
 @torch.inference_mode()
+def delete_in_place(index_path: str, subset: list[int], device: str,
+                    loaded: dict[str, Any]) -> dict[str, Any] | None:
+    """What delete_from_index does, from the indexes already in HBM: `loaded` (device -> the DeviceIndex of the
+    directory as it is on disk) are compacted first (DeviceIndex.delete), on every device, and the compacted indexes
+    are returned.  Only then are files written, from the compacted arrays of `device`: every file of a chunk that
+    loses a document, the ``{i}.metadata.json`` of every later chunk (its embedding offset moves), the inverted file
+    and ``metadata.json``, last.  The directory ends byte for byte as delete_from_index leaves it, and chunks before
+    the first dropped document are not touched.
+
+    Returns None, having written nothing, when the delete would leave no document or the compaction fails: the
+    caller then runs delete_from_index."""
+    meta = store.read_metadata(index_path)
+    if meta is None:
+        raise RuntimeError("Failed to delete from index: metadata.json not found")
+    n_chunks = int(meta["num_chunks"])
+    chunks: list[tuple[int, list[int]]] = []  # (chunk, its document lengths) of every chunk delete_from_index reads
+    for i in range(n_chunks):
+        dl_path = os.path.join(index_path, f"doclens.{i}.json")
+        if os.path.exists(dl_path):
+            with open(dl_path) as f:
+                chunks.append((i, json.load(f)))
+    n_docs = sum(len(lens) for _, lens in chunks)
+    drop = sorted({int(d) for d in subset if 0 <= int(d) < n_docs})
+    compact = bool(meta.get("compress_only", False))
+    if len(drop) == n_docs or any(idx.num_documents != n_docs or idx.has_ivf == compact for idx in loaded.values()):
+        return None
+    try:
+        shrunk = {d: idx.delete(drop) for d, idx in loaded.items()}
+    except Exception as e:
+        print(f"Warning: deleting in place failed, the chunk files will be rewritten and the index loaded again: {e}")
+        return None
+    idx = shrunk[device]
+    offsets = idx.doc_offsets.cpu()
+    drop_t = torch.tensor(drop, dtype=torch.int64)
+    doc_base = new_base = 0
+    moved = False  # a document before this chunk was dropped: its embedding offset changes
+    for i, lens in chunks:
+        lo, hi = doc_base, doc_base + len(lens)
+        gone = drop_t[(drop_t >= lo) & (drop_t < hi)] - lo
+        n_kept = len(lens) - int(gone.shape[0])
+        t0, t1 = int(offsets[new_base]), int(offsets[new_base + n_kept])
+        if gone.numel():
+            keep = torch.ones(len(lens), dtype=torch.bool)
+            keep[gone] = False
+            new_lens = torch.tensor(lens, dtype=torch.int64)[keep].tolist()
+            store.write_chunk(index_path, i, idx.doc_codes[t0:t1], idx.doc_residuals[t0:t1], new_lens, t0)
+            moved = True
+        elif moved:
+            store.write_chunk_metadata(index_path, i, len(lens), t1 - t0, t0)
+        doc_base, new_base = hi, new_base + n_kept
+    n_cells = int(meta.get("num_partitions", 1))
+    if not compact:
+        _write_merged_ivf(index_path, idx, n_cells)
+    store.write_metadata(index_path, num_chunks=n_chunks, nbits=int(meta["nbits"]), num_partitions=n_cells,
+                         num_embeddings=int(offsets[-1]), num_documents=idx.num_documents, compress_only=compact)
+    return shrunk
+
+
+@torch.inference_mode()
 def delete_from_index(index_path: str, subset: list[int], device: str) -> None:
     """delete.rs:26-145: drop the documents, keep the chunk structure, rebuild the IVF."""
     meta = store.read_metadata(index_path)

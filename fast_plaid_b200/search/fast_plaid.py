@@ -415,10 +415,18 @@ class FastPlaid:
 
     @torch.inference_mode()
     def delete(self, subset: list[int], _delete_metadata: bool = True, _delete_buffer: bool = True) -> "FastPlaid":  # noqa: ARG002
-        """Remove documents and renumber the rest (fast_plaid.py:1045-1157, delete.rs:26-145)."""
+        """Remove documents and renumber the rest (fast_plaid.py:1045-1157, delete.rs:26-145).
+
+        The index already in HBM is compacted on the device (``DeviceIndex.delete``) and swapped in; only the chunk
+        files that lose a document are rewritten, and later chunks get a new ``{i}.metadata.json``.  Until the old
+        index is released (searches running meanwhile keep their results) the kept data is in memory twice.  The
+        chunk files are rewritten and the directory loaded again instead when the index is sharded, not loaded on
+        every CUDA device, changed on disk by another process since it was loaded, when the delete would leave no
+        document, or when the compaction fails."""
         from ..index import update as _update
 
         with self.lock:
+            loaded = self._appendable()
             # an index last updated by the reference may carry its buffer of recent raw documents (the most recent
             # ones, fast_plaid.py:1084-1091): trim it like the reference does (:1118-1145) so that a later update by
             # either implementation does not resurrect deleted documents
@@ -434,7 +442,12 @@ class FastPlaid:
                         save_list_tensors_on_disk(buffer_path, keep_b)
                     else:
                         os.remove(buffer_path)
-            _update.delete_from_index(self.index, subset, device=self.devices[0])
+            shrunk = None
+            if loaded is not None:
+                shrunk = _update.delete_in_place(self.index, subset, self.devices[0], loaded)
+                del loaded
+            if shrunk is None:
+                _update.delete_from_index(self.index, subset, device=self.devices[0])
             if os.path.exists(os.path.join(self.index, "metadata.db")) and _delete_metadata:
                 from ..filtering import delete as _meta_delete
 
@@ -449,7 +462,15 @@ class FastPlaid:
                         save_list_tensors_on_disk(emb_path, keep)
                     else:
                         os.remove(emb_path)
-            self._swap_in_fresh()
+            if shrunk is None:
+                self._swap_in_fresh()
+            else:
+                with self._index_swap_lock:
+                    old = self.indices
+                    self.indices = shrunk
+                    self._update_mtime()
+                    self._cpu_loaded = True
+                self._retire(old)
         return self
 
     # ------------------------------------------------------------------ search

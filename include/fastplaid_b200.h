@@ -136,6 +136,33 @@ int fpb_ivf_append(int device, int64_t n_cells, const int64_t* d_ivf_offsets, co
                    int64_t* d_out_offsets, int32_t* d_out_pids, int64_t out_capacity, int64_t* h_n_ivf,
                    void* stream);
 
+/*
+ * Deleting documents -- replaces `delete_from_index`'s filtering and renumbering (rust/index/delete.rs:26-145) on the
+ * device.  Both entry points take the dropped ids as d_drop (i32 [n_drop], sorted, unique, in [0, n_docs); ids out of
+ * order or out of range are refused before any row is written).  Kept documents keep their order; a kept document's
+ * new id is its old id minus the number of dropped ids below it.  The inputs are only read, so a handle over them
+ * stays valid.  Bad sizes and NULL pointers are refused before any CUDA call.  Synchronous on `stream`.
+ *
+ * fpb_docs_compact -- the kept documents of an index of n_docs documents (d_doc_offsets i64 [n_docs + 1]): writes
+ * their offsets to d_out_offsets (i64 [n_docs - n_drop + 1], from 0) and sets *h_n_tokens to their token count.
+ * Unless d_out_codes is NULL (a call that sizes the output), also copies their codes (i32), residual rows (u8, pd =
+ * 16, 32 or 64 bytes each, 16-byte aligned arrays) and, when both norm pointers are non-NULL, token norms (f16) into
+ * the out arrays (room for out_capacity tokens).  fpb_index_create on the compacted arrays computes the norms itself.
+ *
+ * fpb_ivf_delete -- the inverted file of the kept documents from the old one (d_ivf_offsets i64 [n_cells + 1] into
+ * d_ivf_pids): every cell's postings of kept documents, renumbered, in their order.  Writes d_out_offsets (i64
+ * [n_cells + 1]), sets *h_n_ivf to the number of postings and, unless d_out_pids is NULL (a call that sizes the
+ * output), writes them to d_out_pids (i32, room for out_capacity ids).  Equal to building the inverted file of the
+ * kept documents from scratch.
+ */
+int fpb_docs_compact(int device, int64_t n_docs, const int64_t* d_doc_offsets, const int32_t* d_doc_codes,
+                     const uint8_t* d_doc_residuals, const void* d_token_norms, int pd, const int32_t* d_drop,
+                     int64_t n_drop, int64_t* d_out_offsets, int32_t* d_out_codes, uint8_t* d_out_residuals,
+                     void* d_out_norms, int64_t out_capacity, int64_t* h_n_tokens, void* stream);
+int fpb_ivf_delete(int device, int64_t n_cells, const int64_t* d_ivf_offsets, const int32_t* d_ivf_pids,
+                   int64_t n_docs, const int32_t* d_drop, int64_t n_drop, int64_t* d_out_offsets, int32_t* d_out_pids,
+                   int64_t out_capacity, int64_t* h_n_ivf, void* stream);
+
 /* Search parameters -- mirrors `SearchParameters` (rust/search/search.rs:171-200).
  * `batch_size` (document batch of the approximate stage) only bounds memory in the
  * reference and does not change values (search.rs:558-586); it is accepted and ignored. */
