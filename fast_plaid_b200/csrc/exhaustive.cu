@@ -222,39 +222,25 @@ extern "C" int fpb_exhaustive_subset_workspace_bytes(const fpb_index* ix, int B,
   return FPB_OK;
 }
 
-extern "C" int fpb_search_exhaustive_subset(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
-                                            const int32_t* d_list_ids, const int64_t* d_list_offsets, int n_lists,
-                                            int64_t max_list_len, const int32_t* h_query_list, void* d_ws,
-                                            size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores,
-                                            int32_t* d_out_counts, void* stream) {
-  // shapes, then the lists, then the index
-  if (top_k < 1) {
-    fpb_set_error("fpb_search_exhaustive_subset: top_k=%d must be >= 1", top_k);
-    return FPB_ERR_INVALID;
-  }
-  FPB_TRY(check_exhaustive_shapes(B, Q, top_k));
-  FPB_TRY(check_lists(n_lists, max_list_len));
-  if (!h_query_list) {
-    fpb_set_error("fpb_search_exhaustive_subset: NULL h_query_list");
-    return FPB_ERR_INVALID;
-  }
-  for (int b = 0; b < B; ++b) {
-    if (h_query_list[b] < 0 || h_query_list[b] >= n_lists) {
-      fpb_set_error("fpb_search_exhaustive_subset: h_query_list[%d]=%d is not in [0, n_lists=%d)", b,
-                    h_query_list[b], n_lists);
-      return FPB_ERR_INVALID;
-    }
-  }
+namespace {
+
+// The list walk of fpb_search_exhaustive_subset and fpb_search_exhaustive_filter once their shapes and lists are
+// checked: the index and workspace checks, then the pointers (lists_ok: the list pointers are usable), the host
+// table, K7 over the lists, selection and ranking.
+int exhaustive_list_search(const char* who, const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
+                           const ExLists& lists, bool lists_ok, int n_lists, int64_t max_list_len,
+                           const int32_t* h_query_list,
+                           void* d_ws, size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores,
+                           int32_t* d_out_counts, void* stream) {
   ExLayout X;
   FPB_TRY(exhaustive_layout(ix, B, Q, top_k, &X, n_lists, max_list_len));
   FPB_TRY(check_workspace(X, d_ws, ws_bytes));
-  if (!d_queries || !d_list_offsets || (max_list_len > 0 && !d_list_ids) || !d_out_ids || !d_out_scores ||
-      !d_out_counts) {
-    fpb_set_error("fpb_search_exhaustive_subset: NULL query, list or output pointer");
+  if (!d_queries || !lists_ok || !d_out_ids || !d_out_scores || !d_out_counts) {
+    fpb_set_error("%s: NULL query, list or output pointer", who);
     return FPB_ERR_INVALID;
   }
   if ((reinterpret_cast<uintptr_t>(d_queries) & 15u) != 0) {
-    fpb_set_error("fpb_search_exhaustive_subset: queries must be 16-byte aligned");
+    fpb_set_error("%s: queries must be 16-byte aligned", who);
     return FPB_ERR_INVALID;
   }
 
@@ -290,8 +276,7 @@ extern "C" int fpb_search_exhaustive_subset(const fpb_index* ix, const void* d_q
   char* base = static_cast<char*>(d_ws);
   // pageable source: staged before the call returns, so the host table may go out of scope
   FPB_CUDA_CHECK(cudaMemcpyAsync(base + X.off_table, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
-  FPB_TRY(launch_exhaustive_list_scores(ix, X, base, static_cast<const __half*>(d_queries), d_list_ids,
-                                        d_list_offsets, max_list_len, st));
+  FPB_TRY(launch_exhaustive_list_scores(ix, X, base, static_cast<const __half*>(d_queries), lists, st));
   float* scores = reinterpret_cast<float*>(base + X.off_scores);
   int32_t* cand = reinterpret_cast<int32_t*>(base + X.off_cand);
   int32_t* n_cand = reinterpret_cast<int32_t*>(base + X.off_n_cand);
@@ -304,4 +289,74 @@ extern "C" int fpb_search_exhaustive_subset(const fpb_index* ix, const void* d_q
   FPB_TRY(launch_rank(sel_scores, sel_ids, n_sel, top_k, B, top_k, ix->doc_id_base, d_out_ids, d_out_scores,
                       d_out_counts, st));
   return FPB_OK;
+}
+
+}  // namespace
+
+extern "C" int fpb_search_exhaustive_subset(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
+                                            const int32_t* d_list_ids, const int64_t* d_list_offsets, int n_lists,
+                                            int64_t max_list_len, const int32_t* h_query_list, void* d_ws,
+                                            size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores,
+                                            int32_t* d_out_counts, void* stream) {
+  // shapes, then the lists, then the index
+  if (top_k < 1) {
+    fpb_set_error("fpb_search_exhaustive_subset: top_k=%d must be >= 1", top_k);
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(check_exhaustive_shapes(B, Q, top_k));
+  FPB_TRY(check_lists(n_lists, max_list_len));
+  if (!h_query_list) {
+    fpb_set_error("fpb_search_exhaustive_subset: NULL h_query_list");
+    return FPB_ERR_INVALID;
+  }
+  for (int b = 0; b < B; ++b) {
+    if (h_query_list[b] < 0 || h_query_list[b] >= n_lists) {
+      fpb_set_error("fpb_search_exhaustive_subset: h_query_list[%d]=%d is not in [0, n_lists=%d)", b,
+                    h_query_list[b], n_lists);
+      return FPB_ERR_INVALID;
+    }
+  }
+  const ExLists lists{d_list_ids, d_list_offsets, max_list_len, nullptr, 0};
+  return exhaustive_list_search("fpb_search_exhaustive_subset", ix, d_queries, B, Q, top_k, lists,
+                                d_list_offsets && (max_list_len == 0 || d_list_ids), n_lists, max_list_len,
+                                h_query_list, d_ws, ws_bytes, d_out_ids, d_out_scores, d_out_counts, stream);
+}
+
+extern "C" int fpb_exhaustive_filter_workspace_bytes(const fpb_index* ix, int B, int Q, int top_k, int n_filters,
+                                                     int64_t max_count, size_t* out) {
+  if (!out) {
+    fpb_set_error("fpb_exhaustive_filter_workspace_bytes: NULL output pointer");
+    return FPB_ERR_INVALID;
+  }
+  if (top_k < 1) {
+    fpb_set_error("fpb_exhaustive_filter_workspace_bytes: top_k=%d must be >= 1", top_k);
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(check_exhaustive_shapes(B, Q, top_k));
+  FPB_TRY(check_lists(n_filters, max_count));
+  ExLayout X;
+  FPB_TRY(exhaustive_layout(ix, B, Q, top_k, &X, n_filters, max_count));
+  *out = size_t(X.total_bytes);
+  return FPB_OK;
+}
+
+extern "C" int fpb_search_exhaustive_filter(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
+                                            const uint32_t* d_filters, int n_filters, int64_t n_bits,
+                                            int64_t max_count, const int32_t* h_query_filter, void* d_ws,
+                                            size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores,
+                                            int32_t* d_out_counts, void* stream) {
+  const char* who = "fpb_search_exhaustive_filter";
+  if (top_k < 1) {
+    fpb_set_error("%s: top_k=%d must be >= 1", who, top_k);
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(check_exhaustive_shapes(B, Q, top_k));
+  FPB_TRY(check_filter_args(who, d_filters, n_filters, n_bits, h_query_filter, B));
+  if (max_count < 0) {
+    fpb_set_error("%s: max_count=%lld must be >= 0", who, (long long)max_count);
+    return FPB_ERR_INVALID;
+  }
+  const ExLists lists{nullptr, nullptr, 0, d_filters, n_bits};
+  return exhaustive_list_search(who, ix, d_queries, B, Q, top_k, lists, true, n_filters, max_count, h_query_filter,
+                                d_ws, ws_bytes, d_out_ids, d_out_scores, d_out_counts, stream);
 }

@@ -567,16 +567,21 @@ int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, c
 }
 
 int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
-                                  const int32_t* d_list_ids, const int64_t* d_list_offsets, int64_t max_list_len,
-                                  cudaStream_t st) {
+                                  const ExLists& lists, cudaStream_t st) {
   const ExListTable t = ExListTable::at(reinterpret_cast<int32_t*>(ws + X.off_table), X.n_lists, X.B, X.n_rows);
   int32_t* ids = reinterpret_cast<int32_t*>(ws + X.off_lists);
   int32_t* count = reinterpret_cast<int32_t*>(ws + X.off_lcount);
   int32_t* chunk_pfx = reinterpret_cast<int32_t*>(ws + X.off_chunks);
   // 1. every list sorted and deduplicated: a document bitmap per list, compacted in id order
   uint32_t* bitmap = reinterpret_cast<uint32_t*>(ws + X.off_bitmap);
-  FPB_TRY(launch_doc_bitmap(ix, d_list_ids, d_list_offsets, max_list_len, X.n_lists, bitmap, X.words, st));
-  FPB_TRY(launch_compact(bitmap, nullptr, X.words, ids, int(X.cap), count, X.n_lists, st));
+  if (lists.d_filters) {
+    FPB_TRY(launch_filter_lists(ix, lists.d_filters, lists.n_bits, X.n_lists, bitmap, X.words, ids, int(X.cap), count,
+                                st));
+  } else {
+    FPB_TRY(launch_doc_bitmap(ix, lists.d_list_ids, lists.d_list_offsets, lists.max_list_len, X.n_lists, bitmap,
+                              X.words, st));
+    FPB_TRY(launch_compact(bitmap, nullptr, X.words, ids, int(X.cap), count, X.n_lists, st));
+  }
   const int dpc = k7_docs_per_chunk(ix, X.list_docs);
   k7_list_chunks_kernel<<<1, 1024, 0, st>>>(count, t, X.n_lists, dpc, chunk_pfx);
   FPB_LAUNCH_CHECK("k7_list_chunks");

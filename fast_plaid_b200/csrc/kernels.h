@@ -199,6 +199,23 @@ inline int launch_emit_records(const fpb_index* ix, const Ws& ws, fpb_record* d_
 int launch_doc_bitmap(const fpb_index* ix, const int32_t* d_ids, const int64_t* d_offsets, int64_t max_len,
                       int n_lists, uint32_t* bitmap, int words, cudaStream_t st);
 
+// ---- Filters (filter.cu): packed bitmaps over GLOBAL document ids, [n_filters, ceil(n_bits / 32)] uint32 ----------
+// The arguments every filtered entry point checks before any CUDA call: non-NULL bitmaps and map, 1 <= n_filters <=
+// 65535, n_bits >= 0, h_query_filter[b] in [0, n_filters) for b < B.  Sets the error (prefixed by `who`).
+int check_filter_args(const char* who, const uint32_t* d_filters, int n_filters, int64_t n_bits,
+                      const int32_t* h_query_filter, int B);
+// The filter stage of a search: the sbitmap / cbitmap rows of the workspace (FPB_FLAG_SUBSET) that subset_mark_kernel
+// builds from id lists, built once per distinct filter and copied to the other queries of the filter (no compaction)
+int launch_filter(const fpb_index* ix, const Ws& ws, const uint32_t* d_filters, int n_filters, int64_t n_bits,
+                  const int32_t* h_query_filter, cudaStream_t st);
+// whether the filter stage accumulates a row's centroid bitmap (cwords words) in shared memory
+bool fpb_filter_centroids_in_shared(const fpb_index* ix, int cwords);
+// The exhaustive search's lists from filter rows: list l is the index's range of filter l, as a document bitmap
+// [n_lists, words] and then its sorted local ids ids [n_lists, cap] and their numbers count [n_lists].  A list of more
+// than cap documents keeps its first cap.
+int launch_filter_lists(const fpb_index* ix, const uint32_t* d_filters, int64_t n_bits, int n_lists,
+                        uint32_t* bitmap, int words, int32_t* ids, int cap, int32_t* count, cudaStream_t st);
+
 // The shape limits of the exhaustive search: B >= 1, 1 <= Q <= 256, 0 <= top_k <= FPB_EX_MAX_TOP_K (top_k = 0: the
 // scores alone).  Sets the error and returns FPB_ERR_INVALID / FPB_ERR_UNSUPPORTED outside them.
 constexpr int FPB_EX_MAX_TOP_K = 4096;  // the k6_rank bound (one shared-memory bitonic sort per query)
@@ -244,7 +261,15 @@ struct ExListTable {
 
 int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
                              float* d_scores, cudaStream_t st);  // K7 + finalize
+// The documents of a list walk's lists: id lists (d_list_ids / d_list_offsets / max_list_len, launch_doc_bitmap), or
+// filter rows when d_filters is not NULL (launch_filter_lists)
+struct ExLists {
+  const int32_t* d_list_ids;
+  const int64_t* d_list_offsets;
+  int64_t max_list_len;
+  const uint32_t* d_filters;
+  int64_t n_bits;
+};
 // list walk: canonical lists, K7 over them, and the [B, cap] scores / candidates / counts of the layout
 int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* ws, const __half* d_queries,
-                                  const int32_t* d_list_ids, const int64_t* d_list_offsets, int64_t max_list_len,
-                                  cudaStream_t st);
+                                  const ExLists& lists, cudaStream_t st);

@@ -26,7 +26,45 @@ int search_batch(const fpb_index* ix, const void* d_queries, int B, int Q, const
   return launch_rank(ix, c.ws, p->top_k, d_out_ids, d_out_scores, d_out_counts, c.st);
 }
 
+// fpb_search_batch_filter: the filter stage in place of the subset stage, then the same stages
+int search_batch_filter(const fpb_index* ix, const void* d_queries, int B, int Q, const fpb_params* p,
+                        const uint32_t* d_filters, int n_filters, int64_t n_bits, const int32_t* h_query_filter,
+                        void* d_ws, size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
+                        void* stream) {
+  Call c;
+  FPB_TRY(c.begin(ix, B, Q, p, d_ws, ws_bytes, true, stream));
+  FPB_TRY(run_centroid_scores(ix, c.ws, d_queries, c.st));
+  FPB_TRY(launch_filter(ix, c.ws, d_filters, n_filters, n_bits, h_query_filter, c.st));
+  FPB_TRY(launch_subset_compact(ix, c.ws, c.st));
+  FPB_TRY(run_probe_to_select(ix, c.ws, true, c.st));
+  FPB_TRY(launch_maxsim(ix, c.ws, c.st));
+  return launch_rank(ix, c.ws, p->top_k, d_out_ids, d_out_scores, d_out_counts, c.st);
+}
+
+// the checks every filtered search entry point makes before any CUDA call
+int check_filter_search(const char* who, const fpb_params* p, const uint32_t* d_filters, int n_filters,
+                        int64_t n_bits, const int32_t* h_query_filter, int B) {
+  if (p && !(p->flags & FPB_FLAG_SUBSET)) {
+    fpb_set_error("%s: params->flags must contain FPB_FLAG_SUBSET", who);
+    return FPB_ERR_INVALID;
+  }
+  return check_filter_args(who, d_filters, n_filters, n_bits, h_query_filter, B);
+}
+
 }  // namespace
+
+extern "C" int fpb_search_batch_filter(const fpb_index* ix, const void* d_queries, int B, int Q, const fpb_params* p,
+                                       const uint32_t* d_filters, int n_filters, int64_t n_bits,
+                                       const int32_t* h_query_filter, void* d_ws, size_t ws_bytes,
+                                       int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, void* stream) {
+  if (!d_queries || !d_out_ids || !d_out_scores || !d_out_counts) {
+    fpb_set_error("fpb_search_batch_filter: NULL query or output pointer");
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(check_filter_search("fpb_search_batch_filter", p, d_filters, n_filters, n_bits, h_query_filter, B));
+  return search_batch_filter(ix, d_queries, B, Q, p, d_filters, n_filters, n_bits, h_query_filter, d_ws, ws_bytes,
+                             d_out_ids, d_out_scores, d_out_counts, stream);
+}
 
 extern "C" int fpb_search_batch(const fpb_index* ix, const void* d_queries, int B, int Q,
                                 const fpb_params* p, void* d_ws, size_t ws_bytes, int64_t* d_out_ids,
@@ -112,6 +150,24 @@ extern "C" int fpb_shard_subset_begin(const fpb_index* ix, const void* d_queries
   return FPB_OK;
 }
 
+extern "C" int fpb_shard_filter_begin(const fpb_index* ix, const void* d_queries, int B, int Q, const fpb_params* p,
+                                      const uint32_t* d_filters, int n_filters, int64_t n_bits,
+                                      const int32_t* h_query_filter, void* d_ws, size_t ws_bytes,
+                                      uint32_t* d_cbitmap_out, void* stream) {
+  if (!d_queries || !d_cbitmap_out) {
+    fpb_set_error("fpb_shard_filter_begin: NULL query or centroid-bitmap pointer");
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(check_filter_search("fpb_shard_filter_begin", p, d_filters, n_filters, n_bits, h_query_filter, B));
+  Call c;
+  FPB_TRY(c.begin(ix, B, Q, p, d_ws, ws_bytes, true, stream));
+  FPB_TRY(run_centroid_scores(ix, c.ws, d_queries, c.st));
+  FPB_TRY(launch_filter(ix, c.ws, d_filters, n_filters, n_bits, h_query_filter, c.st));
+  FPB_CUDA_CHECK(cudaMemcpyAsync(d_cbitmap_out, c.ws.cbitmap(), size_t(c.L.B) * c.L.cbitmap_words * 4,
+                                 cudaMemcpyDeviceToDevice, c.st));
+  return FPB_OK;
+}
+
 extern "C" int fpb_shard_subset_keys(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws,
                                      size_t ws_bytes, const uint32_t* d_all_cbitmaps, int n_shards,
                                      uint64_t* d_keys, void* stream) {
@@ -171,6 +227,15 @@ extern "C" int fpb_stage_subset(const fpb_index* ix, const int32_t* d_subset_ids
   Call c;
   FPB_TRY(c.begin(ix, B, Q, p, d_ws, ws_bytes, false, stream));
   return launch_subset(ix, c.ws, d_subset_ids, d_subset_offsets, max_subset_len, c.st);
+}
+extern "C" int fpb_stage_filter(const fpb_index* ix, const uint32_t* d_filters, int n_filters, int64_t n_bits,
+                                const int32_t* h_query_filter, int B, int Q, const fpb_params* p, void* d_ws,
+                                size_t ws_bytes, void* stream) {
+  FPB_TRY(check_filter_search("fpb_stage_filter", p, d_filters, n_filters, n_bits, h_query_filter, B));
+  Call c;
+  FPB_TRY(c.begin(ix, B, Q, p, d_ws, ws_bytes, false, stream));
+  FPB_TRY(launch_filter(ix, c.ws, d_filters, n_filters, n_bits, h_query_filter, c.st));
+  return launch_subset_compact(ix, c.ws, c.st);
 }
 extern "C" int fpb_stage_probe(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws,
                                size_t ws_bytes, void* stream) {

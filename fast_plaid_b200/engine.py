@@ -115,6 +115,13 @@ EXPORTED_SYMBOLS = [
     "fpb_search_batch",
     "fpb_search_batch_subset",
     "fpb_search_batch_host",
+    "fpb_filter_from_ids",
+    "fpb_filter_from_mask",
+    "fpb_search_batch_filter",
+    "fpb_stage_filter",
+    "fpb_shard_filter_begin",
+    "fpb_exhaustive_filter_workspace_bytes",
+    "fpb_search_exhaustive_filter",
     "fpb_stage_centroid_scores",
     "fpb_stage_subset",
     "fpb_stage_probe",
@@ -214,6 +221,23 @@ def load_library() -> ctypes.CDLL:
                                                 vp, vp, vp, vp]
         lib.fpb_stage_subset.restype = i32
         lib.fpb_stage_subset.argtypes = [vp, vp, vp, i64, i32, i32, ctypes.POINTER(FpbParams), vp, sz, vp]
+        lib.fpb_filter_from_ids.restype = i32
+        lib.fpb_filter_from_ids.argtypes = [i32, vp, i64, i32, vp, i64, vp, vp]
+        lib.fpb_filter_from_mask.restype = i32
+        lib.fpb_filter_from_mask.argtypes = [i32, vp, i32, i64, vp, vp]
+        lib.fpb_search_batch_filter.restype = i32
+        lib.fpb_search_batch_filter.argtypes = [vp, vp, i32, i32, ctypes.POINTER(FpbParams), vp, i32, i64, vp, vp, sz,
+                                                vp, vp, vp, vp]
+        lib.fpb_stage_filter.restype = i32
+        lib.fpb_stage_filter.argtypes = [vp, vp, i32, i64, vp, i32, i32, ctypes.POINTER(FpbParams), vp, sz, vp]
+        lib.fpb_shard_filter_begin.restype = i32
+        lib.fpb_shard_filter_begin.argtypes = [vp, vp, i32, i32, ctypes.POINTER(FpbParams), vp, i32, i64, vp, vp, sz,
+                                               vp, vp]
+        lib.fpb_exhaustive_filter_workspace_bytes.restype = i32
+        lib.fpb_exhaustive_filter_workspace_bytes.argtypes = [vp, i32, i32, i32, i32, i64, ctypes.POINTER(sz)]
+        lib.fpb_search_exhaustive_filter.restype = i32
+        lib.fpb_search_exhaustive_filter.argtypes = [vp, vp, i32, i32, i32, vp, i32, i64, i64, vp, vp, sz, vp, vp,
+                                                     vp, vp]
         lib.fpb_search_batch_host.restype = i32
         lib.fpb_search_batch_host.argtypes = [
             vp, vp, i32, i32, ctypes.POINTER(FpbParams), vp, sz, vp, vp, vp, vp, vp, vp, vp, vp,
@@ -321,6 +345,75 @@ def group_subsets(subset) -> tuple[list, list[int]]:
             by_object[id(s)] = l
         query_list.append(l)
     return lists, query_list
+
+
+@dataclasses.dataclass
+class Filter:
+    """Search filters in their device form: `bitmap` int32 [n_filters, ceil(n_bits / 32)] over GLOBAL document ids
+    (document i is bit i & 31 of word i >> 5; ids >= n_bits are never set) on the index's device, and the filter of
+    every query (`query_filter`, host ints).  Queries that share a filter share its expansion on the device."""
+    bitmap: torch.Tensor
+    query_filter: list[int]
+    n_bits: int
+
+    @property
+    def n_filters(self) -> int:
+        return int(self.bitmap.shape[0])
+
+    def queries(self, s: int, e: int) -> "Filter":
+        """The filters of queries s..e-1 (the same bitmaps)."""
+        return Filter(self.bitmap, self.query_filter[s:e], self.n_bits)
+
+    def call_rows(self, s: int, e: int) -> tuple[torch.Tensor, list[int]]:
+        """What one call over queries s..e-1 passes: the rows of the filters they use (a view when those rows are
+        contiguous, a gathered copy otherwise) and every query's index among them."""
+        used = sorted(set(self.query_filter[s:e]))
+        if used[-1] - used[0] + 1 == len(used):
+            rows = self.bitmap[used[0]:used[-1] + 1]
+        else:
+            rows = self.bitmap.index_select(0, torch.tensor(used, device=self.bitmap.device))
+        local = {f: i for i, f in enumerate(used)}
+        return rows, [local[f] for f in self.query_filter[s:e]]
+
+    @staticmethod
+    def from_ids(ids: torch.Tensor, n_bits: int, device: torch.device | str, num_queries: int) -> "Filter":
+        """ids: integer [L] (one filter for all num_queries queries) or [num_queries, L] (one per query), any device.
+        Any order; duplicates count once; ids outside [0, n_bits) are ignored (-1 pads a row)."""
+        device = torch.device(device)
+        rows = ids.reshape(1, -1) if ids.dim() == 1 else ids
+        F, L = int(rows.shape[0]), int(rows.shape[1])
+        flat = rows.to(device=device, dtype=torch.int64).contiguous().view(-1)
+        offs = torch.arange(F + 1, dtype=torch.int64, device=device) * L
+        words = (int(n_bits) + 31) // 32
+        bitmap = torch.empty((F, words), dtype=torch.int32, device=device)
+        with torch.cuda.device(device):
+            _check(load_library().fpb_filter_from_ids(
+                device.index or 0, flat.data_ptr() if flat.numel() else None, flat.numel(), F, offs.data_ptr(),
+                int(n_bits), bitmap.data_ptr(), torch.cuda.current_stream(device).cuda_stream))
+        return Filter(bitmap, [0] * num_queries if ids.dim() == 1 else list(range(F)), int(n_bits))
+
+    @staticmethod
+    def from_mask(mask: torch.Tensor, device: torch.device | str, num_queries: int) -> "Filter":
+        """mask: bool [n] (one filter for all num_queries queries) or [num_queries, n] (one per query), any device;
+        n_bits = n."""
+        device = torch.device(device)
+        rows = mask.reshape(1, -1) if mask.dim() == 1 else mask
+        F, n = int(rows.shape[0]), int(rows.shape[1])
+        m = rows.to(device=device, dtype=torch.bool).contiguous()
+        bitmap = torch.empty((F, (n + 31) // 32), dtype=torch.int32, device=device)
+        if m.numel():
+            with torch.cuda.device(device):
+                _check(load_library().fpb_filter_from_mask(device.index or 0, m.data_ptr(), F, n, bitmap.data_ptr(),
+                                                           torch.cuda.current_stream(device).cuda_stream))
+        return Filter(bitmap, [0] * num_queries if mask.dim() == 1 else list(range(F)), n)
+
+
+def _popcount(x: torch.Tensor) -> torch.Tensor:
+    """Set bits of every element of a non-negative int64 tensor holding 32-bit words."""
+    x = x - ((x >> 1) & 0x55555555)
+    x = (x & 0x33333333) + ((x >> 2) & 0x33333333)
+    x = (x + (x >> 4)) & 0x0F0F0F0F
+    return (x * 0x01010101 & 0xFFFFFFFF) >> 24
 
 
 def _require_cuda() -> None:
@@ -1035,13 +1128,41 @@ class DeviceIndex:
         ids = ids.clamp(-1, 2**31 - 1).to(torch.int32)
         return ids.to(self.device), offs.to(self.device), (max(lens) if lens else 0)
 
+    def _check_filter(self, filter: Filter, B: int) -> None:
+        if len(filter.query_filter) != B:
+            raise ValueError("Subset length must match number of queries.")
+        bad = [(b, f) for b, f in enumerate(filter.query_filter) if not 0 <= f < filter.n_filters]
+        if bad:
+            raise ValueError(f"query_filter[{bad[0][0]}]={bad[0][1]} is not in [0, n_filters={filter.n_filters})")
+        bm = filter.bitmap
+        if (bm.device != self.device or bm.dtype != torch.int32 or bm.dim() != 2 or not bm.is_contiguous()
+                or filter.n_bits < 0 or bm.shape[1] < (filter.n_bits + 31) // 32):
+            raise ValueError(f"expected contiguous filter bitmaps int32 [n_filters, >= ceil(n_bits / 32)] with "
+                             f"n_bits={filter.n_bits} on {self.device}, got {bm.dtype} {list(bm.shape)} on "
+                             f"{bm.device}{'' if bm.is_contiguous() else ' (not contiguous)'}")
+
+    def filter_counts(self, filter: Filter) -> torch.Tensor:
+        """int64 [n_filters] on this device: the documents of each filter inside this index's range of global ids."""
+        lo, hi = self.doc_id_base, min(self.doc_id_base + self.num_documents, filter.n_bits)
+        if hi <= lo:
+            return torch.zeros(filter.n_filters, dtype=torch.int64, device=self.device)
+        w0, w1 = lo >> 5, (hi + 31) >> 5
+        words = filter.bitmap[:, w0:w1].to(torch.int64) & 0xFFFFFFFF
+        keep = torch.full((w1 - w0,), 0xFFFFFFFF, dtype=torch.int64, device=self.device)
+        keep[0] &= (0xFFFFFFFF << (lo & 31)) & 0xFFFFFFFF
+        if hi & 31:
+            keep[-1] &= (1 << (hi & 31)) - 1
+        return _popcount(words & keep).sum(1)
+
     def search(
-        self, queries: torch.Tensor, params: FpbParams, subset: list[list[int]] | None = None
+        self, queries: torch.Tensor, params: FpbParams, subset: list[list[int]] | None = None,
+        filter: Filter | None = None,
     ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries: fp16 [B, Q, D] on this device.  Returns device tensors
         (ids int64 [B, top_k], scores f32 [B, top_k], counts int32 [B]).  Asynchronous.
         `subset`: per query a list of GLOBAL doc ids to restrict the search to
-        (search.rs:494-517, :544-547)."""
+        (search.rs:494-517, :544-547).  `filter`: the same restriction in device form (fpb_search_batch_filter);
+        for the same documents the result is the same bytes."""
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k = params.top_k
@@ -1054,12 +1175,32 @@ class DeviceIndex:
             if len(subset) != B:
                 raise ValueError("Subset length must match number of queries.")
             params = self.with_flags(params, FPB_FLAG_SUBSET)
+        if filter is not None:
+            self._check_filter(filter, B)
+            params = self.with_flags(params, FPB_FLAG_SUBSET)
         step = self.max_queries_per_call(Q, params)
+        if filter is not None:
+            step = min(step, 65535)  # the library's limit on filters per call
+        keep = []
         with self._exclusive(), torch.cuda.device(self.device):
             for s in range(0, B, step):
                 e = min(B, s + step)
                 buf, lay = self.workspace(e - s, Q, params)
-                if subset is None:
+                if filter is not None:
+                    # each call passes the filters of its own queries: at most e - s of them
+                    rows, local = filter.call_rows(s, e)
+                    keep.append(rows)
+                    h_map = (ctypes.c_int32 * (e - s))(*local)
+                    _check(
+                        self._lib.fpb_search_batch_filter(
+                            self._handle, queries[s:e].data_ptr(), e - s, Q, ctypes.byref(params),
+                            rows.data_ptr(), rows.shape[0], filter.n_bits, h_map, buf.data_ptr(),
+                            buf.numel(), ids[s:e].data_ptr(), scores[s:e].data_ptr(), counts[s:e].data_ptr(),
+                            self._stream(),
+                        )
+                    )
+                    self._keepalive = keep  # until the stream has consumed them
+                elif subset is None:
                     _check(
                         self._lib.fpb_search_batch(
                             self._handle, queries[s:e].data_ptr(), e - s, Q, ctypes.byref(params), buf.data_ptr(),
@@ -1153,14 +1294,18 @@ class DeviceIndex:
         return int(out.value)
 
     def search_exhaustive(self, queries: torch.Tensor, top_k: int, budget_bytes: int = 6 << 30,
-                          subset: list[list[int]] | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                          subset: list[list[int]] | torch.Tensor | None = None,
+                          filter: Filter | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Exact top_k over every document: (ids int64 [B, top_k] global, scores f32 [B, top_k], counts int32 [B]),
         the result contract of `search`.  The batch is split into calls whose workspace fits `budget_bytes`;
         the result does not depend on the split.  Asynchronous.
 
         `subset`: per query a list of GLOBAL doc ids (any order; duplicates and ids outside the index are ignored).
         Query b is then ranked among the documents of subset[b] only, with counts[b] = min(top_k, #documents), and
-        every score is the one `exhaustive_scores` gives the same document."""
+        every score is the one `exhaustive_scores` gives the same document.  `subset` may also be an integer tensor
+        [B, L] on this device, a row of ids per query (padded with any id outside the index, such as -1): each row is
+        then a list of its own, with no host list made.  `filter`: the restriction in device form
+        (fpb_search_exhaustive_filter); for the same documents the result is the same bytes."""
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k = int(top_k)
@@ -1168,6 +1313,15 @@ class DeviceIndex:
         scores = torch.empty((B, k), dtype=torch.float32, device=self.device)
         counts = torch.empty((B,), dtype=torch.int32, device=self.device)
         if B == 0:
+            return ids, scores, counts
+        if filter is not None:
+            self._check_filter(filter, B)
+            self._search_exhaustive_filter(queries, k, budget_bytes, filter, ids, scores, counts)
+            return ids, scores, counts
+        if isinstance(subset, torch.Tensor):
+            if subset.dim() != 2 or subset.shape[0] != B:
+                raise ValueError("Subset length must match number of queries.")
+            self._search_exhaustive_id_rows(queries, k, budget_bytes, subset, ids, scores, counts)
             return ids, scores, counts
         if subset is not None:
             if len(subset) != B:
@@ -1216,6 +1370,66 @@ class DeviceIndex:
                     )
                 )
                 keep.append((sid, soff))
+        self._keepalive = keep  # until the stream has consumed them
+
+    def _search_exhaustive_id_rows(self, queries: torch.Tensor, k: int, budget_bytes: int, rows: torch.Tensor,
+                                   ids: torch.Tensor, scores: torch.Tensor, counts: torch.Tensor) -> None:
+        """search_exhaustive with ids [B, L]: row b is query b's list, offsets built on the device."""
+        B, Q, _ = queries.shape
+        L = int(rows.shape[1])
+        # int32 like _subset_csr: an id past int32 is past every index and stays ignored
+        flat = rows.to(self.device).clamp(-1, 2**31 - 1).to(torch.int32).contiguous().view(-1)
+        if flat.numel() == 0:
+            flat = torch.full((1,), -1, dtype=torch.int32, device=self.device)
+        step = self._exhaustive_step(B, Q, k, budget_bytes, lambda b: self.exhaustive_subset_workspace_bytes(
+            b, Q, k, b, L))
+        step = min(step, 65535)  # the library's limit on lists per call
+        offs = torch.arange(step + 1, dtype=torch.int64, device=self.device) * L
+        with self._exclusive(), torch.cuda.device(self.device):
+            for s in range(0, B, step):
+                e = min(B, s + step)
+                h_list = (ctypes.c_int32 * (e - s))(*range(e - s))
+                buf = self._buffer(self.exhaustive_subset_workspace_bytes(e - s, Q, k, e - s, L))
+                _check(
+                    self._lib.fpb_search_exhaustive_subset(
+                        self._handle, queries[s:e].data_ptr(), e - s, Q, k, flat[s * L:].data_ptr(), offs.data_ptr(),
+                        e - s, L, h_list, buf.data_ptr(), buf.numel(), ids[s:e].data_ptr(), scores[s:e].data_ptr(),
+                        counts[s:e].data_ptr(), self._stream(),
+                    )
+                )
+        self._keepalive = (flat, offs)  # until the stream has consumed them
+
+    def exhaustive_filter_workspace_bytes(self, B: int, Q: int, top_k: int, n_filters: int, max_count: int) -> int:
+        """Workspace of fpb_search_exhaustive_filter."""
+        out = ctypes.c_size_t()
+        _check(self._lib.fpb_exhaustive_filter_workspace_bytes(self._handle, B, Q, top_k, n_filters, max_count,
+                                                               ctypes.byref(out)))
+        return int(out.value)
+
+    def _search_exhaustive_filter(self, queries: torch.Tensor, k: int, budget_bytes: int, filter: Filter,
+                                  ids: torch.Tensor, scores: torch.Tensor, counts: torch.Tensor) -> None:
+        """search_exhaustive with filters: each call passes the filters of its own queries, one list each."""
+        B, Q, _ = queries.shape
+        n_used = len(set(filter.query_filter))
+        max_count = int(self.filter_counts(filter).max())  # sizes the workspace: one synchronisation
+        step = self._exhaustive_step(B, Q, k, budget_bytes, lambda b: self.exhaustive_filter_workspace_bytes(
+            b, Q, k, min(b, n_used), max_count))
+        step = min(step, 65535)  # the library's limit on filters per call
+        keep = []
+        with self._exclusive(), torch.cuda.device(self.device):
+            for s in range(0, B, step):
+                e = min(B, s + step)
+                rows, local = filter.call_rows(s, e)
+                keep.append(rows)
+                h_map = (ctypes.c_int32 * (e - s))(*local)
+                buf = self._buffer(self.exhaustive_filter_workspace_bytes(e - s, Q, k, rows.shape[0], max_count))
+                _check(
+                    self._lib.fpb_search_exhaustive_filter(
+                        self._handle, queries[s:e].data_ptr(), e - s, Q, k, rows.data_ptr(), rows.shape[0],
+                        filter.n_bits, max_count, h_map, buf.data_ptr(), buf.numel(), ids[s:e].data_ptr(),
+                        scores[s:e].data_ptr(), counts[s:e].data_ptr(), self._stream(),
+                    )
+                )
         self._keepalive = keep  # until the stream has consumed them
 
     # -- document-sharded exhaustive search ------------------------------------------------------
@@ -1447,15 +1661,26 @@ class DeviceIndex:
                                                    buf.data_ptr(), buf.numel(), keys.data_ptr(), self._stream()))
         return keys
 
-    def shard_subset_begin(self, queries: torch.Tensor, params: FpbParams, subset: list[list[int]]) -> torch.Tensor:
+    def shard_subset_begin(self, queries: torch.Tensor, params: FpbParams, subset: list[list[int]] | None = None,
+                           filter: Filter | None = None) -> torch.Tensor:
         """Sharded search with a `subset`, step 1a: centroid scores and this shard's bitmaps.  Returns the
         shard's centroid bitmap, int32 [B, cbitmap_words], for the all-gather.  `params.flags` must carry
-        FPB_FLAG_SUBSET; `subset` holds GLOBAL document ids."""
+        FPB_FLAG_SUBSET; `subset` holds GLOBAL document ids.  `filter`: the restriction in device form over global
+        ids, of which this shard reads its own range (fpb_shard_filter_begin)."""
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         buf, lay = self.workspace(B, Q, params)
-        sid, soff, smax = self._subset_csr(subset, 0, B)
         cb = torch.empty((B, lay.cbitmap_words), dtype=torch.int32, device=self.device)
+        if filter is not None:
+            self._check_filter(filter, B)
+            h_map = (ctypes.c_int32 * B)(*filter.query_filter)
+            with self._exclusive(), torch.cuda.device(self.device):
+                _check(self._lib.fpb_shard_filter_begin(self._handle, queries.data_ptr(), B, Q, ctypes.byref(params),
+                                                        filter.bitmap.data_ptr(), filter.n_filters, filter.n_bits,
+                                                        h_map, buf.data_ptr(), buf.numel(), cb.data_ptr(),
+                                                        self._stream()))
+            return cb
+        sid, soff, smax = self._subset_csr(subset, 0, B)
         with self._exclusive(), torch.cuda.device(self.device):
             _check(self._lib.fpb_shard_subset_begin(self._handle, queries.data_ptr(), B, Q, ctypes.byref(params),
                                                     sid.data_ptr(), soff.data_ptr(), smax, buf.data_ptr(),
@@ -1510,12 +1735,13 @@ class DeviceIndex:
 
     # -- stage-level access for the parity tests and the roofline bench -------------------
     def run_stages(self, queries: torch.Tensor, params: FpbParams, upto: str = "rank",
-                   subset: list[list[int]] | None = None) -> dict[str, Any]:
-        """Run the pipeline stage by stage and return views of every intermediate."""
+                   subset: list[list[int]] | None = None, filter: Filter | None = None) -> dict[str, Any]:
+        """Run the pipeline stage by stage and return views of every intermediate.  With `subset` or `filter` the
+        "subset" / "filter" stage runs after centroid_scores, and the views include sbitmap, cbitmap and clist."""
         order = ["centroid_scores", "probe", "candidates", "approx", "select", "maxsim", "rank"]
-        if subset is not None:
+        if subset is not None or filter is not None:
             params = self.with_flags(params, FPB_FLAG_SUBSET)
-            order.insert(1, "subset")
+            order.insert(1, "subset" if filter is None else "filter")
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         buf, lay = self.workspace(B, Q, params)
@@ -1532,6 +1758,11 @@ class DeviceIndex:
                     _check(self._lib.fpb_stage_subset(self._handle, sid.data_ptr(), soff.data_ptr(), smax, B, Q, p,
                                                       buf.data_ptr(), buf.numel(), st))
                     torch.cuda.synchronize(self.device)
+                elif name == "filter":
+                    self._check_filter(filter, B)
+                    h_map = (ctypes.c_int32 * B)(*filter.query_filter)
+                    _check(self._lib.fpb_stage_filter(self._handle, filter.bitmap.data_ptr(), filter.n_filters,
+                                                      filter.n_bits, h_map, B, Q, p, buf.data_ptr(), buf.numel(), st))
                 elif name == "rank":
                     k = params.top_k
                     ids = torch.empty((B, k), dtype=torch.int64, device=self.device)
@@ -1589,6 +1820,13 @@ class DeviceIndex:
             "n_refine": v(lay.off_n_refine, B * 4, torch.int32, (B,)),
             "thresh": v(lay.off_thresh, B * 4, torch.float32, (B,)),
             "stats": v(lay.off_stats, 64, torch.int64, (8,)),
+            # subset / filter structures (FPB_FLAG_SUBSET)
+            **({} if not lay.flags & FPB_FLAG_SUBSET else {
+                "sbitmap": v(lay.off_sbitmap, B * lay.bitmap_words * 4, torch.int32, (B, lay.bitmap_words)),
+                "cbitmap": v(lay.off_cbitmap, B * lay.cbitmap_words * 4, torch.int32, (B, lay.cbitmap_words)),
+                "n_clist": v(lay.off_n_clist, B * 4, torch.int32, (B,)),
+                "clist": v(lay.off_clist, B * K * 4, torch.int32, (B, K)),
+            }),
         }
 
     def walk_layout(self) -> tuple[torch.Tensor, torch.Tensor]:

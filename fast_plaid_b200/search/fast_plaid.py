@@ -14,6 +14,7 @@ There is no CPU search path: ``device="cpu"`` can build / update / delete an ind
 
 from __future__ import annotations
 
+import dataclasses
 import gc
 import glob
 import json
@@ -35,7 +36,7 @@ except ImportError:  # pragma: no cover - filelock ships with the image
     FileLockTimeout = Exception  # type: ignore
 
 from .. import engine as _engine
-from ..engine import DeviceIndex, IndexTensors
+from ..engine import DeviceIndex, Filter, IndexTensors
 from ..index import build as _build
 from ..index import store as _store
 
@@ -66,6 +67,46 @@ try:  # CPython helper built next to the CUDA library (csrc/py/results.c); host 
     from .. import _fpb_results
 except ImportError:  # pragma: no cover - the build produces it
     _fpb_results = None
+
+
+@dataclasses.dataclass
+class _SubsetTensor:
+    """A `subset=` that takes the device filter path: integer ids [L] or a bool mask [num_documents] shared by the
+    batch, or one row of either per query ([B, L] / [B, num_documents]), on any device."""
+    data: torch.Tensor
+
+    @property
+    def per_query(self) -> bool:
+        return self.data.dim() == 2
+
+    def queries(self, s: int, e: int) -> "_SubsetTensor":
+        return _SubsetTensor(self.data[s:e]) if self.per_query else self
+
+    def to_filter(self, idx: DeviceIndex, num_queries: int) -> Filter:
+        """The filters on idx's device.  Id forms get n_bits = the end of idx's range of global ids: an id past it is
+        not in this index (a shard expands only its own range).  A mask covers the whole index."""
+        if self.data.dtype == torch.bool:
+            return Filter.from_mask(self.data, idx.device, num_queries)
+        return Filter.from_ids(self.data, idx.doc_id_base + idx.num_documents, idx.device, num_queries)
+
+
+def _sharded_num_documents(range_end: int, device: torch.device | str) -> int:
+    """The largest `range_end` over the ranks of the torch.distributed process group (collective)."""
+    import torch.distributed as dist
+
+    dev = device if dist.get_backend() == "nccl" else torch.device("cpu")
+    t = torch.tensor([int(range_end)], dtype=torch.int64, device=dev)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    return int(t.item())
+
+
+def _split_subset(subset, chunk: int, n_chunks: int) -> list:
+    """The subset of each chunk of `chunk` queries (several devices in one process)."""
+    if subset is None:
+        return [None] * n_chunks
+    if isinstance(subset, _SubsetTensor):
+        return [subset.queries(i * chunk, (i + 1) * chunk) for i in range(n_chunks)]
+    return [subset[i : i + chunk] for i in range(0, len(subset), chunk)]
 
 
 def _results_to_lists(ids: torch.Tensor, scores: torch.Tensor, counts: torch.Tensor) -> list[list[tuple[int, float]]]:
@@ -509,6 +550,40 @@ class FastPlaid:
             raise ValueError("Subset length must match number of queries.")
         return subset
 
+    @staticmethod
+    def _subset_tensor(subset, num_queries: int, num_documents) -> _SubsetTensor | None:
+        """The `subset=` forms that take the device filter path, checked: a tensor (integer ids [L] or [B, L], bool
+        mask [num_documents] or [B, num_documents]), one id, or one id list for the whole batch.  None for the other
+        forms (no subset, one list per query).  `num_documents()`: the documents of the index."""
+        if isinstance(subset, torch.Tensor):
+            if subset.dtype.is_floating_point or subset.dtype.is_complex:
+                raise ValueError(f"subset tensor must hold integer document ids or a bool mask, got {subset.dtype}")
+            if subset.dim() not in (1, 2):
+                raise ValueError(f"subset tensor must be 1-D (shared by the batch) or 2-D (one row per query), got "
+                                 f"shape {list(subset.shape)}")
+            if subset.dim() == 2 and subset.shape[0] != num_queries:
+                raise ValueError("Subset length must match number of queries.")
+            if subset.dtype == torch.bool:
+                n = num_documents()
+                if subset.shape[-1] != n:
+                    raise ValueError(f"subset mask of shape {list(subset.shape)} does not cover the index's "
+                                     f"{n} documents")
+            return _SubsetTensor(subset)
+        if isinstance(subset, int):
+            return _SubsetTensor(torch.tensor([subset], dtype=torch.int64))
+        if isinstance(subset, list) and subset and isinstance(subset[0], int):
+            return _SubsetTensor(torch.tensor(subset, dtype=torch.int64))
+        return None
+
+    def _num_documents(self, idx: DeviceIndex) -> int:
+        """Documents of the whole index, the length of a mask.  On a document-sharded index of several ranks it is
+        the largest end of the ranks' ranges (one all-reduce: every rank passes the same `subset=`, so every rank
+        reaches it); the metadata of an attached shard holds its own count only."""
+        end = idx.doc_id_base + idx.num_documents
+        if self.shard is None or self.shard[1] == 1:
+            return end
+        return _sharded_num_documents(end, idx.device)
+
     def _prepare_search(self, queries_embeddings, subset):
         """fast_plaid.py:743-795"""
         search_indices = self._loaded_indices()
@@ -527,7 +602,9 @@ class FastPlaid:
                     f"Index could not be loaded on device '{device}'. Check CUDA memory or device availability."
                 )
         queries_embeddings = self._as_query_tensor(queries_embeddings)
-        subset = self._per_query_subsets(subset, queries_embeddings.shape[0])
+        B = queries_embeddings.shape[0]
+        tensor = self._subset_tensor(subset, B, lambda: self._num_documents(search_indices[self.devices[0]]))
+        subset = tensor if tensor is not None else self._per_query_subsets(subset, B)
         return search_indices, queries_embeddings, subset
 
     def _search_device(self, idx: DeviceIndex, queries: torch.Tensor, params,
@@ -537,6 +614,11 @@ class FastPlaid:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         if self.shard is not None:
             return self._search_sharded(idx, queries, params, subset)
+        if isinstance(subset, _SubsetTensor):
+            q16 = queries.to(torch.float16).to(idx.device)
+            filt = subset.to_filter(idx, q16.shape[0])
+            ids, scores, counts = idx.search(q16, params, filter=filt)
+            return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         if subset is not None:
             q16 = queries.to(torch.float16).to(idx.device)
             ids, scores, counts = idx.search(q16, params, subset=subset)
@@ -594,7 +676,11 @@ class FastPlaid:
         # the subset documents touch (search.rs:494-517); with sharded documents that set is the union of the
         # shards' centroid bitmaps
         params = DeviceIndex.with_flags(params, _engine.FPB_FLAG_SUBSET)
-        cbitmap = idx.shard_subset_begin(q16, params, subset)
+        if isinstance(subset, _SubsetTensor):  # each shard expands its own range of the global bitmaps
+            filt = subset.to_filter(idx, q16.shape[0])
+            cbitmap = idx.shard_subset_begin(q16, params, filter=filt)
+        else:
+            cbitmap = idx.shard_subset_begin(q16, params, subset)
         all_keys = all_gather(idx.shard_subset_keys(all_gather(cbitmap), int(q16.shape[1]), params))
         # step 2: exact scores of the globally surviving documents only, all-gather of the records
         rec = idx.shard_exact_records(all_keys, rank, int(q16.shape[1]), params)
@@ -614,7 +700,15 @@ class FastPlaid:
         n_processes: int | None = None,  # noqa: ARG002  (CPU-only knob in the reference)
     ) -> list[list[tuple[int, float]]]:
         """Search the index (fast_plaid.py:930-983).  Returns, per query, up to ``top_k``
-        ``(doc_id, score)`` pairs in rank order."""
+        ``(doc_id, score)`` pairs in rank order.
+
+        ``subset`` restricts the search to a set of documents.  ``None`` or ``[]``: no restriction.  One id or one
+        id list: the set of every query.  A list of lists: one set per query.  A tensor on any device: integer ids
+        ``[L]`` (the set of every query) or ``[B, L]`` (one row per query, padded with any id outside the index such
+        as -1), or a bool mask ``[num_documents]`` (every query) or ``[B, num_documents]`` (one per query).  Order
+        and duplicates do not matter and unknown ids are ignored.  Everything but a list of lists becomes a bitmap
+        on the GPU, and queries that share one share its expansion; the result is the one the same sets give as
+        lists of lists."""
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
         params = DeviceIndex.make_params(top_k, n_full_scores, n_ivf_probe, batch_size)
         if len(self.devices) == 1:
@@ -624,7 +718,7 @@ class FastPlaid:
         n = len(self.devices)
         chunk = math.ceil(queries.shape[0] / n)
         chunks = list(torch.split(queries, chunk))
-        sub_chunks = [None] * len(chunks) if subset is None else [subset[i : i + chunk] for i in range(0, len(subset), chunk)]
+        sub_chunks = _split_subset(subset, chunk, len(chunks))
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
                 ex.submit(self._search_device, search_indices[d], chunks[i], params, sub_chunks[i])
@@ -641,7 +735,14 @@ class FastPlaid:
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         q16 = queries.to(device=idx.device, dtype=torch.float16)  # the fp16 cast of `search` (fast_plaid.py:241)
-        ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset)
+        if isinstance(subset, _SubsetTensor) and subset.per_query and subset.data.dtype != torch.bool:
+            # candidate rows to re-rank: each row is a list of the list walk as it stands
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset.data.to(idx.device))
+        elif isinstance(subset, _SubsetTensor):
+            filt = subset.to_filter(idx, q16.shape[0])
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, filter=filt)
+        else:
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
     def _exhaustive_sharded_step(self, idx: DeviceIndex, B: int, Q: int, top_k: int, budget_bytes: int) -> int:
@@ -693,8 +794,8 @@ class FastPlaid:
         Queries take the forms ``search`` accepts.  ``top_k`` <= 4096.
 
         ``subset`` restricts each query to a set of documents, in the forms ``search`` accepts: one id, one id list
-        for every query (e.g. the result of ``filtering.where``), or one list per query (e.g. first-stage candidates
-        to re-rank); ``None`` or ``[]`` means no restriction.  Order and duplicates do not matter and unknown ids are
+        for every query (e.g. the result of ``filtering.where``), one list per query (e.g. first-stage candidates
+        to re-rank), or the tensor forms; ``None`` or ``[]`` means no restriction.  Order and duplicates do not matter and unknown ids are
         ignored.  A query then gets the ``min(top_k, #documents)`` best of its set, each with the score the
         unrestricted search gives that document: restricting to a subset is the full exhaustive ranking filtered to
         the subset.  The cost grows with the listed documents rather than the index; queries that share a list share
@@ -734,7 +835,7 @@ class FastPlaid:
         n = len(self.devices)
         chunk = math.ceil(queries.shape[0] / n)
         chunks = list(torch.split(queries, chunk))
-        sub_chunks = [None] * len(chunks) if subset is None else [subset[i : i + chunk] for i in range(0, len(subset), chunk)]
+        sub_chunks = _split_subset(subset, chunk, len(chunks))
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
                 ex.submit(self._search_exhaustive_device, search_indices[d], chunks[i], top_k, sub_chunks[i])

@@ -263,6 +263,31 @@ int fpb_search_batch_subset(const fpb_index* index, const void* d_queries, int B
                             size_t workspace_bytes, int64_t* d_out_ids, float* d_out_scores,
                             int32_t* d_out_counts, void* stream);
 
+/* ---- Filters: one device form for every `subset=` form ----
+ * A filter is a packed bitmap over GLOBAL document ids: row f of d_bitmap [n_filters, ceil(n_bits / 32)] uint32,
+ * bit (id & 31) of word (id >> 5) set when document `id` is in filter f.  Ids >= n_bits are never set.
+ *   fpb_filter_from_ids   d_ids i64 [n_ids], row f owning [d_row_offsets[f], d_row_offsets[f+1]) (device i64
+ *                         [n_filters + 1]); any order, duplicates count once, ids outside [0, n_bits) and elements
+ *                         outside every row are ignored.  The bitmap is cleared first.
+ *   fpb_filter_from_mask  d_mask [n_filters, n_bits] bytes (bool / uint8, nonzero = set), one ballot per word.
+ * Both refuse NULL pointers, n_filters < 1 and n_bits < 0 before any CUDA call; n_bits = 0 writes nothing. */
+int fpb_filter_from_ids(int device, const int64_t* d_ids, int64_t n_ids, int n_filters, const int64_t* d_row_offsets,
+                        int64_t n_bits, uint32_t* d_bitmap, void* stream);
+int fpb_filter_from_mask(int device, const uint8_t* d_mask, int n_filters, int64_t n_bits, uint32_t* d_bitmap,
+                         void* stream);
+
+/* fpb_search_batch_subset with query b restricted to filter h_query_filter[b] (HOST i32 [B], each in
+ * [0, n_filters); read during the call only) of d_filters [n_filters, ceil(n_bits / 32)].  The document bitmap and
+ * the centroid bitmap of the subset stage are built once per distinct filter and copied to the other queries of
+ * that filter; everything after them is the subset search's.  For the same documents the result is the bytes of
+ * fpb_search_batch_subset.  params->flags must contain FPB_FLAG_SUBSET; the workspace is fpb_workspace_layout's.
+ * NULL pointers, n_filters outside [1, 65535], n_bits < 0, a map entry out of range and a missing FPB_FLAG_SUBSET are
+ * refused before any CUDA call. */
+int fpb_search_batch_filter(const fpb_index* index, const void* d_queries, int B, int Q, const fpb_params* params,
+                            const uint32_t* d_filters, int n_filters, int64_t n_bits, const int32_t* h_query_filter,
+                            void* d_workspace, size_t workspace_bytes, int64_t* d_out_ids, float* d_out_scores,
+                            int32_t* d_out_counts, void* stream);
+
 /* Same call with HOST buffers: H2D of the queries, the search, D2H of the results and a
  * stream synchronise all happen inside.  d_out_* are device scratch of the same shapes. */
 int fpb_search_batch_host(const fpb_index* index, const void* h_queries, int B, int Q,
@@ -278,6 +303,9 @@ int fpb_stage_centroid_scores(const fpb_index*, const void* d_queries, int B, in
 int fpb_stage_subset(const fpb_index*, const int32_t* d_subset_ids, const int64_t* d_subset_offsets,
                      int64_t max_subset_len, int B, int Q, const fpb_params*, void* d_workspace, size_t,
                      void* stream); /* search.rs:496-503: run between centroid_scores and probe */
+int fpb_stage_filter(const fpb_index*, const uint32_t* d_filters, int n_filters, int64_t n_bits,
+                     const int32_t* h_query_filter, int B, int Q, const fpb_params*, void* d_workspace, size_t,
+                     void* stream); /* the filter form of fpb_stage_subset (fpb_search_batch_filter) */
 int fpb_stage_probe(const fpb_index*, int B, int Q, const fpb_params*, void* d_workspace,
                     size_t, void* stream); /* search.rs:520-532 */
 int fpb_stage_candidates(const fpb_index*, int B, int Q, const fpb_params*, void* d_workspace,
@@ -340,6 +368,11 @@ int fpb_shard_subset_begin(const fpb_index* index, const void* d_queries, int B,
                            const fpb_params* params, const int32_t* d_subset_ids,
                            const int64_t* d_subset_offsets, int64_t max_subset_len, void* d_workspace,
                            size_t workspace_bytes, uint32_t* d_cbitmap_out, void* stream);
+/* 1a with filters (fpb_search_batch_filter's arguments): each shard expands only its own range
+ * [doc_id_base, doc_id_base + n_docs) of the global bitmaps.  Then 1b and the later steps as above. */
+int fpb_shard_filter_begin(const fpb_index* index, const void* d_queries, int B, int Q, const fpb_params* params,
+                           const uint32_t* d_filters, int n_filters, int64_t n_bits, const int32_t* h_query_filter,
+                           void* d_workspace, size_t workspace_bytes, uint32_t* d_cbitmap_out, void* stream);
 int fpb_shard_subset_keys(const fpb_index* index, int B, int Q, const fpb_params* params, void* d_workspace,
                           size_t workspace_bytes, const uint32_t* d_all_cbitmaps /* [n_shards, B, words] */,
                           int n_shards, uint64_t* d_keys /* [B, R] */, void* stream);
@@ -430,6 +463,21 @@ int fpb_search_exhaustive_subset(const fpb_index* index, const void* d_queries, 
                                  int64_t max_list_len, const int32_t* h_query_list, void* d_workspace,
                                  size_t workspace_bytes, int64_t* d_out_ids, float* d_out_scores,
                                  int32_t* d_out_counts, void* stream);
+
+/* fpb_search_exhaustive_subset with filters (fpb_search_batch_filter's d_filters / n_filters / n_bits /
+ * h_query_filter): list l is this index's range of filter l, so every query of a filter shares one decode of its
+ * documents.  max_count bounds the set documents of every filter inside [doc_id_base, doc_id_base + n_docs): it
+ * sizes the workspace like max_list_len.  A filter with more documents in the range than max_count is cut to its
+ * first max_count of them (in id order), so its queries are ranked among those only: pass the exact maximum (or
+ * more) for the full result.
+ * Results and limits are those of fpb_search_exhaustive_subset (n_filters <= 65535).
+ * fpb_exhaustive_filter_workspace_bytes: the workspace of a call with these shapes and filters. */
+int fpb_exhaustive_filter_workspace_bytes(const fpb_index* index, int B, int Q, int top_k, int n_filters,
+                                          int64_t max_count, size_t* out);
+int fpb_search_exhaustive_filter(const fpb_index* index, const void* d_queries, int B, int Q, int top_k,
+                                 const uint32_t* d_filters, int n_filters, int64_t n_bits, int64_t max_count,
+                                 const int32_t* h_query_filter, void* d_workspace, size_t workspace_bytes,
+                                 int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, void* stream);
 
 /* Exhaustive search on a document-sharded index: the result of fpb_search_exhaustive on one GPU holding the whole
  * index, byte for byte (global ids in rank order, counts = min(top_k, total documents), tails id -1 / score -inf).
