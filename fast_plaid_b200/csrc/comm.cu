@@ -138,6 +138,7 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
                                         int B, int Q, const fpb_params* p, void* d_ws, size_t ws_bytes, void* d_scratch,
                                         size_t scratch_bytes, int64_t* d_out_ids, float* d_out_scores,
                                         int32_t* d_out_counts, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_search_batch_sharded", ix));
   if (!ix || !comm || !p || !d_queries || !d_ws || !d_scratch || !d_out_ids || !d_out_scores || !d_out_counts) {
     fpb_set_error("fpb_search_batch_sharded: NULL argument");
     return FPB_ERR_INVALID;
@@ -219,6 +220,7 @@ extern "C" int fpb_search_exhaustive_sharded(const fpb_index* ix, fpb_comm* comm
                                              size_t ws_bytes, void* d_scratch, size_t scratch_bytes,
                                              int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
                                              void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_search_exhaustive_sharded", ix));
   // every refusal comes before the collective and depends only on arguments every rank has in common (the
   // workspace and the scratch are sized per rank by the caller): shapes, pointers, grid, merge limit
   if (top_k < 1) {

@@ -73,6 +73,10 @@ struct fpb_index {
   // (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint; has_tmap = 0 if unavailable)
   alignas(64) unsigned char tmap_centroids[128];
   int has_tmap;
+  // grouped results (fpb_index_with_groups, groups.cu): the group of every local document, [N] in [0, n_groups),
+  // borrowed like the other arrays; NULL / 0 on a handle without groups
+  const int32_t* doc_group;
+  int64_t n_groups;
 };
 
 void fpb_set_error(const char* fmt, ...);

@@ -75,6 +75,10 @@ int exhaustive_layout(const fpb_index* ix, int B, int Q, int top_k, ExLayout* X,
     X->off_cand = take(int64_t(B) * cap * 4);
     X->off_n_cand = take(int64_t(B) * 4);
   }
+  if (sel && ix->doc_group) {
+    const int64_t cols = lists ? cap : N;  // accumulator entries per query
+    X->off_gkeys = ix->n_groups <= cols ? X->off_acc : take(int64_t(B) * ix->n_groups * 8);
+  }
   X->total_bytes = off;
   return FPB_OK;
 }
@@ -143,12 +147,24 @@ extern "C" int fpb_exhaustive_scores(const fpb_index* ix, const void* d_queries,
 namespace {
 
 // The selected lists of a full scan, in the workspace: per query the n_sel[b] best local documents (ids, scores)
-// by (score desc, id asc), rows of stride top_k.
+// by (score desc, id asc), rows of stride top_k.  On a handle with groups nothing is selected: all_scores holds the
+// [B, N] scores and gkeys the group keys' room.
 struct ExSelected {
   int32_t* n_sel;
   int32_t* ids;
   float* scores;
+  float* all_scores;
+  uint64_t* gkeys;
 };
+
+// The grouped ranking of exact search: the group maximum over the [B, cols] scores, then the top_k groups
+int rank_groups(const fpb_index* ix, const float* scores, const int32_t* cand, const int32_t* n, int64_t cols, int B,
+                int top_k, uint64_t* gkeys, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
+                cudaStream_t st) {
+  FPB_TRY(launch_group_max(scores, cand, n, cols, B, ix->doc_group, ix->n_groups, gkeys, ix->sm_count, st));
+  return launch_group_select(gkeys, ix->n_groups, B, top_k, ix->doc_id_base, d_out_ids, d_out_scores, d_out_counts,
+                             st);
+}
 
 // The checks and the whole computation of a full-scan search up to its selected lists: K7 scores every document,
 // k3b_select keeps the top_k of each query with every document a candidate.
@@ -175,7 +191,10 @@ int exhaustive_select(const char* who, const fpb_index* ix, const void* d_querie
   out->n_sel = reinterpret_cast<int32_t*>(base + X.off_n_rerank);
   out->ids = reinterpret_cast<int32_t*>(base + X.off_rerank);
   out->scores = reinterpret_cast<float*>(base + X.off_rerank_approx);
+  out->all_scores = scores;
+  out->gkeys = reinterpret_cast<uint64_t*>(base + X.off_gkeys);
   FPB_TRY(launch_exhaustive_scores(ix, X, base, static_cast<const __half*>(d_queries), scores, st));
+  if (ix->doc_group) return FPB_OK;
   // every document is a candidate, and its "approximate" score is its exact one: the selected list holds the exact
   // scores that k6_rank orders
   return launch_select(scores, nullptr, nullptr, int(ix->N), B, top_k, out->ids, out->scores, out->n_sel, st);
@@ -190,12 +209,16 @@ extern "C" int fpb_search_exhaustive(const fpb_index* ix, const void* d_queries,
   ExSelected sel;
   FPB_TRY(exhaustive_select("fpb_search_exhaustive", ix, d_queries, B, Q, top_k, d_ws, ws_bytes,
                             d_out_ids && d_out_scores && d_out_counts, st, &sel));
+  if (ix->doc_group)
+    return rank_groups(ix, sel.all_scores, nullptr, nullptr, ix->N, B, top_k, sel.gkeys, d_out_ids, d_out_scores,
+                       d_out_counts, st);
   return launch_rank(sel.scores, sel.ids, sel.n_sel, top_k, B, top_k, ix->doc_id_base, d_out_ids, d_out_scores,
                      d_out_counts, st);
 }
 
 extern "C" int fpb_shard_exhaustive_records(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
                                             void* d_ws, size_t ws_bytes, fpb_record* d_records, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_shard_exhaustive_records", ix));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ExSelected sel;
   FPB_TRY(exhaustive_select("fpb_shard_exhaustive_records", ix, d_queries, B, Q, top_k, d_ws, ws_bytes,
@@ -280,6 +303,9 @@ int exhaustive_list_search(const char* who, const fpb_index* ix, const void* d_q
   float* scores = reinterpret_cast<float*>(base + X.off_scores);
   int32_t* cand = reinterpret_cast<int32_t*>(base + X.off_cand);
   int32_t* n_cand = reinterpret_cast<int32_t*>(base + X.off_n_cand);
+  if (ix->doc_group)
+    return rank_groups(ix, scores, cand, n_cand, X.cap, B, top_k, reinterpret_cast<uint64_t*>(base + X.off_gkeys),
+                       d_out_ids, d_out_scores, d_out_counts, st);
   int32_t* n_sel = reinterpret_cast<int32_t*>(base + X.off_n_rerank);
   int32_t* sel_ids = reinterpret_cast<int32_t*>(base + X.off_rerank);
   float* sel_scores = reinterpret_cast<float*>(base + X.off_rerank_approx);

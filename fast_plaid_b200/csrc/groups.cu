@@ -1,0 +1,368 @@
+// Grouped results (DESIGN §7): each query returns at most one document per group, the group's best under the
+// canonical order (score desc, then id asc), and these representatives in the canonical order.  A handle made by
+// fpb_index_with_groups carries the group of every local document, dense ids in [0, n_groups).
+//   - The re-ranked list of a search (<= 4096 documents per query): K6's canonical sort, then the first entry of
+//     each group, kept in rank order (k6_rank_grouped_kernel).
+//   - Exact search: the maximum canonical key of every (query, group) pair over the exact scores (group_max_kernel),
+//     then the top_k largest of those keys per query (group_select_kernel).  The maximum key is the group's
+//     canonical best document, and a maximum does not depend on the order of the atomics.
+// A group id outside [0, n_groups) is skipped: the host remap never makes one, but the C ABI is public.
+#include "kernels.h"
+#include "select.cuh"
+
+namespace {
+
+// Exclusive prefix of the threads' counts c over a 1024-thread block; *total gets the sum.  warp_sums: 32 ints of
+// shared memory.  Contains two __syncthreads().
+__device__ __forceinline__ int block_exclusive_scan(int c, int* warp_sums, int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int incl = c;
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+    const int v = __shfl_up_sync(0xffffffffu, incl, off);
+    if (lane >= off) incl += v;
+  }
+  if (lane == 31) warp_sums[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    const int ws = warp_sums[lane];
+    int wincl = ws;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, wincl, off);
+      if (lane >= off) wincl += v;
+    }
+    warp_sums[lane] = wincl - ws;
+    if (lane == 31) *total = wincl;
+  }
+  __syncthreads();
+  return warp_sums[warp] + incl - c;
+}
+
+__device__ __forceinline__ bool group_ok(int32_t g, int64_t n_groups) { return g >= 0 && int64_t(g) < n_groups; }
+
+// Grouped K6, one CTA per query: row b of exact / rerank (stride R) holds the scores and local ids of n_rerank[b]
+// documents.  Shared memory: the canonical keys [Rp2], then (group, rank position) keys [Rp2].
+__global__ void __launch_bounds__(1024)
+k6_rank_grouped_kernel(const float* __restrict__ exact, const int32_t* __restrict__ rerank,
+                       const int32_t* __restrict__ n_rerank, int R, int Rp2, int top_k, int64_t doc_id_base,
+                       const int32_t* __restrict__ doc_group, int64_t n_groups, int64_t* __restrict__ out_ids,
+                       float* __restrict__ out_scores, int32_t* __restrict__ out_counts) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);
+  uint64_t* gkeys = keys + Rp2;
+  __shared__ unsigned char first[FPB_EX_MAX_TOP_K];  // first[i]: rank position i is its group's best
+  __shared__ int warp_sums[32];
+  __shared__ int s_total;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int n = n_rerank[b];
+  // 1. the canonical order of the re-ranked documents (a document of no valid group is left out)
+  for (int i = tid; i < Rp2; i += 1024) {
+    uint64_t k = 0;
+    if (i < n) {
+      const int32_t d = rerank[int64_t(b) * R + i];
+      if (group_ok(doc_group[d], n_groups)) k = rank_key_f32(exact[int64_t(b) * R + i], uint32_t(d));
+    }
+    keys[i] = k;
+    first[i] = 0;
+  }
+  __syncthreads();
+  block_sort_desc(keys, Rp2);
+  // 2. (group, rank position) keys: sorted descending, a group's entries are adjacent and its best position first
+  for (int i = tid; i < Rp2; i += 1024) {
+    uint64_t g = 0;
+    if (keys[i]) g = (uint64_t(uint32_t(doc_group[rank_key_id(keys[i])])) << 32) | (0xffffffffu - uint32_t(i));
+    gkeys[i] = g;
+  }
+  __syncthreads();
+  block_sort_desc(gkeys, Rp2);
+  for (int j = tid; j < Rp2; j += 1024) {
+    const uint64_t g = gkeys[j];
+    if (g && (j == 0 || (gkeys[j - 1] >> 32) != (g >> 32))) first[0xffffffffu - uint32_t(g)] = 1;
+  }
+  __syncthreads();
+  // 3. ordered compaction of the kept positions: thread t owns positions [t * per, (t + 1) * per)
+  const int per = Rp2 > 1024 ? Rp2 / 1024 : 1;
+  const int i0 = tid * per;
+  int c = 0;
+  for (int u = 0; u < per; ++u) c += (i0 + u < Rp2 && first[i0 + u]) ? 1 : 0;
+  int pos = block_exclusive_scan(c, warp_sums, &s_total);
+  for (int u = 0; u < per; ++u) {
+    const int i = i0 + u;
+    if (i < Rp2 && first[i]) {
+      if (pos < top_k) {
+        out_ids[int64_t(b) * top_k + pos] = doc_id_base + int64_t(rank_key_id(keys[i]));
+        out_scores[int64_t(b) * top_k + pos] = rank_key_f32_value(keys[i]);
+      }
+      ++pos;
+    }
+  }
+  const int cnt = min(top_k, s_total);
+  for (int i = cnt + tid; i < top_k; i += 1024) {
+    out_ids[int64_t(b) * top_k + i] = -1;
+    out_scores[int64_t(b) * top_k + i] = -INFINITY;
+  }
+  if (tid == 0) out_counts[b] = cnt;
+}
+
+// The group maximum of exact search.  Row b of `scores` (stride cols) holds n[b] scores (n == NULL: all cols), entry p
+// scoring local document cand[b * cols + p] (cand == NULL: p).  gkeys [B, n_groups] (zeroed) receives, per (query,
+// group), the largest rank_key_f32(score, document).  A thread reduces GM_PER consecutive entries run by run (one
+// atomic per run of one group), and the warp combines the lanes whose last runs share a group, so one group or long
+// runs of one group cost one atomic per warp and pass.
+constexpr int GM_PER = 8;
+__global__ void __launch_bounds__(256)
+group_max_kernel(const float* __restrict__ scores, const int32_t* __restrict__ cand, const int32_t* __restrict__ n,
+                 int64_t cols, int B, const int32_t* __restrict__ doc_group, int64_t n_groups,
+                 unsigned long long* __restrict__ gkeys) {
+  const int lane = threadIdx.x & 31;
+  const int64_t runs = (cols + GM_PER - 1) / GM_PER, total = int64_t(B) * runs;
+  const int64_t stride = int64_t(gridDim.x) * blockDim.x;  // a multiple of 32: whole warps iterate together
+  for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i - lane < total; i += stride) {
+    int64_t b = 0, p0 = 0, len = 0;
+    if (i < total) {
+      b = i / runs;
+      p0 = (i % runs) * GM_PER;
+      len = n ? n[b] : cols;
+    }
+    uint64_t best = 0;
+    int64_t g_cur = -1;
+#pragma unroll
+    for (int u = 0; u < GM_PER; ++u) {
+      const int64_t p = p0 + u;
+      if (p < len) {
+        const int32_t d = cand ? cand[b * cols + p] : int32_t(p);
+        const int32_t g = doc_group[d];
+        if (group_ok(g, n_groups)) {
+          const uint64_t k = rank_key_f32(scores[b * cols + p], uint32_t(d));
+          if (g != g_cur) {
+            if (best) atomicMax(&gkeys[b * n_groups + g_cur], (unsigned long long)best);
+            g_cur = g;
+            best = k;
+          } else if (k > best) {
+            best = k;
+          }
+        }
+      }
+    }
+    const unsigned long long slot = best ? (unsigned long long)(b * n_groups + g_cur) : ~0ull;
+    const unsigned peers = __match_any_sync(0xffffffffu, slot);
+    const uint32_t hi = __reduce_max_sync(peers, uint32_t(best >> 32));
+    const uint32_t lo = __reduce_max_sync(peers, uint32_t(best >> 32) == hi ? uint32_t(best) : 0u);
+    if (best && lane == __ffs(peers) - 1) atomicMax(&gkeys[slot], (unsigned long long)((uint64_t(hi) << 32) | lo));
+  }
+}
+
+// Digits of the 64-bit key for the radix passes, most significant first (K3b's)
+__constant__ int GS_LO[6] = {53, 42, 32, 21, 10, 0};
+__constant__ int GS_W[6] = {11, 11, 10, 11, 11, 10};
+constexpr int GS_BCAP = 2048;  // capacity of the threshold bucket on the fast path
+
+// One CTA per query: the top_k largest non-empty keys of row b of gkeys [B, n_groups], in descending order, written
+// as K6 writes its ranking.  The keys are distinct (each names its own document), so the top_k are the keys at or
+// above the top_k-th.  The steps are K3b's: linear value buckets over the [min, max] score range, and only the
+// threshold bucket ordered by the whole key; radix passes over the key when that bucket is too large.
+__global__ void __launch_bounds__(1024)
+group_select_kernel(const unsigned long long* __restrict__ gkeys, int64_t n_groups, int top_k, int Rp2,
+                    int64_t doc_id_base, int64_t* __restrict__ out_ids, float* __restrict__ out_scores,
+                    int32_t* __restrict__ out_counts) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);  // [Rp2]
+  __shared__ int hist[SEL_BINS];
+  __shared__ int s_need, s_hd, s_cnt, s_cnt2, s_fast, s_nz;
+  __shared__ uint64_t s_prefix, s_mask;
+  __shared__ uint64_t bkeys[GS_BCAP];
+  __shared__ float s_red[64];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+  const unsigned long long* row = gkeys + int64_t(b) * n_groups;
+  float mn = INFINITY, mx = -INFINITY;
+  int nz = 0;
+  for (int64_t i = tid; i < n_groups; i += 1024) {
+    const uint64_t k = row[i];
+    if (k) {
+      const float v = rank_key_f32_value(k);
+      mn = fminf(mn, v);
+      mx = fmaxf(mx, v);
+      ++nz;
+    }
+  }
+  for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
+  if (tid == 0) {
+    s_cnt = 0;
+    s_cnt2 = 0;
+    s_fast = 0;
+    s_nz = 0;
+  }
+  block_min_max(mn, mx, s_red);
+  if (nz) atomicAdd(&s_nz, nz);
+  __syncthreads();
+  const int64_t n_nz = s_nz;
+  if (n_nz <= top_k) {  // every non-empty group is selected
+    for (int64_t i = tid; i < n_groups; i += 1024) {
+      const uint64_t k = row[i];
+      if (k) keys[atomicAdd(&s_cnt, 1)] = k;
+    }
+    __syncthreads();
+  } else {
+    const float range = mx - mn;
+    const bool usable = range > 0.f && range < 3.0e38f;
+    const float scale = usable ? float(SEL_BINS - 1) / range : 0.f;
+    if (usable) {
+      for (int64_t i = tid; i < n_groups; i += 1024) {
+        const uint64_t k = row[i];
+        if (k) atomicAdd(&hist[value_bucket(rank_key_f32_value(k), mn, scale)], 1);
+      }
+      __syncthreads();
+      int hd, rest;
+      if (tid < 32 && warp_find_bucket(hist, SEL_BINS, top_k, &hd, &rest)) {
+        s_need = rest;
+        s_hd = hd;
+        s_fast = hist[hd] <= GS_BCAP ? 1 : 0;
+      }
+      __syncthreads();
+      if (s_fast) {
+        const int t = s_hd;
+        for (int64_t i = tid; i < n_groups; i += 1024) {
+          const uint64_t k = row[i];
+          if (k) {
+            const int bk = value_bucket(rank_key_f32_value(k), mn, scale);
+            if (bk > t) {
+              keys[atomicAdd(&s_cnt, 1)] = k;  // fewer than top_k of these
+            } else if (bk == t) {
+              bkeys[atomicAdd(&s_cnt2, 1)] = k;  // at most GS_BCAP of these
+            }
+          }
+        }
+        __syncthreads();
+        const int c2 = s_cnt2, need2 = s_need;
+        for (int i = c2 + tid; i < GS_BCAP; i += 1024) bkeys[i] = 0ull;
+        __syncthreads();
+        block_sort_desc(bkeys, GS_BCAP);
+        const int c1 = s_cnt;
+        for (int i = tid; i < need2; i += 1024) keys[c1 + i] = bkeys[i];
+        __syncthreads();
+        if (tid == 0) s_cnt = c1 + need2;  // == top_k
+        __syncthreads();
+      }
+    }
+    if (!s_fast) {  // radix passes over the 64-bit key: the threshold key T, then every key >= T
+      if (tid == 0) {
+        s_need = top_k;
+        s_prefix = 0;
+        s_mask = 0;
+        s_cnt = 0;
+      }
+      for (int pass = 0; pass < 6; ++pass) {
+        const int lo = GS_LO[pass], width = GS_W[pass];
+        const uint64_t dmask = (1ull << width) - 1ull;
+        for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
+        __syncthreads();
+        const uint64_t prefix = s_prefix, mask = s_mask;
+        const int64_t n_up = (n_groups + 1023) / 1024 * 1024;
+        for (int64_t i = tid; i < n_up; i += 1024) {
+          const uint64_t k = i < n_groups ? row[i] : 0ull;
+          const bool in = k != 0 && (k & mask) == prefix;
+          const unsigned act = __ballot_sync(0xffffffffu, in);
+          if (in) {
+            const int bin = int((k >> lo) & dmask);
+            const unsigned peers = __match_any_sync(act, bin);
+            if (lane == __ffs(peers) - 1) atomicAdd(&hist[bin], __popc(peers));
+          }
+        }
+        __syncthreads();
+        int d, rest;
+        if (tid < 32 && warp_find_bucket(hist, 1 << width, s_need, &d, &rest)) {
+          s_need = rest;
+          s_hd = hist[d];
+          s_prefix = prefix | (uint64_t(d) << lo);
+          s_mask = mask | (dmask << lo);
+        }
+        __syncthreads();
+        if (s_hd == s_need) break;  // the whole bucket is selected
+      }
+      const uint64_t T = s_prefix;  // unprocessed low bits are zero
+      for (int64_t i = tid; i < n_groups; i += 1024) {
+        const uint64_t k = row[i];
+        if (k && k >= T) {
+          const int pos = atomicAdd(&s_cnt, 1);
+          if (pos < Rp2) keys[pos] = k;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  const int cnt = min(s_cnt, top_k);
+  for (int i = cnt + tid; i < Rp2; i += 1024) keys[i] = 0ull;
+  __syncthreads();
+  block_sort_desc(keys, Rp2);
+  for (int i = tid; i < top_k; i += 1024) {
+    int64_t id = -1;
+    float sc = -INFINITY;
+    if (i < cnt) {
+      id = doc_id_base + int64_t(rank_key_id(keys[i]));
+      sc = rank_key_f32_value(keys[i]);
+    }
+    out_ids[int64_t(b) * top_k + i] = id;
+    out_scores[int64_t(b) * top_k + i] = sc;
+  }
+  if (tid == 0) out_counts[b] = cnt;
+}
+
+}  // namespace
+
+int launch_rank_grouped(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,
+                        int64_t doc_id_base, const int32_t* doc_group, int64_t n_groups, int64_t* d_out_ids,
+                        float* d_out_scores, int32_t* d_out_counts, cudaStream_t st) {
+  const int Rp2 = fpb_next_pow2(R);
+  const size_t smem = size_t(Rp2) * 16;  // 64 KB at R = 4096: opt in
+  FPB_CUDA_CHECK(cudaFuncSetAttribute(k6_rank_grouped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  k6_rank_grouped_kernel<<<B, 1024, smem, st>>>(scores, ids, n, R, Rp2, top_k, doc_id_base, doc_group, n_groups,
+                                               d_out_ids, d_out_scores, d_out_counts);
+  FPB_LAUNCH_CHECK("k6_rank_grouped");
+  return FPB_OK;
+}
+
+int launch_group_max(const float* scores, const int32_t* cand, const int32_t* n, int64_t cols, int B,
+                     const int32_t* doc_group, int64_t n_groups, uint64_t* gkeys, int sm_count, cudaStream_t st) {
+  FPB_CUDA_CHECK(cudaMemsetAsync(gkeys, 0, size_t(B) * n_groups * 8, st));
+  const int64_t total = int64_t(B) * ((cols + GM_PER - 1) / GM_PER);
+  group_max_kernel<<<fpb_grid_for(total, 256, sm_count), 256, 0, st>>>(
+      scores, cand, n, cols, B, doc_group, n_groups, reinterpret_cast<unsigned long long*>(gkeys));
+  FPB_LAUNCH_CHECK("group_max");
+  return FPB_OK;
+}
+
+int launch_group_select(const uint64_t* gkeys, int64_t n_groups, int B, int top_k, int64_t doc_id_base,
+                        int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t st) {
+  const int Rp2 = fpb_next_pow2(top_k);
+  // dynamic keys[] (32 KB at top_k = 4096) on top of 25 KB of static shared memory: opt in
+  FPB_CUDA_CHECK(cudaFuncSetAttribute(group_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Rp2 * 8));
+  group_select_kernel<<<B, 1024, size_t(Rp2) * 8, st>>>(reinterpret_cast<const unsigned long long*>(gkeys), n_groups,
+                                                       top_k, Rp2, doc_id_base, d_out_ids, d_out_scores,
+                                                       d_out_counts);
+  FPB_LAUNCH_CHECK("group_select");
+  return FPB_OK;
+}
+
+extern "C" int fpb_index_with_groups(fpb_index** out, const fpb_index* ix, const int32_t* d_doc_group,
+                                     int64_t n_groups) {
+  if (!out) {
+    fpb_set_error("fpb_index_with_groups: out is NULL");
+    return FPB_ERR_INVALID;
+  }
+  *out = nullptr;
+  if (!ix || !d_doc_group) {
+    fpb_set_error("fpb_index_with_groups: NULL index or group array");
+    return FPB_ERR_INVALID;
+  }
+  if (n_groups < 1 || n_groups > INT32_MAX) {
+    fpb_set_error("fpb_index_with_groups: n_groups=%lld must be in [1, %d]", (long long)n_groups, INT32_MAX);
+    return FPB_ERR_INVALID;
+  }
+  fpb_index* gx = new fpb_index(*ix);
+  gx->doc_group = d_doc_group;
+  gx->n_groups = n_groups;
+  if (gx->walk) ++gx->walk->refs;
+  *out = gx;
+  return FPB_OK;
+}

@@ -178,13 +178,37 @@ int launch_merge(const fpb_record* d_all_records, int n_shards, int b_stride, in
 int launch_emit_records(const float* exact, const float* approx, const int32_t* ids, const int32_t* n_sel, int B,
                         int R, int64_t doc_id_base, fpb_record* d_records, cudaStream_t st);
 
-// K3b and K6 of the search: select by the candidates' approximate scores, rank by the exact ones
+// ---- Grouped results (groups.cu), on a handle of fpb_index_with_groups ----
+// K6 by group: launch_rank's arguments, then at most one document per group (its best), in the canonical order
+int launch_rank_grouped(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,
+                        int64_t doc_id_base, const int32_t* doc_group, int64_t n_groups, int64_t* d_out_ids,
+                        float* d_out_scores, int32_t* d_out_counts, cudaStream_t st);
+// gkeys [B, n_groups] (cleared here) = per (query, group) the largest rank_key_f32(score, local id) of row b of
+// scores (stride cols), n[b] entries (n NULL: cols), entry p being document cand[b, p] (cand NULL: p)
+int launch_group_max(const float* scores, const int32_t* cand, const int32_t* n, int64_t cols, int B,
+                     const int32_t* doc_group, int64_t n_groups, uint64_t* gkeys, int sm_count, cudaStream_t st);
+// per query the top_k largest non-empty keys of its gkeys row, written as K6 writes its ranking
+int launch_group_select(const uint64_t* gkeys, int64_t n_groups, int B, int top_k, int64_t doc_id_base,
+                        int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t st);
+// The entry points that do not rank for a caller (sharded steps, records, keys) refuse a handle with groups, before
+// any CUDA call
+inline int fpb_refuse_groups(const char* who, const fpb_index* ix) {
+  if (!ix || !ix->doc_group) return FPB_OK;
+  fpb_set_error("%s: an index handle with groups (fpb_index_with_groups) is not supported here", who);
+  return FPB_ERR_UNSUPPORTED;
+}
+
+// K3b and K6 of the search: select by the candidates' approximate scores, rank by the exact ones (by group when the
+// handle carries groups)
 inline int launch_select(const Ws& ws, cudaStream_t st) {
   return launch_select(ws.approx(), ws.cand(), ws.n_cand(), ws.L->cand_cap, ws.L->B, ws.L->R, ws.rerank(),
                        ws.rerank_approx(), ws.n_rerank(), st);
 }
 inline int launch_rank(const fpb_index* ix, const Ws& ws, int top_k, int64_t* d_out_ids, float* d_out_scores,
                        int32_t* d_out_counts, cudaStream_t st) {
+  if (ix->doc_group)
+    return launch_rank_grouped(ws.exact(), ws.rerank(), ws.n_rerank(), ws.L->R, ws.L->B, top_k, ix->doc_id_base,
+                               ix->doc_group, ix->n_groups, d_out_ids, d_out_scores, d_out_counts, st);
   return launch_rank(ws.exact(), ws.rerank(), ws.n_rerank(), ws.L->R, ws.L->B, top_k, ix->doc_id_base, d_out_ids,
                      d_out_scores, d_out_counts, st);
 }
@@ -242,6 +266,9 @@ struct ExLayout {
   int64_t off_table;        // i32 ExListTable, built on the host
   int64_t off_cand;         // i32 [B, cap] query b's candidates (its list's ids)
   int64_t off_n_cand;       // i32 [B] their numbers
+  // a handle with groups (top_k > 0): u64 [B, n_groups] group keys, in the accumulator region (free once K7 is
+  // finalized) when they fit there, after everything else otherwise
+  int64_t off_gkeys;
   int64_t total_bytes;
 };
 

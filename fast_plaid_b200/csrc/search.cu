@@ -109,6 +109,7 @@ extern "C" int fpb_search_batch_host(const fpb_index* ix, const void* h_queries,
 extern "C" int fpb_search_shard(const fpb_index* ix, const void* d_queries, int B, int Q,
                                 const fpb_params* p, void* d_ws, size_t ws_bytes, fpb_record* d_records,
                                 void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_search_shard", ix));
   if (!d_queries || !d_records) {
     fpb_set_error("fpb_search_shard: NULL query or record pointer");
     return FPB_ERR_INVALID;
@@ -122,6 +123,7 @@ extern "C" int fpb_search_shard(const fpb_index* ix, const void* d_queries, int 
 extern "C" int fpb_shard_approx_keys(const fpb_index* ix, const void* d_queries, int B, int Q,
                                      const fpb_params* p, void* d_ws, size_t ws_bytes, uint64_t* d_keys,
                                      void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_shard_approx_keys", ix));
   if (!d_queries || !d_keys) {
     fpb_set_error("fpb_shard_approx_keys: NULL query or key pointer");
     return FPB_ERR_INVALID;
@@ -137,6 +139,7 @@ extern "C" int fpb_shard_subset_begin(const fpb_index* ix, const void* d_queries
                                       const int32_t* d_subset_ids, const int64_t* d_subset_offsets,
                                       int64_t max_subset_len, void* d_ws, size_t ws_bytes,
                                       uint32_t* d_cbitmap_out, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_shard_subset_begin", ix));
   if (!d_queries || !d_subset_offsets || !d_cbitmap_out || (p && !(p->flags & FPB_FLAG_SUBSET))) {
     fpb_set_error("fpb_shard_subset_begin: NULL pointer or FPB_FLAG_SUBSET not set");
     return FPB_ERR_INVALID;
@@ -154,6 +157,7 @@ extern "C" int fpb_shard_filter_begin(const fpb_index* ix, const void* d_queries
                                       const uint32_t* d_filters, int n_filters, int64_t n_bits,
                                       const int32_t* h_query_filter, void* d_ws, size_t ws_bytes,
                                       uint32_t* d_cbitmap_out, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_shard_filter_begin", ix));
   if (!d_queries || !d_cbitmap_out) {
     fpb_set_error("fpb_shard_filter_begin: NULL query or centroid-bitmap pointer");
     return FPB_ERR_INVALID;
@@ -171,6 +175,7 @@ extern "C" int fpb_shard_filter_begin(const fpb_index* ix, const void* d_queries
 extern "C" int fpb_shard_subset_keys(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws,
                                      size_t ws_bytes, const uint32_t* d_all_cbitmaps, int n_shards,
                                      uint64_t* d_keys, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_shard_subset_keys", ix));
   if (!d_all_cbitmaps || !d_keys || n_shards < 1 || (p && !(p->flags & FPB_FLAG_SUBSET))) {
     fpb_set_error("fpb_shard_subset_keys: bad arguments or FPB_FLAG_SUBSET not set");
     return FPB_ERR_INVALID;
@@ -185,6 +190,7 @@ extern "C" int fpb_shard_subset_keys(const fpb_index* ix, int B, int Q, const fp
 extern "C" int fpb_shard_apply_threshold(const fpb_index* ix, const uint64_t* d_all_keys, int n_shards,
                                          int shard_rank, int B, int Q, const fpb_params* p, void* d_ws,
                                          size_t ws_bytes, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_shard_apply_threshold", ix));
   if (!d_all_keys || n_shards < 1 || shard_rank < 0 || shard_rank >= n_shards) {
     fpb_set_error("fpb_shard_apply_threshold: bad arguments");
     return FPB_ERR_INVALID;
@@ -196,6 +202,7 @@ extern "C" int fpb_shard_apply_threshold(const fpb_index* ix, const uint64_t* d_
 
 extern "C" int fpb_shard_exact_records(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws,
                                        size_t ws_bytes, fpb_record* d_records, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_shard_exact_records", ix));
   if (!d_records) {
     fpb_set_error("fpb_shard_exact_records: NULL record pointer");
     return FPB_ERR_INVALID;
@@ -280,6 +287,7 @@ extern "C" int fpb_stage_rank(const fpb_index* ix, int B, int Q, const fpb_param
 }
 extern "C" int fpb_stage_records(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws,
                                  size_t ws_bytes, fpb_record* d_records, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_stage_records", ix));
   if (!d_records) {
     fpb_set_error("fpb_stage_records: NULL record pointer");
     return FPB_ERR_INVALID;
@@ -290,6 +298,7 @@ extern "C" int fpb_stage_records(const fpb_index* ix, int B, int Q, const fpb_pa
 }
 extern "C" int fpb_stage_keys(const fpb_index* ix, int B, int Q, const fpb_params* p, void* d_ws, size_t ws_bytes,
                               uint64_t* d_keys, void* stream) {
+  FPB_TRY(fpb_refuse_groups("fpb_stage_keys", ix));
   if (!d_keys) {
     fpb_set_error("fpb_stage_keys: NULL key pointer");
     return FPB_ERR_INVALID;

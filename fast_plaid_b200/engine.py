@@ -103,6 +103,7 @@ EXPORTED_SYMBOLS = [
     "fpb_index_walk_layout",
     "fpb_index_walk_group",
     "fpb_index_append",
+    "fpb_index_with_groups",
     "fpb_ivf_append",
     "fpb_docs_compact",
     "fpb_ivf_delete",
@@ -195,6 +196,8 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_index_walk_group.argtypes = [vp]
         lib.fpb_index_append.restype = i32
         lib.fpb_index_append.argtypes = [ctypes.POINTER(vp), vp, i64, i64, vp, vp, vp, vp, vp, vp, i64, i64]
+        lib.fpb_index_with_groups.restype = i32
+        lib.fpb_index_with_groups.argtypes = [ctypes.POINTER(vp), vp, vp, i64]
         lib.fpb_ivf_append.restype = i32
         lib.fpb_ivf_append.argtypes = [i32, i64, vp, vp, i64, i64, vp, vp, vp, vp, i64, ctypes.POINTER(i64), vp]
         lib.fpb_docs_compact.restype = i32
@@ -406,6 +409,36 @@ class Filter:
                 _check(load_library().fpb_filter_from_mask(device.index or 0, m.data_ptr(), F, n, bitmap.data_ptr(),
                                                            torch.cuda.current_stream(device).cuda_stream))
         return Filter(bitmap, [0] * num_queries if mask.dim() == 1 else list(range(F)), n)
+
+
+@dataclasses.dataclass
+class Groups:
+    """Grouped results in their device form: `ids` int32 [num_documents] on the index's device, the group of every
+    document renumbered densely to 0 .. n_groups - 1 (fpb_index_with_groups).  Each query then gets at most one
+    document per group, the group's best."""
+    ids: torch.Tensor
+    n_groups: int
+
+    @staticmethod
+    def check(group_by, num_documents: int) -> None:
+        """Refuses a group map that is not a 1-D integer tensor of `num_documents` non-negative values."""
+        if not isinstance(group_by, torch.Tensor):
+            raise ValueError(f"group_by must be a 1-D integer tensor, got {type(group_by).__name__}")
+        if group_by.dtype.is_floating_point or group_by.dtype.is_complex or group_by.dtype == torch.bool:
+            raise ValueError(f"group_by must hold integer group ids, got {group_by.dtype}")
+        if group_by.dim() != 1:
+            raise ValueError(f"group_by must be 1-D (one group per document), got shape {list(group_by.shape)}")
+        if group_by.shape[0] != num_documents:
+            raise ValueError(f"group_by has {group_by.shape[0]} entries, the index has {num_documents} documents")
+        if group_by.numel() and bool((group_by < 0).any()):
+            raise ValueError("group_by values must be non-negative")
+
+    @staticmethod
+    def from_tensor(group_by: torch.Tensor, num_documents: int, device: torch.device | str) -> "Groups":
+        """The device form of a user's group map: any non-negative integers, not necessarily dense or sorted."""
+        Groups.check(group_by, num_documents)
+        uniq, inverse = torch.unique(group_by.to(device), return_inverse=True)
+        return Groups(inverse.to(torch.int32).contiguous(), max(int(uniq.numel()), 1))
 
 
 def _popcount(x: torch.Tensor) -> torch.Tensor:
@@ -877,6 +910,28 @@ class DeviceIndex:
             self._last_stream = st
             yield
 
+    @contextlib.contextmanager
+    def _grouped(self, groups: Groups):
+        """Within the block every search of this index ranks by `groups`: the index's handle is swapped for one that
+        carries them (fpb_index_with_groups), under the search lock, and swapped back after."""
+        if (groups.ids.device != self.device or groups.ids.dtype != torch.int32 or groups.ids.dim() != 1
+                or groups.ids.shape[0] != self.num_documents or not groups.ids.is_contiguous()):
+            raise ValueError(f"expected contiguous group ids int32 [{self.num_documents}] on {self.device}, got "
+                             f"{groups.ids.dtype} {list(groups.ids.shape)} on {groups.ids.device}")
+        with self._search_lock:
+            if getattr(self, "_handle", None) is None or not self._handle.value:
+                raise RuntimeError("this DeviceIndex has been closed")
+            handle = ctypes.c_void_p()
+            _check(self._lib.fpb_index_with_groups(ctypes.byref(handle), self._handle, groups.ids.data_ptr(),
+                                                   groups.n_groups))
+            own, self._handle = self._handle, handle
+            try:
+                yield
+            finally:
+                self._handle = own
+                self._lib.fpb_index_destroy(handle)
+                self._groups_keepalive = groups.ids  # until the stream has consumed them
+
     # -- lifetime ------------------------------------------------------------------------
     def close(self) -> None:
         lock = getattr(self, "_search_lock", None)
@@ -1156,13 +1211,17 @@ class DeviceIndex:
 
     def search(
         self, queries: torch.Tensor, params: FpbParams, subset: list[list[int]] | None = None,
-        filter: Filter | None = None,
+        filter: Filter | None = None, groups: Groups | None = None,
     ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries: fp16 [B, Q, D] on this device.  Returns device tensors
         (ids int64 [B, top_k], scores f32 [B, top_k], counts int32 [B]).  Asynchronous.
         `subset`: per query a list of GLOBAL doc ids to restrict the search to
         (search.rs:494-517, :544-547).  `filter`: the same restriction in device form (fpb_search_batch_filter);
-        for the same documents the result is the same bytes."""
+        for the same documents the result is the same bytes.  `groups`: at most one document per group among the
+        n_full_scores / 4 re-ranked ones, each group's best (fpb_index_with_groups)."""
+        if groups is not None:
+            with self._grouped(groups):
+                return self.search(queries, params, subset, filter)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k = params.top_k
@@ -1294,8 +1353,8 @@ class DeviceIndex:
         return int(out.value)
 
     def search_exhaustive(self, queries: torch.Tensor, top_k: int, budget_bytes: int = 6 << 30,
-                          subset: list[list[int]] | torch.Tensor | None = None,
-                          filter: Filter | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                          subset: list[list[int]] | torch.Tensor | None = None, filter: Filter | None = None,
+                          groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Exact top_k over every document: (ids int64 [B, top_k] global, scores f32 [B, top_k], counts int32 [B]),
         the result contract of `search`.  The batch is split into calls whose workspace fits `budget_bytes`;
         the result does not depend on the split.  Asynchronous.
@@ -1305,7 +1364,13 @@ class DeviceIndex:
         every score is the one `exhaustive_scores` gives the same document.  `subset` may also be an integer tensor
         [B, L] on this device, a row of ids per query (padded with any id outside the index, such as -1): each row is
         then a list of its own, with no host list made.  `filter`: the restriction in device form
-        (fpb_search_exhaustive_filter); for the same documents the result is the same bytes."""
+        (fpb_search_exhaustive_filter); for the same documents the result is the same bytes.
+
+        `groups`: at most one document per group, the group's best, and top_k counts groups: the exhaustive ranking
+        (restricted to the subset or filter) with each group's first document kept."""
+        if groups is not None:
+            with self._grouped(groups):
+                return self.search_exhaustive(queries, top_k, budget_bytes, subset, filter)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k = int(top_k)
@@ -1526,11 +1591,14 @@ class DeviceIndex:
         return io["d_q"]
 
     def search_host(
-        self, queries_host: torch.Tensor, params: FpbParams
+        self, queries_host: torch.Tensor, params: FpbParams, groups: Groups | None = None,
     ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries_host: float [B, Q, D] in HOST memory.  The H2D copy, the search and the D2H copies of the
         results all happen inside the C-ABI call, which synchronises the stream.  Returns HOST tensors
-        (ids, scores, counts)."""
+        (ids, scores, counts).  `groups`: as in `search`."""
+        if groups is not None:
+            with self._grouped(groups):
+                return self.search_host(queries_host, params)
         B, Q, _ = self._check_queries(queries_host, host=True).shape
         if B == 0:
             k = params.top_k

@@ -575,6 +575,12 @@ class FastPlaid:
             return _SubsetTensor(torch.tensor(subset, dtype=torch.int64))
         return None
 
+    def _check_group_by(self, group_by) -> None:
+        """`group_by` on a document-sharded index is refused before any communicator or collective exists."""
+        if group_by is not None and self.shard is not None:
+            raise NotImplementedError("group_by= on a document-sharded index is not implemented: each group's best "
+                                      "document would have to be chosen across the ranks")
+
     def _num_documents(self, idx: DeviceIndex) -> int:
         """Documents of the whole index, the length of a mask.  On a document-sharded index of several ranks it is
         the largest end of the ranks' ranges (one all-reduce: every rank passes the same `subset=`, so every rank
@@ -608,27 +614,30 @@ class FastPlaid:
         return search_indices, queries_embeddings, subset
 
     def _search_device(self, idx: DeviceIndex, queries: torch.Tensor, params,
-                       subset: list[list[int]] | None = None) -> list[list[tuple[int, float]]]:
+                       subset: list[list[int]] | None = None, group_by: torch.Tensor | None = None,
+                       ) -> list[list[tuple[int, float]]]:
         """search_on_device (fast_plaid.py:188-253) for the whole batch."""
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         if self.shard is not None:
             return self._search_sharded(idx, queries, params, subset)
+        # the group map is remapped on every device that searches
+        groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device)
         if isinstance(subset, _SubsetTensor):
             q16 = queries.to(torch.float16).to(idx.device)
             filt = subset.to_filter(idx, q16.shape[0])
-            ids, scores, counts = idx.search(q16, params, filter=filt)
+            ids, scores, counts = idx.search(q16, params, filter=filt, groups=groups)
             return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         if subset is not None:
             q16 = queries.to(torch.float16).to(idx.device)
-            ids, scores, counts = idx.search(q16, params, subset=subset)
+            ids, scores, counts = idx.search(q16, params, subset=subset, groups=groups)
             return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         if queries.device.type == "cuda":
             q16 = queries.to(device=idx.device, dtype=torch.float16)  # fast_plaid.py:241
-            ids, scores, counts = idx.search(q16, params)
+            ids, scores, counts = idx.search(q16, params, groups=groups)
             return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         # fp16 cast on the host like the reference (fast_plaid.py:241), straight into pinned staging
-        ids, scores, counts = idx.search_host(queries, params)
+        ids, scores, counts = idx.search_host(queries, params, groups=groups)
         return _results_to_lists(ids, scores, counts)
 
     def _shard_comm(self, idx: DeviceIndex):
@@ -698,6 +707,7 @@ class FastPlaid:
         show_progress: bool = True,  # noqa: ARG002  (one launch sequence per batch: nothing to show)
         subset: list[list[int]] | list[int] | None = None,
         n_processes: int | None = None,  # noqa: ARG002  (CPU-only knob in the reference)
+        group_by: torch.Tensor | None = None,
     ) -> list[list[tuple[int, float]]]:
         """Search the index (fast_plaid.py:930-983).  Returns, per query, up to ``top_k``
         ``(doc_id, score)`` pairs in rank order.
@@ -708,11 +718,22 @@ class FastPlaid:
         as -1), or a bool mask ``[num_documents]`` (every query) or ``[B, num_documents]`` (one per query).  Order
         and duplicates do not matter and unknown ids are ignored.  Everything but a list of lists becomes a bitmap
         on the GPU, and queries that share one share its expansion; the result is the one the same sets give as
-        lists of lists."""
+        lists of lists.
+
+        ``group_by`` (a 1-D integer tensor of ``num_documents`` non-negative group ids, on any device, e.g. the page's
+        PDF or the passage's document) returns at most one document per group: the group's best, ranked as usual.
+        Grouping applies to the ``n_full_scores / 4`` documents the search re-ranks, so the result is the ungrouped
+        search with ``top_k = n_full_scores // 4`` collapsed to each group's first document and cut to ``top_k``:
+        fewer than ``top_k`` documents come back when those re-ranked documents hold fewer groups.  Raise
+        ``n_full_scores`` for more, or use ``search_exhaustive``, whose grouping is exact.  Not supported with
+        ``shard=``."""
+        self._check_group_by(group_by)
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
         params = DeviceIndex.make_params(top_k, n_full_scores, n_ivf_probe, batch_size)
+        if group_by is not None:
+            _engine.Groups.check(group_by, search_indices[self.devices[0]].num_documents)
         if len(self.devices) == 1:
-            return self._search_device(search_indices[self.devices[0]], queries, params, subset)
+            return self._search_device(search_indices[self.devices[0]], queries, params, subset, group_by)
         # several devices in ONE process: replicated index, query list split across devices
         # (the reference's multi-GPU mode, fast_plaid.py:893-928)
         n = len(self.devices)
@@ -721,7 +742,7 @@ class FastPlaid:
         sub_chunks = _split_subset(subset, chunk, len(chunks))
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
-                ex.submit(self._search_device, search_indices[d], chunks[i], params, sub_chunks[i])
+                ex.submit(self._search_device, search_indices[d], chunks[i], params, sub_chunks[i], group_by)
                 for i, d in enumerate(self.devices)
                 if i < len(chunks)
             ]
@@ -731,18 +752,20 @@ class FastPlaid:
         return out
 
     def _search_exhaustive_device(self, idx: DeviceIndex, queries: torch.Tensor, top_k: int,
-                                  subset: list[list[int]] | None = None) -> list[list[tuple[int, float]]]:
+                                  subset: list[list[int]] | None = None, group_by: torch.Tensor | None = None,
+                                  ) -> list[list[tuple[int, float]]]:
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
+        groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device)
         q16 = queries.to(device=idx.device, dtype=torch.float16)  # the fp16 cast of `search` (fast_plaid.py:241)
         if isinstance(subset, _SubsetTensor) and subset.per_query and subset.data.dtype != torch.bool:
             # candidate rows to re-rank: each row is a list of the list walk as it stands
-            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset.data.to(idx.device))
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset.data.to(idx.device), groups=groups)
         elif isinstance(subset, _SubsetTensor):
             filt = subset.to_filter(idx, q16.shape[0])
-            ids, scores, counts = idx.search_exhaustive(q16, top_k, filter=filt)
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, filter=filt, groups=groups)
         else:
-            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset)
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset, groups=groups)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
     def _exhaustive_sharded_step(self, idx: DeviceIndex, B: int, Q: int, top_k: int, budget_bytes: int) -> int:
@@ -785,6 +808,7 @@ class FastPlaid:
         queries_embeddings: torch.Tensor | list[torch.Tensor],
         top_k: int = 10,
         subset: list[list[int]] | list[int] | None = None,
+        group_by: torch.Tensor | None = None,
     ) -> list[list[tuple[int, float]]]:
         """Exact search: score EVERY document with the exact MaxSim formula of the re-rank stage and return,
         per query, the ``top_k`` best ``(doc_id, score)`` pairs in rank order (score desc, then id asc).
@@ -810,7 +834,12 @@ class FastPlaid:
         A score sums the per-query-token fp16 maxima exactly and rounds once to fp32; ``search`` keeps an fp32
         running sum.  The two agree whenever that running sum is exact (the usual case); otherwise the same
         document's score can differ in the last bit between ``search`` and ``search_exhaustive``.  In exchange the
-        result is the same bytes however the work is ordered or the batch is split."""
+        result is the same bytes however the work is ordered or the batch is split.
+
+        ``group_by`` (as in ``search``) returns at most one document per group, exactly: the full ranking of the
+        query (restricted to ``subset``) with each group's first document kept, ``top_k`` <= 4096 groups.  Not
+        supported with ``shard=``."""
+        self._check_group_by(group_by)
         if self.shard is not None and not (subset is None or (isinstance(subset, list) and not subset)):
             raise NotImplementedError(
                 "search_exhaustive with subset= on a document-sharded index is not implemented: each rank would "
@@ -827,10 +856,12 @@ class FastPlaid:
                     "torch.distributed process group: FastPlaid exchanges the shards' results over no other channel"
                 )
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
+        if group_by is not None:
+            _engine.Groups.check(group_by, search_indices[self.devices[0]].num_documents)
         if self.shard is not None:
             return self._search_exhaustive_sharded(search_indices[self.devices[0]], queries, top_k)
         if len(self.devices) == 1:
-            return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k, subset)
+            return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k, subset, group_by)
         # several devices in ONE process hold replicas: the query list is split across them, like `search`
         n = len(self.devices)
         chunk = math.ceil(queries.shape[0] / n)
@@ -838,7 +869,8 @@ class FastPlaid:
         sub_chunks = _split_subset(subset, chunk, len(chunks))
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
-                ex.submit(self._search_exhaustive_device, search_indices[d], chunks[i], top_k, sub_chunks[i])
+                ex.submit(self._search_exhaustive_device, search_indices[d], chunks[i], top_k, sub_chunks[i],
+                          group_by)
                 for i, d in enumerate(self.devices)
                 if i < len(chunks)
             ]
@@ -858,11 +890,12 @@ class FastPlaid:
         show_progress: bool = True,
         subset: list[list[int]] | list[int] | None = None,
         n_processes: int | None = None,
+        group_by: torch.Tensor | None = None,
     ) -> list[list[tuple[int, float, torch.Tensor]]]:
         """``search`` plus, per result, the ``[query_tokens, doc_tokens]`` fp16 similarity
-        matrix (fast_plaid.py:985-1043, search.rs:668-686)."""
+        matrix (fast_plaid.py:985-1043, search.rs:668-686).  ``group_by``: as in ``search``."""
         base = self.search(queries_embeddings, top_k, batch_size, n_full_scores, n_ivf_probe, show_progress,
-                           subset, n_processes)
+                           subset, n_processes, group_by)
         search_indices, queries, _ = self._prepare_search(queries_embeddings, None)
         # several devices in one process hold replicas: any of them can produce every matrix
         idx = search_indices[self.devices[0]]

@@ -123,6 +123,25 @@ int fpb_index_append(fpb_index** out, const fpb_index* index, int64_t n_docs, in
                      int64_t max_doc_len);
 
 /*
+ * fpb_index_with_groups -- grouped results: a new handle over every array of `index` (shared, like
+ * fpb_index_append's handles share the walk layout) that also carries d_doc_group (i32 [n_docs], borrowed: the caller
+ * keeps it alive until the handle's last search has run), the group of every local document, dense in [0, n_groups).
+ * Each query then gets at most one document per group: the group's best under the canonical order (score desc, then
+ * id asc), these ranked in that order, d_out_counts[b] = min(top_k, groups present), tails id -1 / score -inf, and
+ * every score the ungrouped search's, bit for bit.  A document whose group is outside [0, n_groups) is skipped.
+ *   - fpb_search_batch, _subset, _filter, _host and fpb_stage_rank group the re-ranked list (the n_full_scores / 4
+ *     documents of the approximate stage): the ungrouped search with top_k = n_full_scores / 4, each group's first
+ *     document kept, cut to top_k.  So fewer than top_k documents can come back; a larger n_full_scores gives more.
+ *   - fpb_search_exhaustive, _subset and _filter are exact: the exhaustive ranking (of the query's list) with each
+ *     group's first document kept.  top_k <= 4096 counts groups.  Their *_workspace_bytes include the group keys'
+ *     scratch, [B, n_groups] u64 beyond what the accumulator region holds.
+ *   - The sharded entry points and those that emit records or keys return FPB_ERR_UNSUPPORTED.
+ * NULL pointers and n_groups outside [1, INT32_MAX] are refused before any CUDA call.  Destroy the handle with
+ * fpb_index_destroy; `index` stays valid.  fpb_index_append on it returns a handle without groups.
+ */
+int fpb_index_with_groups(fpb_index** out, const fpb_index* index, const int32_t* d_doc_group, int64_t n_groups);
+
+/*
  * fpb_ivf_append -- the inverted file of an index of n_old_docs documents grown by n_new_docs documents (ids
  * n_old_docs ..): for every one of the n_cells cells, its old list (d_ivf_offsets i64 [n_cells + 1] into d_ivf_pids)
  * followed by the ascending ids of the new documents with a token in that cell.  The new documents' codes are
