@@ -218,6 +218,7 @@ extern "C" int fpb_index_append(fpb_index** out, const fpb_index* ix, int64_t n_
   nx->ivf_pids = d_ivf_pids;
   nx->doc_group = nullptr;  // a group map covers the old documents only
   nx->n_groups = 0;
+  nx->max_per_group = 0;
   int rc = launch_token_norms(nx, static_cast<__half*>(d_token_norms), ix->E, nullptr);
   if (rc == FPB_OK) rc = fpb_extend_walk_layout(nx, ix->N);  // synchronises the device
   if (rc != FPB_OK) {

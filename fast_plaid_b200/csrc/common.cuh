@@ -77,6 +77,8 @@ struct fpb_index {
   // borrowed like the other arrays; NULL / 0 on a handle without groups
   const int32_t* doc_group;
   int64_t n_groups;
+  // documents kept per group (fpb_index_with_groups_max), in [1, FPB_MAX_PER_GROUP] on a handle with groups
+  int max_per_group;
 };
 
 void fpb_set_error(const char* fmt, ...);

@@ -77,7 +77,8 @@ int exhaustive_layout(const fpb_index* ix, int B, int Q, int top_k, ExLayout* X,
   }
   if (sel && ix->doc_group) {
     const int64_t cols = lists ? cap : N;  // accumulator entries per query
-    X->off_gkeys = ix->n_groups <= cols ? X->off_acc : take(int64_t(B) * ix->n_groups * 8);
+    const int64_t keys = int64_t(ix->max_per_group) * ix->n_groups;  // m rounds of n_groups keys per query
+    X->off_gkeys = keys <= cols ? X->off_acc : take(int64_t(B) * keys * 8);
   }
   X->total_bytes = off;
   return FPB_OK;
@@ -157,13 +158,15 @@ struct ExSelected {
   uint64_t* gkeys;
 };
 
-// The grouped ranking of exact search: the group maximum over the [B, cols] scores, then the top_k groups
+// The grouped ranking of exact search: m rounds of the group maximum over the [B, cols] scores (the m best keys of
+// every group), then the top_k largest of these m * n_groups keys
 int rank_groups(const fpb_index* ix, const float* scores, const int32_t* cand, const int32_t* n, int64_t cols, int B,
                 int top_k, uint64_t* gkeys, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
                 cudaStream_t st) {
-  FPB_TRY(launch_group_max(scores, cand, n, cols, B, ix->doc_group, ix->n_groups, gkeys, ix->sm_count, st));
-  return launch_group_select(gkeys, ix->n_groups, B, top_k, ix->doc_id_base, d_out_ids, d_out_scores, d_out_counts,
-                             st);
+  FPB_TRY(launch_group_max(scores, cand, n, cols, B, ix->doc_group, ix->n_groups, ix->max_per_group, gkeys,
+                           ix->sm_count, st));
+  return launch_group_select(gkeys, int64_t(ix->max_per_group) * ix->n_groups, B, top_k, ix->doc_id_base, d_out_ids,
+                             d_out_scores, d_out_counts, st);
 }
 
 // The checks and the whole computation of a full-scan search up to its selected lists: K7 scores every document,

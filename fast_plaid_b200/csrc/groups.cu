@@ -1,11 +1,13 @@
-// Grouped results (DESIGN §7): each query returns at most one document per group, the group's best under the
-// canonical order (score desc, then id asc), and these representatives in the canonical order.  A handle made by
-// fpb_index_with_groups carries the group of every local document, dense ids in [0, n_groups).
-//   - The re-ranked list of a search (<= 4096 documents per query): K6's canonical sort, then the first entry of
+// Grouped results (DESIGN §7): each query returns at most m documents per group, the group's m best under the
+// canonical order (score desc, then id asc), and these in the canonical order.  A handle made by
+// fpb_index_with_groups(_max) carries the group of every local document, dense ids in [0, n_groups), and m.
+//   - The re-ranked list of a search (<= 4096 documents per query): K6's canonical sort, then the first m entries of
 //     each group, kept in rank order (k6_rank_grouped_kernel).
 //   - Exact search: the maximum canonical key of every (query, group) pair over the exact scores (group_max_kernel),
 //     then the top_k largest of those keys per query (group_select_kernel).  The maximum key is the group's
-//     canonical best document, and a maximum does not depend on the order of the atomics.
+//     canonical best document, and a maximum does not depend on the order of the atomics.  At m > 1, m rounds of
+//     the maximum (group_round_max_kernel), round r bounded by round r - 1's key, give the m best keys of every
+//     group, and the selection runs over all m * n_groups of them.
 // A group id outside [0, n_groups) is skipped: the host remap never makes one, but the C ABI is public.
 #include "kernels.h"
 #include "select.cuh"
@@ -42,16 +44,18 @@ __device__ __forceinline__ int block_exclusive_scan(int c, int* warp_sums, int* 
 __device__ __forceinline__ bool group_ok(int32_t g, int64_t n_groups) { return g >= 0 && int64_t(g) < n_groups; }
 
 // Grouped K6, one CTA per query: row b of exact / rerank (stride R) holds the scores and local ids of n_rerank[b]
-// documents.  Shared memory: the canonical keys [Rp2], then (group, rank position) keys [Rp2].
+// documents, of which the first m of each group in the canonical order are kept (ONE: the instance for m = 1, which
+// ignores m).  Shared memory: the canonical keys [Rp2], then (group, rank position) keys [Rp2].
+template <bool ONE>
 __global__ void __launch_bounds__(1024)
 k6_rank_grouped_kernel(const float* __restrict__ exact, const int32_t* __restrict__ rerank,
                        const int32_t* __restrict__ n_rerank, int R, int Rp2, int top_k, int64_t doc_id_base,
                        const int32_t* __restrict__ doc_group, int64_t n_groups, int64_t* __restrict__ out_ids,
-                       float* __restrict__ out_scores, int32_t* __restrict__ out_counts) {
+                       float* __restrict__ out_scores, int32_t* __restrict__ out_counts, int m) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);
   uint64_t* gkeys = keys + Rp2;
-  __shared__ unsigned char first[FPB_EX_MAX_TOP_K];  // first[i]: rank position i is its group's best
+  __shared__ unsigned char first[FPB_EX_MAX_TOP_K];  // first[i]: rank position i is among its group's m best
   __shared__ int warp_sums[32];
   __shared__ int s_total;
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -68,7 +72,8 @@ k6_rank_grouped_kernel(const float* __restrict__ exact, const int32_t* __restric
   }
   __syncthreads();
   block_sort_desc(keys, Rp2);
-  // 2. (group, rank position) keys: sorted descending, a group's entries are adjacent and its best position first
+  // 2. (group, rank position) keys: sorted descending, a group's entries are adjacent and its best position first,
+  // so entry j is among its group's m best when the entry m places before it belongs to another group
   for (int i = tid; i < Rp2; i += 1024) {
     uint64_t g = 0;
     if (keys[i]) g = (uint64_t(uint32_t(doc_group[rank_key_id(keys[i])])) << 32) | (0xffffffffu - uint32_t(i));
@@ -78,7 +83,8 @@ k6_rank_grouped_kernel(const float* __restrict__ exact, const int32_t* __restric
   block_sort_desc(gkeys, Rp2);
   for (int j = tid; j < Rp2; j += 1024) {
     const uint64_t g = gkeys[j];
-    if (g && (j == 0 || (gkeys[j - 1] >> 32) != (g >> 32))) first[0xffffffffu - uint32_t(g)] = 1;
+    if (g && (ONE ? j == 0 || (gkeys[j - 1] >> 32) != (g >> 32) : j < m || (gkeys[j - m] >> 32) != (g >> 32)))
+      first[0xffffffffu - uint32_t(g)] = 1;
   }
   __syncthreads();
   // 3. ordered compaction of the kept positions: thread t owns positions [t * per, (t + 1) * per)
@@ -106,15 +112,17 @@ k6_rank_grouped_kernel(const float* __restrict__ exact, const int32_t* __restric
 }
 
 // The group maximum of exact search.  Row b of `scores` (stride cols) holds n[b] scores (n == NULL: all cols), entry p
-// scoring local document cand[b * cols + p] (cand == NULL: p).  gkeys [B, n_groups] (zeroed) receives, per (query,
-// group), the largest rank_key_f32(score, document).  A thread reduces GM_PER consecutive entries run by run (one
-// atomic per run of one group), and the warp combines the lanes whose last runs share a group, so one group or long
-// runs of one group cost one atomic per warp and pass.
+// scoring local document cand[b * cols + p] (cand == NULL: p).  gkeys (rows of stride row_stride, zeroed) receives
+// at b * row_stride + g, per (query, group), the largest rank_key_f32(score, document); with a `bound` (same layout),
+// the largest below bound[b * row_stride + g], so a group whose bound is 0 is skipped.  A thread reduces GM_PER
+// consecutive entries run by run (one atomic per run of one group), and the warp combines the lanes whose last runs
+// share a group, so one group or long runs of one group cost one atomic per warp and pass.
 constexpr int GM_PER = 8;
-__global__ void __launch_bounds__(256)
-group_max_kernel(const float* __restrict__ scores, const int32_t* __restrict__ cand, const int32_t* __restrict__ n,
-                 int64_t cols, int B, const int32_t* __restrict__ doc_group, int64_t n_groups,
-                 unsigned long long* __restrict__ gkeys) {
+__device__ __forceinline__ void group_max(const float* __restrict__ scores, const int32_t* __restrict__ cand,
+                                          const int32_t* __restrict__ n, int64_t cols, int B,
+                                          const int32_t* __restrict__ doc_group, int64_t n_groups, int64_t row_stride,
+                                          const unsigned long long* __restrict__ bound,
+                                          unsigned long long* __restrict__ gkeys) {
   const int lane = threadIdx.x & 31;
   const int64_t runs = (cols + GM_PER - 1) / GM_PER, total = int64_t(B) * runs;
   const int64_t stride = int64_t(gridDim.x) * blockDim.x;  // a multiple of 32: whole warps iterate together
@@ -125,8 +133,8 @@ group_max_kernel(const float* __restrict__ scores, const int32_t* __restrict__ c
       p0 = (i % runs) * GM_PER;
       len = n ? n[b] : cols;
     }
-    uint64_t best = 0;
-    int64_t g_cur = -1;
+    uint64_t best = 0, lim = 0;
+    int64_t g_cur = -1, g_lim = -1;
 #pragma unroll
     for (int u = 0; u < GM_PER; ++u) {
       const int64_t p = p0 + u;
@@ -135,8 +143,15 @@ group_max_kernel(const float* __restrict__ scores, const int32_t* __restrict__ c
         const int32_t g = doc_group[d];
         if (group_ok(g, n_groups)) {
           const uint64_t k = rank_key_f32(scores[b * cols + p], uint32_t(d));
+          if (bound) {  // one load per run: the bound is the (query, group)'s
+            if (g != g_lim) {
+              g_lim = g;
+              lim = bound[b * row_stride + g];
+            }
+            if (k >= lim) continue;
+          }
           if (g != g_cur) {
-            if (best) atomicMax(&gkeys[b * n_groups + g_cur], (unsigned long long)best);
+            if (best) atomicMax(&gkeys[b * row_stride + g_cur], (unsigned long long)best);
             g_cur = g;
             best = k;
           } else if (k > best) {
@@ -145,12 +160,30 @@ group_max_kernel(const float* __restrict__ scores, const int32_t* __restrict__ c
         }
       }
     }
-    const unsigned long long slot = best ? (unsigned long long)(b * n_groups + g_cur) : ~0ull;
+    const unsigned long long slot = best ? (unsigned long long)(b * row_stride + g_cur) : ~0ull;
     const unsigned peers = __match_any_sync(0xffffffffu, slot);
     const uint32_t hi = __reduce_max_sync(peers, uint32_t(best >> 32));
     const uint32_t lo = __reduce_max_sync(peers, uint32_t(best >> 32) == hi ? uint32_t(best) : 0u);
     if (best && lane == __ffs(peers) - 1) atomicMax(&gkeys[slot], (unsigned long long)((uint64_t(hi) << 32) | lo));
   }
+}
+
+// gkeys [B, n_groups]: each group's best
+__global__ void __launch_bounds__(256)
+group_max_kernel(const float* __restrict__ scores, const int32_t* __restrict__ cand, const int32_t* __restrict__ n,
+                 int64_t cols, int B, const int32_t* __restrict__ doc_group, int64_t n_groups,
+                 unsigned long long* __restrict__ gkeys) {
+  group_max(scores, cand, n, cols, B, doc_group, n_groups, n_groups, nullptr, gkeys);
+}
+
+// One round of the m best keys per group: rows of stride m * n_groups, bound NULL in the first round, else the
+// previous round's keys
+__global__ void __launch_bounds__(256)
+group_round_max_kernel(const float* __restrict__ scores, const int32_t* __restrict__ cand,
+                       const int32_t* __restrict__ n, int64_t cols, int B, const int32_t* __restrict__ doc_group,
+                       int64_t n_groups, int64_t row_stride, const unsigned long long* __restrict__ bound,
+                       unsigned long long* __restrict__ gkeys) {
+  group_max(scores, cand, n, cols, B, doc_group, n_groups, row_stride, bound, gkeys);
 }
 
 // Digits of the 64-bit key for the radix passes, most significant first (K3b's)
@@ -311,24 +344,40 @@ group_select_kernel(const unsigned long long* __restrict__ gkeys, int64_t n_grou
 }  // namespace
 
 int launch_rank_grouped(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,
-                        int64_t doc_id_base, const int32_t* doc_group, int64_t n_groups, int64_t* d_out_ids,
-                        float* d_out_scores, int32_t* d_out_counts, cudaStream_t st) {
+                        int64_t doc_id_base, const int32_t* doc_group, int64_t n_groups, int max_per_group,
+                        int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t st) {
   const int Rp2 = fpb_next_pow2(R);
   const size_t smem = size_t(Rp2) * 16;  // 64 KB at R = 4096: opt in
-  FPB_CUDA_CHECK(cudaFuncSetAttribute(k6_rank_grouped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-  k6_rank_grouped_kernel<<<B, 1024, smem, st>>>(scores, ids, n, R, Rp2, top_k, doc_id_base, doc_group, n_groups,
-                                               d_out_ids, d_out_scores, d_out_counts);
+  const bool one = max_per_group <= 1;
+  const auto kernel = one ? k6_rank_grouped_kernel<true> : k6_rank_grouped_kernel<false>;
+  FPB_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  kernel<<<B, 1024, smem, st>>>(scores, ids, n, R, Rp2, top_k, doc_id_base, doc_group, n_groups, d_out_ids,
+                                d_out_scores, d_out_counts, max_per_group);
   FPB_LAUNCH_CHECK("k6_rank_grouped");
   return FPB_OK;
 }
 
 int launch_group_max(const float* scores, const int32_t* cand, const int32_t* n, int64_t cols, int B,
-                     const int32_t* doc_group, int64_t n_groups, uint64_t* gkeys, int sm_count, cudaStream_t st) {
-  FPB_CUDA_CHECK(cudaMemsetAsync(gkeys, 0, size_t(B) * n_groups * 8, st));
+                     const int32_t* doc_group, int64_t n_groups, int max_per_group, uint64_t* gkeys, int sm_count,
+                     cudaStream_t st) {
+  const int m = max_per_group > 1 ? max_per_group : 1;
+  FPB_CUDA_CHECK(cudaMemsetAsync(gkeys, 0, size_t(B) * m * n_groups * 8, st));
   const int64_t total = int64_t(B) * ((cols + GM_PER - 1) / GM_PER);
-  group_max_kernel<<<fpb_grid_for(total, 256, sm_count), 256, 0, st>>>(
-      scores, cand, n, cols, B, doc_group, n_groups, reinterpret_cast<unsigned long long*>(gkeys));
-  FPB_LAUNCH_CHECK("group_max");
+  const int grid = fpb_grid_for(total, 256, sm_count);
+  auto* keys = reinterpret_cast<unsigned long long*>(gkeys);
+  if (m == 1) {
+    group_max_kernel<<<grid, 256, 0, st>>>(scores, cand, n, cols, B, doc_group, n_groups, keys);
+    FPB_LAUNCH_CHECK("group_max");
+    return FPB_OK;
+  }
+  // round r: each group's best key below its round r - 1 key, so after m rounds a row holds the m best keys of
+  // every group (fewer, the rest 0, for a group of fewer documents)
+  const int64_t stride = int64_t(m) * n_groups;
+  for (int r = 0; r < m; ++r) {
+    group_round_max_kernel<<<grid, 256, 0, st>>>(scores, cand, n, cols, B, doc_group, n_groups, stride,
+                                                 r ? keys + (r - 1) * n_groups : nullptr, keys + r * n_groups);
+    FPB_LAUNCH_CHECK("group_round_max");
+  }
   return FPB_OK;
 }
 
@@ -344,25 +393,44 @@ int launch_group_select(const uint64_t* gkeys, int64_t n_groups, int B, int top_
   return FPB_OK;
 }
 
-extern "C" int fpb_index_with_groups(fpb_index** out, const fpb_index* ix, const int32_t* d_doc_group,
-                                     int64_t n_groups) {
+namespace {
+
+int index_with_groups(const char* who, fpb_index** out, const fpb_index* ix, const int32_t* d_doc_group,
+                      int64_t n_groups, int max_per_group) {
   if (!out) {
-    fpb_set_error("fpb_index_with_groups: out is NULL");
+    fpb_set_error("%s: out is NULL", who);
     return FPB_ERR_INVALID;
   }
   *out = nullptr;
   if (!ix || !d_doc_group) {
-    fpb_set_error("fpb_index_with_groups: NULL index or group array");
+    fpb_set_error("%s: NULL index or group array", who);
     return FPB_ERR_INVALID;
   }
   if (n_groups < 1 || n_groups > INT32_MAX) {
-    fpb_set_error("fpb_index_with_groups: n_groups=%lld must be in [1, %d]", (long long)n_groups, INT32_MAX);
+    fpb_set_error("%s: n_groups=%lld must be in [1, %d]", who, (long long)n_groups, INT32_MAX);
+    return FPB_ERR_INVALID;
+  }
+  if (max_per_group < 1 || max_per_group > FPB_MAX_PER_GROUP) {
+    fpb_set_error("%s: max_per_group=%d must be in [1, %d]", who, max_per_group, FPB_MAX_PER_GROUP);
     return FPB_ERR_INVALID;
   }
   fpb_index* gx = new fpb_index(*ix);
   gx->doc_group = d_doc_group;
   gx->n_groups = n_groups;
+  gx->max_per_group = max_per_group;
   if (gx->walk) ++gx->walk->refs;
   *out = gx;
   return FPB_OK;
+}
+
+}  // namespace
+
+extern "C" int fpb_index_with_groups(fpb_index** out, const fpb_index* ix, const int32_t* d_doc_group,
+                                     int64_t n_groups) {
+  return index_with_groups("fpb_index_with_groups", out, ix, d_doc_group, n_groups, 1);
+}
+
+extern "C" int fpb_index_with_groups_max(fpb_index** out, const fpb_index* ix, const int32_t* d_doc_group,
+                                         int64_t n_groups, int max_per_group) {
+  return index_with_groups("fpb_index_with_groups_max", out, ix, d_doc_group, n_groups, max_per_group);
 }

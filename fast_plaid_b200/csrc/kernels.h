@@ -179,15 +179,18 @@ int launch_emit_records(const float* exact, const float* approx, const int32_t* 
                         int R, int64_t doc_id_base, fpb_record* d_records, cudaStream_t st);
 
 // ---- Grouped results (groups.cu), on a handle of fpb_index_with_groups ----
-// K6 by group: launch_rank's arguments, then at most one document per group (its best), in the canonical order
+// K6 by group: launch_rank's arguments, then at most max_per_group documents per group (its best ones), in the
+// canonical order
 int launch_rank_grouped(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,
-                        int64_t doc_id_base, const int32_t* doc_group, int64_t n_groups, int64_t* d_out_ids,
-                        float* d_out_scores, int32_t* d_out_counts, cudaStream_t st);
-// gkeys [B, n_groups] (cleared here) = per (query, group) the largest rank_key_f32(score, local id) of row b of
-// scores (stride cols), n[b] entries (n NULL: cols), entry p being document cand[b, p] (cand NULL: p)
+                        int64_t doc_id_base, const int32_t* doc_group, int64_t n_groups, int max_per_group,
+                        int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t st);
+// gkeys [B, m * n_groups] (cleared here), m = max_per_group: round r (at offset r * n_groups of a row) holds per
+// (query, group) the largest rank_key_f32(score, local id) below round r - 1's key, over row b of scores (stride
+// cols), n[b] entries (n NULL: cols), entry p being document cand[b, p] (cand NULL: p).  Round 0 is the group's best.
 int launch_group_max(const float* scores, const int32_t* cand, const int32_t* n, int64_t cols, int B,
-                     const int32_t* doc_group, int64_t n_groups, uint64_t* gkeys, int sm_count, cudaStream_t st);
-// per query the top_k largest non-empty keys of its gkeys row, written as K6 writes its ranking
+                     const int32_t* doc_group, int64_t n_groups, int max_per_group, uint64_t* gkeys, int sm_count,
+                     cudaStream_t st);
+// per query the top_k largest non-empty keys of its gkeys row (n_groups keys), written as K6 writes its ranking
 int launch_group_select(const uint64_t* gkeys, int64_t n_groups, int B, int top_k, int64_t doc_id_base,
                         int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t st);
 // The entry points that do not rank for a caller (sharded steps, records, keys) refuse a handle with groups, before
@@ -208,7 +211,8 @@ inline int launch_rank(const fpb_index* ix, const Ws& ws, int top_k, int64_t* d_
                        int32_t* d_out_counts, cudaStream_t st) {
   if (ix->doc_group)
     return launch_rank_grouped(ws.exact(), ws.rerank(), ws.n_rerank(), ws.L->R, ws.L->B, top_k, ix->doc_id_base,
-                               ix->doc_group, ix->n_groups, d_out_ids, d_out_scores, d_out_counts, st);
+                               ix->doc_group, ix->n_groups, ix->max_per_group, d_out_ids, d_out_scores,
+                               d_out_counts, st);
   return launch_rank(ws.exact(), ws.rerank(), ws.n_rerank(), ws.L->R, ws.L->B, top_k, ix->doc_id_base, d_out_ids,
                      d_out_scores, d_out_counts, st);
 }
@@ -266,8 +270,8 @@ struct ExLayout {
   int64_t off_table;        // i32 ExListTable, built on the host
   int64_t off_cand;         // i32 [B, cap] query b's candidates (its list's ids)
   int64_t off_n_cand;       // i32 [B] their numbers
-  // a handle with groups (top_k > 0): u64 [B, n_groups] group keys, in the accumulator region (free once K7 is
-  // finalized) when they fit there, after everything else otherwise
+  // a handle with groups (top_k > 0): u64 [B, max_per_group * n_groups] group keys, in the accumulator region (free
+  // once K7 is finalized) when they fit there, after everything else otherwise
   int64_t off_gkeys;
   int64_t total_bytes;
 };

@@ -104,6 +104,7 @@ EXPORTED_SYMBOLS = [
     "fpb_index_walk_group",
     "fpb_index_append",
     "fpb_index_with_groups",
+    "fpb_index_with_groups_max",
     "fpb_ivf_append",
     "fpb_docs_compact",
     "fpb_ivf_delete",
@@ -198,6 +199,8 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_index_append.argtypes = [ctypes.POINTER(vp), vp, i64, i64, vp, vp, vp, vp, vp, vp, i64, i64]
         lib.fpb_index_with_groups.restype = i32
         lib.fpb_index_with_groups.argtypes = [ctypes.POINTER(vp), vp, vp, i64]
+        lib.fpb_index_with_groups_max.restype = i32
+        lib.fpb_index_with_groups_max.argtypes = [ctypes.POINTER(vp), vp, vp, i64, i32]
         lib.fpb_ivf_append.restype = i32
         lib.fpb_ivf_append.argtypes = [i32, i64, vp, vp, i64, i64, vp, vp, vp, vp, i64, ctypes.POINTER(i64), vp]
         lib.fpb_docs_compact.restype = i32
@@ -411,13 +414,28 @@ class Filter:
         return Filter(bitmap, [0] * num_queries if mask.dim() == 1 else list(range(F)), n)
 
 
+# The largest max_per_group (FPB_MAX_PER_GROUP): exact search takes one pass over the scores per kept document
+MAX_PER_GROUP = 64
+
+
 @dataclasses.dataclass
 class Groups:
     """Grouped results in their device form: `ids` int32 [num_documents] on the index's device, the group of every
-    document renumbered densely to 0 .. n_groups - 1 (fpb_index_with_groups).  Each query then gets at most one
-    document per group, the group's best."""
+    document renumbered densely to 0 .. n_groups - 1 (fpb_index_with_groups_max).  Each query then gets at most
+    `max_per_group` documents per group, the group's best ones."""
     ids: torch.Tensor
     n_groups: int
+    max_per_group: int = 1
+
+    @staticmethod
+    def check_max_per_group(max_per_group, group_by) -> None:
+        """Refuses a max_per_group that is not an int in [1, MAX_PER_GROUP], or that is not 1 without a group map."""
+        if type(max_per_group) is not int:  # noqa: E721  (bool is an int subclass, and is refused)
+            raise ValueError(f"max_per_group must be an int, got {type(max_per_group).__name__}")
+        if not 1 <= max_per_group <= MAX_PER_GROUP:
+            raise ValueError(f"max_per_group={max_per_group} must be in [1, {MAX_PER_GROUP}]")
+        if max_per_group != 1 and group_by is None:
+            raise ValueError("max_per_group applies to grouped results: pass group_by= as well")
 
     @staticmethod
     def check(group_by, num_documents: int) -> None:
@@ -434,11 +452,13 @@ class Groups:
             raise ValueError("group_by values must be non-negative")
 
     @staticmethod
-    def from_tensor(group_by: torch.Tensor, num_documents: int, device: torch.device | str) -> "Groups":
+    def from_tensor(group_by: torch.Tensor, num_documents: int, device: torch.device | str,
+                    max_per_group: int = 1) -> "Groups":
         """The device form of a user's group map: any non-negative integers, not necessarily dense or sorted."""
         Groups.check(group_by, num_documents)
+        Groups.check_max_per_group(max_per_group, group_by)
         uniq, inverse = torch.unique(group_by.to(device), return_inverse=True)
-        return Groups(inverse.to(torch.int32).contiguous(), max(int(uniq.numel()), 1))
+        return Groups(inverse.to(torch.int32).contiguous(), max(int(uniq.numel()), 1), max_per_group)
 
 
 def _popcount(x: torch.Tensor) -> torch.Tensor:
@@ -913,7 +933,7 @@ class DeviceIndex:
     @contextlib.contextmanager
     def _grouped(self, groups: Groups):
         """Within the block every search of this index ranks by `groups`: the index's handle is swapped for one that
-        carries them (fpb_index_with_groups), under the search lock, and swapped back after."""
+        carries them (fpb_index_with_groups_max), under the search lock, and swapped back after."""
         if (groups.ids.device != self.device or groups.ids.dtype != torch.int32 or groups.ids.dim() != 1
                 or groups.ids.shape[0] != self.num_documents or not groups.ids.is_contiguous()):
             raise ValueError(f"expected contiguous group ids int32 [{self.num_documents}] on {self.device}, got "
@@ -922,8 +942,8 @@ class DeviceIndex:
             if getattr(self, "_handle", None) is None or not self._handle.value:
                 raise RuntimeError("this DeviceIndex has been closed")
             handle = ctypes.c_void_p()
-            _check(self._lib.fpb_index_with_groups(ctypes.byref(handle), self._handle, groups.ids.data_ptr(),
-                                                   groups.n_groups))
+            _check(self._lib.fpb_index_with_groups_max(ctypes.byref(handle), self._handle, groups.ids.data_ptr(),
+                                                       groups.n_groups, groups.max_per_group))
             own, self._handle = self._handle, handle
             try:
                 yield
@@ -1217,8 +1237,8 @@ class DeviceIndex:
         (ids int64 [B, top_k], scores f32 [B, top_k], counts int32 [B]).  Asynchronous.
         `subset`: per query a list of GLOBAL doc ids to restrict the search to
         (search.rs:494-517, :544-547).  `filter`: the same restriction in device form (fpb_search_batch_filter);
-        for the same documents the result is the same bytes.  `groups`: at most one document per group among the
-        n_full_scores / 4 re-ranked ones, each group's best (fpb_index_with_groups)."""
+        for the same documents the result is the same bytes.  `groups`: at most groups.max_per_group documents per
+        group among the n_full_scores / 4 re-ranked ones, each group's best ones (fpb_index_with_groups_max)."""
         if groups is not None:
             with self._grouped(groups):
                 return self.search(queries, params, subset, filter)
@@ -1366,8 +1386,8 @@ class DeviceIndex:
         then a list of its own, with no host list made.  `filter`: the restriction in device form
         (fpb_search_exhaustive_filter); for the same documents the result is the same bytes.
 
-        `groups`: at most one document per group, the group's best, and top_k counts groups: the exhaustive ranking
-        (restricted to the subset or filter) with each group's first document kept."""
+        `groups`: at most groups.max_per_group documents per group, the group's best ones: the exhaustive ranking
+        (restricted to the subset or filter) with each group's first max_per_group documents kept, cut to top_k."""
         if groups is not None:
             with self._grouped(groups):
                 return self.search_exhaustive(queries, top_k, budget_bytes, subset, filter)

@@ -615,14 +615,15 @@ class FastPlaid:
 
     def _search_device(self, idx: DeviceIndex, queries: torch.Tensor, params,
                        subset: list[list[int]] | None = None, group_by: torch.Tensor | None = None,
-                       ) -> list[list[tuple[int, float]]]:
+                       max_per_group: int = 1) -> list[list[tuple[int, float]]]:
         """search_on_device (fast_plaid.py:188-253) for the whole batch."""
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         if self.shard is not None:
             return self._search_sharded(idx, queries, params, subset)
         # the group map is remapped on every device that searches
-        groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device)
+        groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device,
+                                                                          max_per_group)
         if isinstance(subset, _SubsetTensor):
             q16 = queries.to(torch.float16).to(idx.device)
             filt = subset.to_filter(idx, q16.shape[0])
@@ -708,6 +709,7 @@ class FastPlaid:
         subset: list[list[int]] | list[int] | None = None,
         n_processes: int | None = None,  # noqa: ARG002  (CPU-only knob in the reference)
         group_by: torch.Tensor | None = None,
+        max_per_group: int = 1,
     ) -> list[list[tuple[int, float]]]:
         """Search the index (fast_plaid.py:930-983).  Returns, per query, up to ``top_k``
         ``(doc_id, score)`` pairs in rank order.
@@ -726,14 +728,22 @@ class FastPlaid:
         search with ``top_k = n_full_scores // 4`` collapsed to each group's first document and cut to ``top_k``:
         fewer than ``top_k`` documents come back when those re-ranked documents hold fewer groups.  Raise
         ``n_full_scores`` for more, or use ``search_exhaustive``, whose grouping is exact.  Not supported with
-        ``shard=``."""
+        ``shard=``.
+
+        ``max_per_group`` (an int in [1, 64], with ``group_by``) keeps up to that many documents per group: walking
+        the ranking, a document is kept when fewer than ``max_per_group`` documents of its group were kept before
+        it, and ``top_k`` counts documents.  So "the 10 best pages, at most 2 from any one PDF" is ``top_k=10,
+        group_by=pdf_of_page, max_per_group=2``.  ``max_per_group=1`` is the one-per-group result, and one at least
+        as large as every group gives the ungrouped result.  Here too the rule applies to the re-ranked documents."""
+        _engine.Groups.check_max_per_group(max_per_group, group_by)
         self._check_group_by(group_by)
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
         params = DeviceIndex.make_params(top_k, n_full_scores, n_ivf_probe, batch_size)
         if group_by is not None:
             _engine.Groups.check(group_by, search_indices[self.devices[0]].num_documents)
         if len(self.devices) == 1:
-            return self._search_device(search_indices[self.devices[0]], queries, params, subset, group_by)
+            return self._search_device(search_indices[self.devices[0]], queries, params, subset, group_by,
+                                       max_per_group)
         # several devices in ONE process: replicated index, query list split across devices
         # (the reference's multi-GPU mode, fast_plaid.py:893-928)
         n = len(self.devices)
@@ -742,7 +752,8 @@ class FastPlaid:
         sub_chunks = _split_subset(subset, chunk, len(chunks))
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
-                ex.submit(self._search_device, search_indices[d], chunks[i], params, sub_chunks[i], group_by)
+                ex.submit(self._search_device, search_indices[d], chunks[i], params, sub_chunks[i], group_by,
+                          max_per_group)
                 for i, d in enumerate(self.devices)
                 if i < len(chunks)
             ]
@@ -753,10 +764,11 @@ class FastPlaid:
 
     def _search_exhaustive_device(self, idx: DeviceIndex, queries: torch.Tensor, top_k: int,
                                   subset: list[list[int]] | None = None, group_by: torch.Tensor | None = None,
-                                  ) -> list[list[tuple[int, float]]]:
+                                  max_per_group: int = 1) -> list[list[tuple[int, float]]]:
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
-        groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device)
+        groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device,
+                                                                          max_per_group)
         q16 = queries.to(device=idx.device, dtype=torch.float16)  # the fp16 cast of `search` (fast_plaid.py:241)
         if isinstance(subset, _SubsetTensor) and subset.per_query and subset.data.dtype != torch.bool:
             # candidate rows to re-rank: each row is a list of the list walk as it stands
@@ -809,6 +821,7 @@ class FastPlaid:
         top_k: int = 10,
         subset: list[list[int]] | list[int] | None = None,
         group_by: torch.Tensor | None = None,
+        max_per_group: int = 1,
     ) -> list[list[tuple[int, float]]]:
         """Exact search: score EVERY document with the exact MaxSim formula of the re-rank stage and return,
         per query, the ``top_k`` best ``(doc_id, score)`` pairs in rank order (score desc, then id asc).
@@ -838,7 +851,9 @@ class FastPlaid:
 
         ``group_by`` (as in ``search``) returns at most one document per group, exactly: the full ranking of the
         query (restricted to ``subset``) with each group's first document kept, ``top_k`` <= 4096 groups.  Not
-        supported with ``shard=``."""
+        supported with ``shard=``.  ``max_per_group`` (as in ``search``) keeps each group's first ``max_per_group``
+        documents of that ranking, exactly; ``top_k`` then counts documents."""
+        _engine.Groups.check_max_per_group(max_per_group, group_by)
         self._check_group_by(group_by)
         if self.shard is not None and not (subset is None or (isinstance(subset, list) and not subset)):
             raise NotImplementedError(
@@ -861,7 +876,8 @@ class FastPlaid:
         if self.shard is not None:
             return self._search_exhaustive_sharded(search_indices[self.devices[0]], queries, top_k)
         if len(self.devices) == 1:
-            return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k, subset, group_by)
+            return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k, subset, group_by,
+                                                  max_per_group)
         # several devices in ONE process hold replicas: the query list is split across them, like `search`
         n = len(self.devices)
         chunk = math.ceil(queries.shape[0] / n)
@@ -870,7 +886,7 @@ class FastPlaid:
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
                 ex.submit(self._search_exhaustive_device, search_indices[d], chunks[i], top_k, sub_chunks[i],
-                          group_by)
+                          group_by, max_per_group)
                 for i, d in enumerate(self.devices)
                 if i < len(chunks)
             ]
@@ -891,11 +907,13 @@ class FastPlaid:
         subset: list[list[int]] | list[int] | None = None,
         n_processes: int | None = None,
         group_by: torch.Tensor | None = None,
+        max_per_group: int = 1,
     ) -> list[list[tuple[int, float, torch.Tensor]]]:
         """``search`` plus, per result, the ``[query_tokens, doc_tokens]`` fp16 similarity
-        matrix (fast_plaid.py:985-1043, search.rs:668-686).  ``group_by``: as in ``search``."""
+        matrix (fast_plaid.py:985-1043, search.rs:668-686).  ``group_by`` and ``max_per_group``: as in ``search``."""
+        _engine.Groups.check_max_per_group(max_per_group, group_by)
         base = self.search(queries_embeddings, top_k, batch_size, n_full_scores, n_ivf_probe, show_progress,
-                           subset, n_processes, group_by)
+                           subset, n_processes, group_by, max_per_group)
         search_indices, queries, _ = self._prepare_search(queries_embeddings, None)
         # several devices in one process hold replicas: any of them can produce every matrix
         idx = search_indices[self.devices[0]]

@@ -138,8 +138,21 @@ int fpb_index_append(fpb_index** out, const fpb_index* index, int64_t n_docs, in
  *   - The sharded entry points and those that emit records or keys return FPB_ERR_UNSUPPORTED.
  * NULL pointers and n_groups outside [1, INT32_MAX] are refused before any CUDA call.  Destroy the handle with
  * fpb_index_destroy; `index` stays valid.  fpb_index_append on it returns a handle without groups.
+ *
+ * fpb_index_with_groups_max -- the same handle carrying max_per_group = m in [1, FPB_MAX_PER_GROUP]: each query keeps
+ * up to m documents per group.  The ranking is the canonical one (restricted to the query's subset) with a document
+ * kept when fewer than m documents of its group were kept before it; top_k counts documents, scores stay the
+ * ungrouped ones bit for bit.  m = 1 is fpb_index_with_groups; m >= the largest group gives the ungrouped ranking.
+ *   - The search entry points apply the rule to the re-ranked list, as above.
+ *   - The exhaustive entry points stay exact: m rounds of the group maximum, round r bounded by round r - 1's key.
+ *     Their *_workspace_bytes report the larger scratch, [B, m * n_groups] u64 beyond what the accumulator region
+ *     holds.
+ * m outside [1, FPB_MAX_PER_GROUP] is refused with the other arguments, before any CUDA call.
  */
 int fpb_index_with_groups(fpb_index** out, const fpb_index* index, const int32_t* d_doc_group, int64_t n_groups);
+#define FPB_MAX_PER_GROUP 64
+int fpb_index_with_groups_max(fpb_index** out, const fpb_index* index, const int32_t* d_doc_group, int64_t n_groups,
+                              int max_per_group);
 
 /*
  * fpb_ivf_append -- the inverted file of an index of n_old_docs documents grown by n_new_docs documents (ids
