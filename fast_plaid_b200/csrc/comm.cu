@@ -138,7 +138,7 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
                                         int B, int Q, const fpb_params* p, void* d_ws, size_t ws_bytes, void* d_scratch,
                                         size_t scratch_bytes, int64_t* d_out_ids, float* d_out_scores,
                                         int32_t* d_out_counts, void* stream) {
-  FPB_TRY(fpb_refuse_groups("fpb_search_batch_sharded", ix));
+  FPB_TRY(fpb_refuse_unsharded_groups("fpb_search_batch_sharded", ix));
   if (!ix || !comm || !p || !d_queries || !d_ws || !d_scratch || !d_out_ids || !d_out_scores || !d_out_counts) {
     fpb_set_error("fpb_search_batch_sharded: NULL argument");
     return FPB_ERR_INVALID;
@@ -207,6 +207,10 @@ extern "C" int fpb_search_batch_sharded(const fpb_index* ix, fpb_comm* comm, int
   FPB_NCCL_CHECK(nccl().AllGather(recs, all_recs, size_t(per_rank) * 16, ncclUint8, comm->comm, st));
   // ---- every rank ranks every query in ONE launch: query q belongs to group q / b_local, whose records are the
   //      [n_shards, b_local, R] block of that group in the gathered array (launch_merge with n_queries > b_stride) ----
+  //      on a shard-grouped handle the stages above ran ungrouped, and the merge applies the rule to the R it keeps
+  if (ix->global_group)
+    return launch_merge_grouped(all_recs, n_shards, b_local, B, R, R, p->top_k, ix->global_group, ix->n_total_docs,
+                                ix->max_per_group, d_out_ids, d_out_scores, d_out_counts, st);
   FPB_TRY(launch_merge(all_recs, n_shards, b_local, B, R, p->top_k, d_out_ids, d_out_scores, d_out_counts, st));
   return FPB_OK;
 }
@@ -220,7 +224,7 @@ extern "C" int fpb_search_exhaustive_sharded(const fpb_index* ix, fpb_comm* comm
                                              size_t ws_bytes, void* d_scratch, size_t scratch_bytes,
                                              int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
                                              void* stream) {
-  FPB_TRY(fpb_refuse_groups("fpb_search_exhaustive_sharded", ix));
+  FPB_TRY(fpb_refuse_unsharded_groups("fpb_search_exhaustive_sharded", ix));
   // every refusal comes before the collective and depends only on arguments every rank has in common (the
   // workspace and the scratch are sized per rank by the caller): shapes, pointers, grid, merge limit
   if (top_k < 1) {
@@ -271,6 +275,10 @@ extern "C" int fpb_search_exhaustive_sharded(const fpb_index* ix, fpb_comm* comm
                                          Q, top_k, d_ws, ws_bytes, recs, st));
   }
   FPB_NCCL_CHECK(nccl().AllGather(recs, all_recs, size_t(per_rank) * 16, ncclUint8, comm->comm, st));
+  // on a shard-grouped handle every record is kept (each shard's top_k under the rule, DESIGN §7) and ruled again
+  if (ix->global_group)
+    return launch_merge_grouped(all_recs, n_shards, b_local, B, top_k, n_shards * top_k, top_k, ix->global_group,
+                                ix->n_total_docs, ix->max_per_group, d_out_ids, d_out_scores, d_out_counts, st);
   FPB_TRY(launch_merge(all_recs, n_shards, b_local, B, top_k, top_k, d_out_ids, d_out_scores, d_out_counts, st));
   return FPB_OK;
 }

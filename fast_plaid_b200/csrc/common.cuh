@@ -79,6 +79,10 @@ struct fpb_index {
   int64_t n_groups;
   // documents kept per group (fpb_index_with_groups_max), in [1, FPB_MAX_PER_GROUP] on a handle with groups
   int max_per_group;
+  // a shard-grouped handle (fpb_index_with_shard_groups) also carries the group of every document of the WHOLE
+  // document-sharded index, [n_total_docs] by global id, for the merge across ranks; NULL / 0 otherwise
+  const int32_t* global_group;
+  int64_t n_total_docs;
 };
 
 void fpb_set_error(const char* fmt, ...);

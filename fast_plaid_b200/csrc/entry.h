@@ -41,6 +41,7 @@ struct Call {
       fpb_set_error("search: NULL index, params or workspace");
       return FPB_ERR_INVALID;
     }
+    FPB_TRY(fpb_refuse_shard_groups("search", ix));  // its merge across ranks runs in the sharded entry points only
     if (need_ivf) FPB_TRY(fpb_require_ivf(ix));
     FPB_TRY(fpb_workspace_layout(ix, B, Q, p, &L));
     FPB_TRY(fpb_require_bytes("workspace", L.total_bytes, ws_bytes));

@@ -80,6 +80,7 @@ int exhaustive_layout(const fpb_index* ix, int B, int Q, int top_k, ExLayout* X,
     const int64_t keys = int64_t(ix->max_per_group) * ix->n_groups;  // m rounds of n_groups keys per query
     X->off_gkeys = keys <= cols ? X->off_acc : take(int64_t(B) * keys * 8);
   }
+  if (sel && ix->global_group) X->off_sel_ids = take(int64_t(B) * top_k * 8);
   X->total_bytes = off;
   return FPB_OK;
 }
@@ -129,6 +130,7 @@ extern "C" int fpb_exhaustive_workspace_bytes(const fpb_index* ix, int B, int Q,
 
 extern "C" int fpb_exhaustive_scores(const fpb_index* ix, const void* d_queries, int B, int Q, void* d_ws,
                                      size_t ws_bytes, float* d_scores, void* stream) {
+  FPB_TRY(fpb_refuse_shard_groups("fpb_exhaustive_scores", ix));
   ExLayout X;
   FPB_TRY(exhaustive_layout(ix, B, Q, 0, &X));
   FPB_TRY(check_workspace(X, d_ws, ws_bytes));
@@ -149,13 +151,14 @@ namespace {
 
 // The selected lists of a full scan, in the workspace: per query the n_sel[b] best local documents (ids, scores)
 // by (score desc, id asc), rows of stride top_k.  On a handle with groups nothing is selected: all_scores holds the
-// [B, N] scores and gkeys the group keys' room.
+// [B, N] scores and gkeys the group keys' room (and, on a shard-grouped handle, out_ids the room of global ids).
 struct ExSelected {
   int32_t* n_sel;
   int32_t* ids;
   float* scores;
   float* all_scores;
   uint64_t* gkeys;
+  int64_t* out_ids;
 };
 
 // The grouped ranking of exact search: m rounds of the group maximum over the [B, cols] scores (the m best keys of
@@ -196,6 +199,7 @@ int exhaustive_select(const char* who, const fpb_index* ix, const void* d_querie
   out->scores = reinterpret_cast<float*>(base + X.off_rerank_approx);
   out->all_scores = scores;
   out->gkeys = reinterpret_cast<uint64_t*>(base + X.off_gkeys);
+  out->out_ids = reinterpret_cast<int64_t*>(base + X.off_sel_ids);
   FPB_TRY(launch_exhaustive_scores(ix, X, base, static_cast<const __half*>(d_queries), scores, st));
   if (ix->doc_group) return FPB_OK;
   // every document is a candidate, and its "approximate" score is its exact one: the selected list holds the exact
@@ -208,6 +212,7 @@ int exhaustive_select(const char* who, const fpb_index* ix, const void* d_querie
 extern "C" int fpb_search_exhaustive(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k, void* d_ws,
                                      size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
                                      void* stream) {
+  FPB_TRY(fpb_refuse_shard_groups("fpb_search_exhaustive", ix));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ExSelected sel;
   FPB_TRY(exhaustive_select("fpb_search_exhaustive", ix, d_queries, B, Q, top_k, d_ws, ws_bytes,
@@ -221,11 +226,18 @@ extern "C" int fpb_search_exhaustive(const fpb_index* ix, const void* d_queries,
 
 extern "C" int fpb_shard_exhaustive_records(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
                                             void* d_ws, size_t ws_bytes, fpb_record* d_records, void* stream) {
-  FPB_TRY(fpb_refuse_groups("fpb_shard_exhaustive_records", ix));
+  FPB_TRY(fpb_refuse_unsharded_groups("fpb_shard_exhaustive_records", ix));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   ExSelected sel;
   FPB_TRY(exhaustive_select("fpb_shard_exhaustive_records", ix, d_queries, B, Q, top_k, d_ws, ws_bytes,
                             d_records != nullptr, st, &sel));
+  if (ix->doc_group) {
+    // this shard's top_k under the rule (its local group map), then one record per result: a tail (-inf, -1) is
+    // a padding record
+    FPB_TRY(rank_groups(ix, sel.all_scores, nullptr, nullptr, ix->N, B, top_k, sel.gkeys, sel.out_ids, sel.scores,
+                        sel.n_sel, st));
+    return launch_results_to_records(sel.out_ids, sel.scores, B, top_k, d_records, st);
+  }
   // approx = exact = the score: the merge's "R best by approx" is then the global top_k, ordered by the same score
   return launch_emit_records(sel.scores, sel.scores, sel.ids, sel.n_sel, B, top_k, ix->doc_id_base, d_records, st);
 }
@@ -258,6 +270,7 @@ int exhaustive_list_search(const char* who, const fpb_index* ix, const void* d_q
                            const int32_t* h_query_list,
                            void* d_ws, size_t ws_bytes, int64_t* d_out_ids, float* d_out_scores,
                            int32_t* d_out_counts, void* stream) {
+  FPB_TRY(fpb_refuse_shard_groups(who, ix));
   ExLayout X;
   FPB_TRY(exhaustive_layout(ix, B, Q, top_k, &X, n_lists, max_list_len));
   FPB_TRY(check_workspace(X, d_ws, ws_bytes));

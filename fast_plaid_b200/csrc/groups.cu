@@ -8,6 +8,9 @@
 //     canonical best document, and a maximum does not depend on the order of the atomics.  At m > 1, m rounds of
 //     the maximum (group_round_max_kernel), round r bounded by round r - 1's key, give the m best keys of every
 //     group, and the selection runs over all m * n_groups of them.
+//   - A document-sharded index (fpb_index_with_shard_groups, DESIGN §7): each shard's exact search selects its own
+//     top_k under the rule, and the merge across ranks (k6_merge_grouped_kernel) applies the rule again to the union
+//     with the group map of the whole index; the approximate search merges ungrouped records the same way.
 // A group id outside [0, n_groups) is skipped: the host remap never makes one, but the C ABI is public.
 #include "kernels.h"
 #include "select.cuh"
@@ -341,6 +344,123 @@ group_select_kernel(const unsigned long long* __restrict__ gkeys, int64_t n_grou
   if (tid == 0) out_counts[b] = cnt;
 }
 
+// The grouped shard merge, one CTA per query, over the gathered records in k6_merge_kernel's layout
+// ([query group][n_shards, B, R]).  It is k6_merge_kernel followed by grouped K6's rule:
+//   1. keep the n_keep best records by (approx desc, id asc) -- skipped when n_keep covers every record;
+//   2. order them by (exact desc, id asc);
+//   3. keep sorted position i when fewer than m documents of its group come before it (global_group by global id);
+//   4. write the first top_k kept ones.
+// Shared memory, 11 bytes per record slot (180 KB at the merge limit): keys [P] (the approximate keys, then the exact
+// keys of the Kp2 = next_pow2(min(n_keep, total)) first slots, then the (group, position) keys), pay [P] (the record
+// index of each slot, carried through both sorts) and kept [P].  Ids and scores are read back from the records.
+__global__ void __launch_bounds__(1024)
+k6_merge_grouped_kernel(const fpb_record* __restrict__ all_groups, int n_shards, int B, int R, int P, int Kp2,
+                        int n_keep, int top_k, const int32_t* __restrict__ global_group, int64_t n_total_docs, int m,
+                        int64_t* __restrict__ out_ids, float* __restrict__ out_scores,
+                        int32_t* __restrict__ out_counts) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);  // [P]
+  uint16_t* pay = reinterpret_cast<uint16_t*>(keys + P);    // [P] record index (P <= 2^14)
+  unsigned char* kept = reinterpret_cast<unsigned char*>(pay + P);  // [P]
+  __shared__ int warp_sums[32];
+  __shared__ int s_valid, s_total;
+  const int b = blockIdx.x % B, tid = threadIdx.x;
+  const fpb_record* all = all_groups + int64_t(blockIdx.x / B) * n_shards * B * R;
+  out_ids += int64_t(blockIdx.x - b) * top_k;
+  out_scores += int64_t(blockIdx.x - b) * top_k;
+  out_counts += blockIdx.x - b;
+  const int total = n_shards * R;
+  auto record = [&](int j) -> const fpb_record& { return all[(int64_t(j / R) * B + b) * R + j % R]; };
+  // 1. the global pruning rule, as k6_merge_kernel applies it
+  const bool prune = n_keep < total;
+  int cand = total;  // slots [0, cand) hold the candidate records
+  if (prune) {
+    if (tid == 0) s_valid = 0;
+    __syncthreads();
+    int local_valid = 0;
+    for (int i = tid; i < P; i += 1024) {
+      uint64_t k = 0;
+      if (i < total) {
+        const fpb_record rec = record(i);
+        if (rec.doc_id >= 0) {
+          k = rank_key_f32(rec.approx, uint32_t(rec.doc_id));
+          ++local_valid;
+        }
+      }
+      keys[i] = k;
+      pay[i] = uint16_t(i);
+    }
+    if (local_valid) atomicAdd(&s_valid, local_valid);
+    __syncthreads();
+    block_sort_desc(keys, P, pay);
+    cand = min(s_valid, n_keep);
+  }
+  // 2. the canonical order of the candidates; a padding record, or one of no valid group, is left out
+  for (int i = tid; i < Kp2; i += 1024) {
+    uint64_t k = 0;
+    if (i < cand) {
+      const int j = prune ? int(pay[i]) : i;
+      const fpb_record rec = record(j);
+      if (rec.doc_id >= 0 && rec.doc_id < n_total_docs && global_group[rec.doc_id] >= 0)
+        k = rank_key_f32(rec.exact, uint32_t(rec.doc_id));
+      pay[i] = uint16_t(j);
+    }
+    keys[i] = k;
+    kept[i] = 0;
+  }
+  __syncthreads();
+  block_sort_desc(keys, Kp2, pay);
+  // 3. (group, rank position) keys in place of the exact keys: sorted descending, a group's entries are adjacent and
+  // its best position first, so entry j is among its group's m best when the entry m places before it is of another
+  for (int i = tid; i < Kp2; i += 1024) {
+    uint64_t g = 0;
+    if (keys[i]) g = (uint64_t(uint32_t(global_group[record(pay[i]).doc_id])) << 32) | (0xffffffffu - uint32_t(i));
+    keys[i] = g;
+  }
+  __syncthreads();
+  block_sort_desc(keys, Kp2);
+  for (int j = tid; j < Kp2; j += 1024) {
+    const uint64_t g = keys[j];
+    if (g && (j < m || (keys[j - m] >> 32) != (g >> 32))) kept[0xffffffffu - uint32_t(g)] = 1;
+  }
+  __syncthreads();
+  // 4. ordered compaction of the kept positions: thread t owns positions [t * per, (t + 1) * per)
+  const int per = Kp2 > 1024 ? Kp2 / 1024 : 1;
+  const int i0 = tid * per;
+  int c = 0;
+  for (int u = 0; u < per; ++u) c += (i0 + u < Kp2 && kept[i0 + u]) ? 1 : 0;
+  int pos = block_exclusive_scan(c, warp_sums, &s_total);
+  for (int u = 0; u < per; ++u) {
+    const int i = i0 + u;
+    if (i < Kp2 && kept[i]) {
+      if (pos < top_k) {
+        const fpb_record rec = record(pay[i]);
+        const uint64_t k = rank_key_f32(rec.exact, uint32_t(rec.doc_id));  // the value K6 writes (-0 as +0)
+        out_ids[int64_t(b) * top_k + pos] = int64_t(rank_key_id(k));
+        out_scores[int64_t(b) * top_k + pos] = rank_key_f32_value(k);
+      }
+      ++pos;
+    }
+  }
+  const int cnt = min(top_k, s_total);
+  for (int i = cnt + tid; i < top_k; i += 1024) {
+    out_ids[int64_t(b) * top_k + i] = -1;
+    out_scores[int64_t(b) * top_k + i] = -INFINITY;
+  }
+  if (tid == 0) out_counts[b] = cnt;
+}
+
+__global__ void results_to_records_kernel(const int64_t* __restrict__ ids, const float* __restrict__ scores, int64_t n,
+                                          fpb_record* __restrict__ rec) {
+  const int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  fpb_record o;
+  o.approx = scores[i];
+  o.exact = scores[i];
+  o.doc_id = ids[i];
+  rec[i] = o;
+}
+
 }  // namespace
 
 int launch_rank_grouped(const float* scores, const int32_t* ids, const int32_t* n, int R, int B, int top_k,
@@ -393,6 +513,61 @@ int launch_group_select(const uint64_t* gkeys, int64_t n_groups, int B, int top_
   return FPB_OK;
 }
 
+int launch_merge_grouped(const fpb_record* d_all_records, int n_shards, int b_stride, int n_queries, int R, int n_keep,
+                         int top_k, const int32_t* global_group, int64_t n_total_docs, int max_per_group,
+                         int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t stream) {
+  const char* who = "fpb_merge_shards_grouped";
+  if (!d_all_records || !global_group || !d_out_ids || !d_out_scores || !d_out_counts) {
+    fpb_set_error("%s: NULL record, group or output pointer", who);
+    return FPB_ERR_INVALID;
+  }
+  if (n_shards < 1 || b_stride < 1 || R < 1 || top_k < 1 || n_queries < 0) {
+    fpb_set_error("%s: n_shards=%d B=%d R=%d top_k=%d must be >= 1", who, n_shards, b_stride, R, top_k);
+    return FPB_ERR_INVALID;
+  }
+  if (n_total_docs < 1 || n_total_docs > INT32_MAX) {
+    fpb_set_error("%s: n_total_docs=%lld must be in [1, %d]", who, (long long)n_total_docs, INT32_MAX);
+    return FPB_ERR_INVALID;
+  }
+  if (max_per_group < 1 || max_per_group > FPB_MAX_PER_GROUP) {
+    fpb_set_error("%s: max_per_group=%d must be in [1, %d]", who, max_per_group, FPB_MAX_PER_GROUP);
+    return FPB_ERR_INVALID;
+  }
+  if (n_keep < 1 || int64_t(n_keep) > int64_t(n_shards) * R) {
+    fpb_set_error("%s: n_keep=%d must be in [1, n_shards*R = %lld]", who, n_keep, (long long)(int64_t(n_shards) * R));
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(check_merge_records(who, n_shards, R));
+  if (n_queries == 0) return FPB_OK;
+  const int total = n_shards * R;
+  const int P = fpb_next_pow2(total);
+  const int Kp2 = fpb_next_pow2(n_keep < total ? n_keep : total);
+  const size_t smem = size_t(P) * (8 + 2 + 1);  // keys, pay, kept: 180 224 B at the limit
+  // opt in on every launch: the attribute is per device and the call costs about a microsecond
+  FPB_CUDA_CHECK(cudaFuncSetAttribute(k6_merge_grouped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  k6_merge_grouped_kernel<<<n_queries, 1024, smem, stream>>>(d_all_records, n_shards, b_stride, R, P, Kp2, n_keep,
+                                                            top_k, global_group, n_total_docs, max_per_group,
+                                                            d_out_ids, d_out_scores, d_out_counts);
+  FPB_LAUNCH_CHECK("k6_merge_grouped");
+  return FPB_OK;
+}
+
+int launch_results_to_records(const int64_t* ids, const float* scores, int B, int top_k, fpb_record* d_records,
+                              cudaStream_t st) {
+  const int64_t n = int64_t(B) * top_k;
+  results_to_records_kernel<<<int((n + 255) / 256), 256, 0, st>>>(ids, scores, n, d_records);
+  FPB_LAUNCH_CHECK("results_to_records");
+  return FPB_OK;
+}
+
+extern "C" int fpb_merge_shards_grouped(const fpb_record* d_all_records, int n_shards, int B, int R, int n_keep,
+                                        int top_k, const int32_t* d_global_group, int64_t n_total_docs,
+                                        int max_per_group, int64_t* d_out_ids, float* d_out_scores,
+                                        int32_t* d_out_counts, void* stream) {
+  return launch_merge_grouped(d_all_records, n_shards, B, B, R, n_keep, top_k, d_global_group, n_total_docs,
+                              max_per_group, d_out_ids, d_out_scores, d_out_counts, static_cast<cudaStream_t>(stream));
+}
+
 namespace {
 
 int index_with_groups(const char* who, fpb_index** out, const fpb_index* ix, const int32_t* d_doc_group,
@@ -418,6 +593,8 @@ int index_with_groups(const char* who, fpb_index** out, const fpb_index* ix, con
   gx->doc_group = d_doc_group;
   gx->n_groups = n_groups;
   gx->max_per_group = max_per_group;
+  gx->global_group = nullptr;  // fpb_index_with_shard_groups sets them
+  gx->n_total_docs = 0;
   if (gx->walk) ++gx->walk->refs;
   *out = gx;
   return FPB_OK;
@@ -433,4 +610,24 @@ extern "C" int fpb_index_with_groups(fpb_index** out, const fpb_index* ix, const
 extern "C" int fpb_index_with_groups_max(fpb_index** out, const fpb_index* ix, const int32_t* d_doc_group,
                                          int64_t n_groups, int max_per_group) {
   return index_with_groups("fpb_index_with_groups_max", out, ix, d_doc_group, n_groups, max_per_group);
+}
+
+extern "C" int fpb_index_with_shard_groups(fpb_index** out, const fpb_index* ix, const int32_t* d_doc_group,
+                                           int64_t n_groups, int max_per_group, const int32_t* d_global_group,
+                                           int64_t n_total_docs) {
+  const char* who = "fpb_index_with_shard_groups";
+  if (out) *out = nullptr;
+  if (out && ix && !d_global_group) {
+    fpb_set_error("%s: NULL global group array", who);
+    return FPB_ERR_INVALID;
+  }
+  if (out && ix && (n_total_docs < 1 || n_total_docs > INT32_MAX || ix->doc_id_base + ix->N > n_total_docs)) {
+    fpb_set_error("%s: n_total_docs=%lld must be in [1, %d] and cover the shard's documents [%lld, %lld)", who,
+                  (long long)n_total_docs, INT32_MAX, (long long)ix->doc_id_base, (long long)(ix->doc_id_base + ix->N));
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(index_with_groups(who, out, ix, d_doc_group, n_groups, max_per_group));
+  (*out)->global_group = d_global_group;
+  (*out)->n_total_docs = n_total_docs;
+  return FPB_OK;
 }

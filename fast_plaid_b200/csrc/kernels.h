@@ -193,11 +193,32 @@ int launch_group_max(const float* scores, const int32_t* cand, const int32_t* n,
 // per query the top_k largest non-empty keys of its gkeys row (n_groups keys), written as K6 writes its ranking
 int launch_group_select(const uint64_t* gkeys, int64_t n_groups, int B, int top_k, int64_t doc_id_base,
                         int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t st);
+// The grouped shard merge: launch_merge's records and query layout, the n_keep best by approx kept, ordered by exact,
+// then at most max_per_group documents per group, the group of global id d being global_group[d] (a record whose id
+// is outside [0, n_total_docs) or whose group is negative is skipped).  Checks every argument before any CUDA call.
+int launch_merge_grouped(const fpb_record* d_all_records, int n_shards, int b_stride, int n_queries, int R, int n_keep,
+                         int top_k, const int32_t* global_group, int64_t n_total_docs, int max_per_group,
+                         int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts, cudaStream_t stream);
+// records [B, top_k] of K6-style results: (score, score, id) for every entry, so a tail (-inf, -1) is a padding record
+int launch_results_to_records(const int64_t* ids, const float* scores, int B, int top_k, fpb_record* d_records,
+                              cudaStream_t st);
 // The entry points that do not rank for a caller (sharded steps, records, keys) refuse a handle with groups, before
 // any CUDA call
 inline int fpb_refuse_groups(const char* who, const fpb_index* ix) {
   if (!ix || !ix->doc_group) return FPB_OK;
   fpb_set_error("%s: an index handle with groups (fpb_index_with_groups) is not supported here", who);
+  return FPB_ERR_UNSUPPORTED;
+}
+// The sharded entry points that merge across ranks take a shard-grouped handle (fpb_index_with_shard_groups) and refuse
+// the other handles with groups, which carry no map of the whole index
+inline int fpb_refuse_unsharded_groups(const char* who, const fpb_index* ix) {
+  return ix && ix->global_group ? FPB_OK : fpb_refuse_groups(who, ix);
+}
+// Every other entry point refuses a shard-grouped handle, before any CUDA call
+inline int fpb_refuse_shard_groups(const char* who, const fpb_index* ix) {
+  if (!ix || !ix->global_group) return FPB_OK;
+  fpb_set_error("%s: a shard-grouped index handle (fpb_index_with_shard_groups) is accepted by the sharded search "
+                "entry points only", who);
   return FPB_ERR_UNSUPPORTED;
 }
 
@@ -273,6 +294,8 @@ struct ExLayout {
   // a handle with groups (top_k > 0): u64 [B, max_per_group * n_groups] group keys, in the accumulator region (free
   // once K7 is finalized) when they fit there, after everything else otherwise
   int64_t off_gkeys;
+  // a shard-grouped handle (top_k > 0): i64 [B, top_k] the ids of the shard's grouped top_k, before they become records
+  int64_t off_sel_ids;
   int64_t total_bytes;
 };
 

@@ -105,6 +105,7 @@ EXPORTED_SYMBOLS = [
     "fpb_index_append",
     "fpb_index_with_groups",
     "fpb_index_with_groups_max",
+    "fpb_index_with_shard_groups",
     "fpb_ivf_append",
     "fpb_docs_compact",
     "fpb_ivf_delete",
@@ -136,6 +137,7 @@ EXPORTED_SYMBOLS = [
     "fpb_stage_records",
     "fpb_search_shard",
     "fpb_merge_shards",
+    "fpb_merge_shards_grouped",
     "fpb_shard_approx_keys",
     "fpb_shard_subset_begin",
     "fpb_shard_subset_keys",
@@ -201,6 +203,8 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_index_with_groups.argtypes = [ctypes.POINTER(vp), vp, vp, i64]
         lib.fpb_index_with_groups_max.restype = i32
         lib.fpb_index_with_groups_max.argtypes = [ctypes.POINTER(vp), vp, vp, i64, i32]
+        lib.fpb_index_with_shard_groups.restype = i32
+        lib.fpb_index_with_shard_groups.argtypes = [ctypes.POINTER(vp), vp, vp, i64, i32, vp, i64]
         lib.fpb_ivf_append.restype = i32
         lib.fpb_ivf_append.argtypes = [i32, i64, vp, vp, i64, i64, vp, vp, vp, vp, i64, ctypes.POINTER(i64), vp]
         lib.fpb_docs_compact.restype = i32
@@ -290,6 +294,8 @@ def load_library() -> ctypes.CDLL:
                                                       sz, vp, vp, vp, vp, vp, vp, vp, vp]
         lib.fpb_merge_shards.restype = i32
         lib.fpb_merge_shards.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp]
+        lib.fpb_merge_shards_grouped.restype = i32
+        lib.fpb_merge_shards_grouped.argtypes = [vp, i32, i32, i32, i32, i32, vp, i64, i32, vp, vp, vp, vp]
         lib.fpb_reconstruct.restype = i32
         lib.fpb_reconstruct.argtypes = [vp, vp, i32, vp, vp, vp]
         for name in ("fpb_cast_f32_to_f16_host", "fpb_cast_f32_to_f16_host_portable"):
@@ -422,10 +428,13 @@ MAX_PER_GROUP = 64
 class Groups:
     """Grouped results in their device form: `ids` int32 [num_documents] on the index's device, the group of every
     document renumbered densely to 0 .. n_groups - 1 (fpb_index_with_groups_max).  Each query then gets at most
-    `max_per_group` documents per group, the group's best ones."""
+    `max_per_group` documents per group, the group's best ones.  On one shard of a document-sharded index
+    (`for_shard`), `ids` covers the shard's documents and `global_ids` int32 [n_total] the whole index's, for the merge
+    across ranks (fpb_index_with_shard_groups)."""
     ids: torch.Tensor
     n_groups: int
     max_per_group: int = 1
+    global_ids: torch.Tensor | None = None
 
     @staticmethod
     def check_max_per_group(max_per_group, group_by) -> None:
@@ -459,6 +468,23 @@ class Groups:
         Groups.check_max_per_group(max_per_group, group_by)
         uniq, inverse = torch.unique(group_by.to(device), return_inverse=True)
         return Groups(inverse.to(torch.int32).contiguous(), max(int(uniq.numel()), 1), max_per_group)
+
+    @staticmethod
+    def for_shard(group_by: torch.Tensor, doc_id_base: int, num_documents: int, device: torch.device | str,
+                  max_per_group: int = 1) -> "Groups":
+        """The device form of a group map of the WHOLE document-sharded index for the shard holding global ids
+        [doc_id_base, doc_id_base + num_documents): its slice renumbered densely (`ids`) and the whole map renumbered
+        densely (`global_ids`, the same on every rank that passes the same map)."""
+        if not isinstance(group_by, torch.Tensor) or group_by.dim() != 1 or group_by.shape[0] < doc_id_base + num_documents:
+            raise ValueError(f"group_by must cover the whole index, at least the shard's documents "
+                             f"[{doc_id_base}, {doc_id_base + num_documents})")
+        Groups.check(group_by, group_by.shape[0])
+        Groups.check_max_per_group(max_per_group, group_by)
+        whole = group_by.to(device)
+        local = Groups.from_tensor(whole[doc_id_base : doc_id_base + num_documents], num_documents, device,
+                                   max_per_group)
+        local.global_ids = torch.unique(whole, return_inverse=True)[1].to(torch.int32).contiguous()
+        return local
 
 
 def _popcount(x: torch.Tensor) -> torch.Tensor:
@@ -933,24 +959,35 @@ class DeviceIndex:
     @contextlib.contextmanager
     def _grouped(self, groups: Groups):
         """Within the block every search of this index ranks by `groups`: the index's handle is swapped for one that
-        carries them (fpb_index_with_groups_max), under the search lock, and swapped back after."""
-        if (groups.ids.device != self.device or groups.ids.dtype != torch.int32 or groups.ids.dim() != 1
-                or groups.ids.shape[0] != self.num_documents or not groups.ids.is_contiguous()):
-            raise ValueError(f"expected contiguous group ids int32 [{self.num_documents}] on {self.device}, got "
-                             f"{groups.ids.dtype} {list(groups.ids.shape)} on {groups.ids.device}")
+        carries them (fpb_index_with_groups_max; fpb_index_with_shard_groups when they carry `global_ids`), under the
+        search lock, and swapped back after.  groups=None: the block runs on the index's own handle."""
+        if groups is None:
+            yield
+            return
+        gl = groups.global_ids
+        for t, n in ((groups.ids, self.num_documents), (gl, None)):
+            if t is not None and (t.device != self.device or t.dtype != torch.int32 or t.dim() != 1
+                                  or (n is not None and t.shape[0] != n) or not t.is_contiguous()):
+                raise ValueError(f"expected contiguous group ids int32 [{n if n is not None else 'n_total'}] on "
+                                 f"{self.device}, got {t.dtype} {list(t.shape)} on {t.device}")
         with self._search_lock:
             if getattr(self, "_handle", None) is None or not self._handle.value:
                 raise RuntimeError("this DeviceIndex has been closed")
             handle = ctypes.c_void_p()
-            _check(self._lib.fpb_index_with_groups_max(ctypes.byref(handle), self._handle, groups.ids.data_ptr(),
-                                                       groups.n_groups, groups.max_per_group))
+            if gl is None:
+                _check(self._lib.fpb_index_with_groups_max(ctypes.byref(handle), self._handle, groups.ids.data_ptr(),
+                                                           groups.n_groups, groups.max_per_group))
+            else:
+                _check(self._lib.fpb_index_with_shard_groups(ctypes.byref(handle), self._handle, groups.ids.data_ptr(),
+                                                             groups.n_groups, groups.max_per_group, gl.data_ptr(),
+                                                             gl.shape[0]))
             own, self._handle = self._handle, handle
             try:
                 yield
             finally:
                 self._handle = own
                 self._lib.fpb_index_destroy(handle)
-                self._groups_keepalive = groups.ids  # until the stream has consumed them
+                self._groups_keepalive = (groups.ids, gl)  # until the stream has consumed them
 
     # -- lifetime ------------------------------------------------------------------------
     def close(self) -> None:
@@ -1518,10 +1555,16 @@ class DeviceIndex:
         self._keepalive = keep  # until the stream has consumed them
 
     # -- document-sharded exhaustive search ------------------------------------------------------
-    def shard_exhaustive_records(self, queries: torch.Tensor, top_k: int) -> torch.Tensor:
+    def shard_exhaustive_records(self, queries: torch.Tensor, top_k: int,
+                                 groups: Groups | None = None) -> torch.Tensor:
         """Step-wise sharded exhaustive search, local half: uint8 [B, top_k, 16] records (score f32 twice, global
         doc id i64) of this shard's top_k documents per query, padded with (-inf, -inf, -1).  The shards' records,
-        all-gathered, go to `merge_records(all_records, top_k)`.  Asynchronous."""
+        all-gathered, go to `merge_records(all_records, top_k)`.  Asynchronous.  `groups` (Groups.for_shard): the
+        shard's top_k under the group rule; the records then go to `merge_records(all_records, top_k, groups,
+        n_keep=n_shards * top_k)`."""
+        if groups is not None:
+            with self._grouped(groups):
+                return self.shard_exhaustive_records(queries, top_k)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k = int(top_k)
@@ -1535,20 +1578,29 @@ class DeviceIndex:
         return rec
 
     def exhaustive_sharded_step(self, n_query_groups: int, B: int, Q: int, top_k: int,
-                                budget_bytes: int = 6 << 30) -> int:
+                                budget_bytes: int = 6 << 30, groups: Groups | None = None) -> int:
         """Most queries per `search_exhaustive_sharded` call whose workspace on this rank, that of
         ceil(step / n_query_groups) queries, fits `budget_bytes`.  It depends on this shard's document count, so the
-        ranks must agree on one step (the smallest of theirs) before the first collective call."""
+        ranks must agree on one step (the smallest of theirs) before the first collective call.  `groups`: the
+        workspace of the grouped call."""
+        if groups is not None:
+            with self._grouped(groups):
+                return self.exhaustive_sharded_step(n_query_groups, B, Q, top_k, budget_bytes)
         G = max(int(n_query_groups), 1)
         return min(B, self._exhaustive_step(-(-B // G), Q, top_k, budget_bytes) * G)
 
     def search_exhaustive_sharded(self, comm: ShardComm, n_query_groups: int, queries: torch.Tensor, top_k: int,
-                                  step: int | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                                  step: int | None = None,
+                                  groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Exhaustive search of a document-sharded index (fpb_search_exhaustive_sharded): queries fp16 [B, Q, D] on
         this device, the SAME batch on every rank of `comm` (collective call).  Returns device tensors (ids, scores,
         counts) for all B queries, the bytes `search_exhaustive` gives on one GPU holding the whole index.
         `step`: queries per collective call, the same on every rank (default: the whole batch in one call;
-        `exhaustive_sharded_step` gives this rank's largest within a memory budget).  Asynchronous."""
+        `exhaustive_sharded_step` gives this rank's largest within a memory budget).  Asynchronous.  `groups`
+        (Groups.for_shard): the grouped result of the whole index, exactly."""
+        if groups is not None:
+            with self._grouped(groups):
+                return self.search_exhaustive_sharded(comm, n_query_groups, queries, top_k, step)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k, G = int(top_k), int(n_query_groups)
@@ -1705,10 +1757,14 @@ class DeviceIndex:
             self._scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
         return buf, self._scratch
 
-    def search_sharded(self, comm: ShardComm, n_query_groups: int, queries: torch.Tensor,
-                       params: FpbParams) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    def search_sharded(self, comm: ShardComm, n_query_groups: int, queries: torch.Tensor, params: FpbParams,
+                       groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries: fp16 [B, Q, D] on this device, the SAME batch on every rank of `comm` (collective call).
-        Returns device tensors (ids, scores, counts) for all B queries."""
+        Returns device tensors (ids, scores, counts) for all B queries.  `groups` (Groups.for_shard): the merge keeps
+        at most groups.max_per_group documents per group of the n_full_scores / 4 it re-ranks, as `search` does."""
+        if groups is not None:
+            with self._grouped(groups):
+                return self.search_sharded(comm, n_query_groups, queries, params)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
         k = params.top_k
@@ -1724,8 +1780,12 @@ class DeviceIndex:
         return ids, scores, counts
 
     def search_sharded_host(self, comm: ShardComm, n_query_groups: int, queries_host: torch.Tensor,
-                            params: FpbParams) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                            params: FpbParams,
+                            groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Host-buffer form of `search_sharded`: fp32/fp16 queries in HOST memory in, host tensors out."""
+        if groups is not None:
+            with self._grouped(groups):
+                return self.search_sharded_host(comm, n_query_groups, queries_host, params)
         B, Q, _ = self._check_queries(queries_host, host=True).shape
         with self._exclusive(), torch.cuda.device(self.device):
             io = self._host_io(B, Q, params.top_k)
@@ -1804,15 +1864,29 @@ class DeviceIndex:
         return rec
 
     def merge_records(
-        self, all_records: torch.Tensor, top_k: int
+        self, all_records: torch.Tensor, top_k: int, groups: Groups | None = None, n_keep: int | None = None,
     ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-        """all_records: uint8 [n_shards, B, R, 16] (all-gathered).  Global prune + rank."""
+        """all_records: uint8 [n_shards, B, R, 16] (all-gathered).  Global prune + rank.  `groups` (Groups.for_shard,
+        its `global_ids` read): the n_keep best records by approximate score (default R: the approximate search's
+        pruning; n_shards * R: every record, for exhaustive records) ranked by exact score, at most
+        groups.max_per_group per group (fpb_merge_shards_grouped)."""
         all_records = self._check_gathered(all_records, torch.uint8, (None, 16))
         n_shards, B, R, _ = all_records.shape
         ids = torch.empty((B, top_k), dtype=torch.int64, device=self.device)
         scores = torch.empty((B, top_k), dtype=torch.float32, device=self.device)
         counts = torch.empty((B,), dtype=torch.int32, device=self.device)
         with self._exclusive(), torch.cuda.device(self.device):
+            if groups is not None:
+                gl = groups.global_ids
+                if gl is None or gl.device != self.device or gl.dtype != torch.int32 or not gl.is_contiguous():
+                    raise ValueError(f"merge_records needs the int32 map of the whole index on {self.device} "
+                                     "(Groups.for_shard)")
+                _check(self._lib.fpb_merge_shards_grouped(
+                    all_records.data_ptr(), n_shards, B, R, R if n_keep is None else int(n_keep), top_k,
+                    gl.data_ptr(), gl.shape[0], groups.max_per_group, ids.data_ptr(), scores.data_ptr(),
+                    counts.data_ptr(), self._stream()))
+                self._groups_keepalive = gl  # until the stream has consumed it
+                return ids, scores, counts
             _check(
                 self._lib.fpb_merge_shards(
                     all_records.data_ptr(), n_shards, B, R, top_k, ids.data_ptr(),

@@ -576,10 +576,22 @@ class FastPlaid:
         return None
 
     def _check_group_by(self, group_by) -> None:
-        """`group_by` on a document-sharded index is refused before any communicator or collective exists."""
-        if group_by is not None and self.shard is not None:
-            raise NotImplementedError("group_by= on a document-sharded index is not implemented: each group's best "
-                                      "document would have to be chosen across the ranks")
+        """`group_by` on a document-sharded index of several ranks needs an initialised torch.distributed process
+        group (the map's length is checked against the whole index through it, and the communicator is made through
+        it): refused without one, before any index load or communicator exists."""
+        if group_by is None or self.shard is None or self.shard[1] == 1:
+            return
+        import torch.distributed as dist
+
+        if not dist.is_initialized():
+            raise NotImplementedError(
+                f"group_by= on a document-sharded index of {self.shard[1]} ranks needs an initialised "
+                "torch.distributed process group: FastPlaid exchanges the shards' results over no other channel")
+
+    def _group_count(self, idx: DeviceIndex) -> int:
+        """The length a group map must have: the whole index's document count on a document-sharded index (every rank
+        passes the map of the whole index), the loaded index's elsewhere."""
+        return idx.num_documents if self.shard is None else self._num_documents(idx)
 
     def _num_documents(self, idx: DeviceIndex) -> int:
         """Documents of the whole index, the length of a mask.  On a document-sharded index of several ranks it is
@@ -620,7 +632,7 @@ class FastPlaid:
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         if self.shard is not None:
-            return self._search_sharded(idx, queries, params, subset)
+            return self._search_sharded(idx, queries, params, subset, group_by, max_per_group)
         # the group map is remapped on every device that searches
         groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device,
                                                                           max_per_group)
@@ -653,8 +665,10 @@ class FastPlaid:
         return self._comm
 
     def _search_sharded(self, idx: DeviceIndex, queries: torch.Tensor, params,
-                        subset: list[list[int]] | None = None) -> list[list[tuple[int, float]]]:
-        """Document-sharded search: local records -> NCCL all-gather -> global prune + rank."""
+                        subset: list[list[int]] | None = None, group_by: torch.Tensor | None = None,
+                        max_per_group: int = 1) -> list[list[tuple[int, float]]]:
+        """Document-sharded search: local records -> NCCL all-gather -> global prune + rank (by group with
+        `group_by`, the map of the whole index)."""
         import torch.distributed as dist
 
         def all_gather(t: torch.Tensor) -> torch.Tensor:
@@ -668,13 +682,15 @@ class FastPlaid:
         rank, world = self.shard
         # refused before the communicator or any all-gather exists (subset search: query_groups == 1)
         _engine.check_merge_records(world // self.query_groups if subset is None else world, params.n_full_scores)
+        groups = None if group_by is None else _engine.Groups.for_shard(group_by, idx.doc_id_base, idx.num_documents,
+                                                                        idx.device, max_per_group)
         if subset is None:
             # the whole exchange below the C ABI: one call per batch, both all-gathers on the search stream
             comm = self._shard_comm(idx)
             if queries.device.type == "cpu" and queries.dtype.is_floating_point:
-                return _results_to_lists(*idx.search_sharded_host(comm, self.query_groups, queries, params))
+                return _results_to_lists(*idx.search_sharded_host(comm, self.query_groups, queries, params, groups))
             q16 = queries.to(device=idx.device, dtype=torch.float16)
-            ids, scores, counts = idx.search_sharded(comm, self.query_groups, q16, params)
+            ids, scores, counts = idx.search_sharded(comm, self.query_groups, q16, params, groups)
             return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         if self.query_groups != 1:
             raise NotImplementedError("subset= with query_groups > 1: use query_groups=1 (plain document sharding)")
@@ -694,7 +710,7 @@ class FastPlaid:
         all_keys = all_gather(idx.shard_subset_keys(all_gather(cbitmap), int(q16.shape[1]), params))
         # step 2: exact scores of the globally surviving documents only, all-gather of the records
         rec = idx.shard_exact_records(all_keys, rank, int(q16.shape[1]), params)
-        ids, scores, counts = idx.merge_records(all_gather(rec), params.top_k)
+        ids, scores, counts = idx.merge_records(all_gather(rec), params.top_k, groups)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
     @torch.inference_mode()
@@ -727,8 +743,10 @@ class FastPlaid:
         Grouping applies to the ``n_full_scores / 4`` documents the search re-ranks, so the result is the ungrouped
         search with ``top_k = n_full_scores // 4`` collapsed to each group's first document and cut to ``top_k``:
         fewer than ``top_k`` documents come back when those re-ranked documents hold fewer groups.  Raise
-        ``n_full_scores`` for more, or use ``search_exhaustive``, whose grouping is exact.  Not supported with
-        ``shard=``.
+        ``n_full_scores`` for more, or use ``search_exhaustive``, whose grouping is exact.  On a document-sharded
+        index (``shard=``) every rank passes the map of the WHOLE index (``num_documents`` of all shards) and gets
+        what one GPU holding the whole index returns; several ranks need an initialised ``torch.distributed``
+        process group.
 
         ``max_per_group`` (an int in [1, 64], with ``group_by``) keeps up to that many documents per group: walking
         the ranking, a document is kept when fewer than ``max_per_group`` documents of its group were kept before
@@ -740,7 +758,7 @@ class FastPlaid:
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
         params = DeviceIndex.make_params(top_k, n_full_scores, n_ivf_probe, batch_size)
         if group_by is not None:
-            _engine.Groups.check(group_by, search_indices[self.devices[0]].num_documents)
+            _engine.Groups.check(group_by, self._group_count(search_indices[self.devices[0]]))
         if len(self.devices) == 1:
             return self._search_device(search_indices[self.devices[0]], queries, params, subset, group_by,
                                        max_per_group)
@@ -780,12 +798,13 @@ class FastPlaid:
             ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset, groups=groups)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
-    def _exhaustive_sharded_step(self, idx: DeviceIndex, B: int, Q: int, top_k: int, budget_bytes: int) -> int:
+    def _exhaustive_sharded_step(self, idx: DeviceIndex, B: int, Q: int, top_k: int, budget_bytes: int,
+                                 groups=None) -> int:
         """Queries per collective call of the sharded exhaustive search, the same on every rank.  Each rank's largest
         step within the budget depends on its own document count, and shards differ by up to one document: two
         ranks at a budget boundary would split the batch differently, make different numbers of collective calls
         and hang.  Every rank takes the smallest of the ranks' steps (one all-reduce on the process group)."""
-        step = idx.exhaustive_sharded_step(self.query_groups, B, Q, top_k, budget_bytes)
+        step = idx.exhaustive_sharded_step(self.query_groups, B, Q, top_k, budget_bytes, groups)
         if self.shard[1] > 1:
             import torch.distributed as dist
 
@@ -796,9 +815,11 @@ class FastPlaid:
         return step
 
     def _search_exhaustive_sharded(self, idx: DeviceIndex, queries: torch.Tensor, top_k: int,
-                                   budget_bytes: int = 6 << 30) -> list[list[tuple[int, float]]]:
+                                   budget_bytes: int = 6 << 30, group_by: torch.Tensor | None = None,
+                                   max_per_group: int = 1) -> list[list[tuple[int, float]]]:
         """Document-sharded exhaustive search: per-shard top_k records -> NCCL all-gather -> merge, in one C-ABI call
-        per step of the batch (csrc/comm.cu).  `budget_bytes` bounds each rank's workspace."""
+        per step of the batch (csrc/comm.cu).  `budget_bytes` bounds each rank's workspace.  `group_by`: the map of
+        the whole index; each shard's top_k under the group rule, merged under it."""
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         rank, world = self.shard
@@ -810,8 +831,11 @@ class FastPlaid:
         B, Q, _ = q16.shape
         if B == 0:
             return []
-        step = self._exhaustive_sharded_step(idx, B, Q, int(top_k), budget_bytes)
-        ids, scores, counts = idx.search_exhaustive_sharded(comm, self.query_groups, q16, top_k, step=step)
+        groups = None if group_by is None else _engine.Groups.for_shard(group_by, idx.doc_id_base, idx.num_documents,
+                                                                        idx.device, max_per_group)
+        step = self._exhaustive_sharded_step(idx, B, Q, int(top_k), budget_bytes, groups)
+        ids, scores, counts = idx.search_exhaustive_sharded(comm, self.query_groups, q16, top_k, step=step,
+                                                            groups=groups)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
     @torch.inference_mode()
@@ -850,9 +874,11 @@ class FastPlaid:
         result is the same bytes however the work is ordered or the batch is split.
 
         ``group_by`` (as in ``search``) returns at most one document per group, exactly: the full ranking of the
-        query (restricted to ``subset``) with each group's first document kept, ``top_k`` <= 4096 groups.  Not
-        supported with ``shard=``.  ``max_per_group`` (as in ``search``) keeps each group's first ``max_per_group``
-        documents of that ranking, exactly; ``top_k`` then counts documents."""
+        query (restricted to ``subset``) with each group's first document kept, ``top_k`` <= 4096 groups.  With
+        ``shard=`` too, where every rank passes the map of the whole index and the result is exact as well: each
+        rank selects its own ``top_k`` under the rule, and the merge applies it again.  ``max_per_group`` (as in
+        ``search``) keeps each group's first ``max_per_group`` documents of that ranking, exactly; ``top_k`` then
+        counts documents."""
         _engine.Groups.check_max_per_group(max_per_group, group_by)
         self._check_group_by(group_by)
         if self.shard is not None and not (subset is None or (isinstance(subset, list) and not subset)):
@@ -872,9 +898,10 @@ class FastPlaid:
                 )
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
         if group_by is not None:
-            _engine.Groups.check(group_by, search_indices[self.devices[0]].num_documents)
+            _engine.Groups.check(group_by, self._group_count(search_indices[self.devices[0]]))
         if self.shard is not None:
-            return self._search_exhaustive_sharded(search_indices[self.devices[0]], queries, top_k)
+            return self._search_exhaustive_sharded(search_indices[self.devices[0]], queries, top_k,
+                                                   group_by=group_by, max_per_group=max_per_group)
         if len(self.devices) == 1:
             return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k, subset, group_by,
                                                   max_per_group)

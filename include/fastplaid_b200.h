@@ -538,6 +538,41 @@ int fpb_search_exhaustive_sharded(const fpb_index* index, fpb_comm* comm, int n_
                                   size_t scratch_bytes, int64_t* d_out_ids, float* d_out_scores,
                                   int32_t* d_out_counts, void* stream);
 
+/* Grouped results on a document-sharded index: the bytes that fpb_index_with_groups_max gives on one GPU holding the
+ * whole index, at every shard count and query-group grid.
+ *   fpb_index_with_shard_groups -- a shard-grouped handle over `index` (one shard, documents [doc_id_base,
+ *       doc_id_base + n_docs) of an index of n_total_docs): d_doc_group (i32 [n_docs]) is the group of each local
+ *       document, dense in [0, n_groups); d_global_group (i32 [n_total_docs]) is the group of every document of the
+ *       WHOLE index by global id, the same map on every rank (its ids need not match d_doc_group's: only which
+ *       documents share a group matters).  Both are borrowed, like fpb_index_with_groups' array.  Accepted by:
+ *         - fpb_search_batch_sharded and _host: the local stages run ungrouped and the final merge applies the rule
+ *           to the n_full_scores / 4 documents it keeps, as fpb_search_batch does on one GPU;
+ *         - fpb_shard_exhaustive_records: this shard's top_k under the rule (exact, by the local map), one record per
+ *           result (approx = exact = score), then padding records (-inf, -inf, -1);
+ *         - fpb_search_exhaustive_sharded: those records, one all-gather, then the grouped merge of all of them.
+ *       fpb_exhaustive_workspace_bytes on it adds the group keys (as on a grouped handle) and B * top_k i64.  Every
+ *       other entry point returns FPB_ERR_UNSUPPORTED on it; the step-wise approximate steps (fpb_shard_*) take the
+ *       plain handle and group only in fpb_merge_shards_grouped.  Handles of fpb_index_with_groups(_max) stay refused
+ *       by the sharded entry points: they carry no map of the whole index.
+ *   fpb_merge_shards_grouped -- the step-wise merge: fpb_merge_shards' records [n_shards, B, R], of which the n_keep
+ *       best by approx are kept (n_keep = R for the approximate search, n_shards * R for the exhaustive records, whose
+ *       approx is their exact score), ordered by exact, then at most max_per_group documents per group kept by
+ *       d_global_group, the first top_k of them written as fpb_merge_shards writes its ranking.  A record whose id is
+ *       outside [0, n_total_docs) or whose group is negative is skipped.  Its shared memory is 11 bytes per record
+ *       slot (180 KB at the merge limit); it needs no scratch.
+ * Exact search stays exact: each shard sends the first top_k documents it keeps under the rule, and every document
+ * the rule keeps on the whole index is among its shard's first top_k (DESIGN §7).  Both calls refuse NULL pointers,
+ * n_groups or n_total_docs outside [1, INT32_MAX], max_per_group outside [1, FPB_MAX_PER_GROUP] and n_keep outside
+ * [1, n_shards * R] with FPB_ERR_INVALID before any CUDA call, and the merge limit of fpb_merge_shards with
+ * FPB_ERR_UNSUPPORTED (the sharded entry points on every rank before the first all-gather).  fpb_index_with_shard_groups
+ * also refuses an n_total_docs below the end of the shard's range. */
+int fpb_index_with_shard_groups(fpb_index** out, const fpb_index* index, const int32_t* d_doc_group, int64_t n_groups,
+                                int max_per_group, const int32_t* d_global_group, int64_t n_total_docs);
+int fpb_merge_shards_grouped(const fpb_record* d_all_records /* [n_shards, B, R] */, int n_shards, int B, int R,
+                             int n_keep, int top_k, const int32_t* d_global_group, int64_t n_total_docs,
+                             int max_per_group, int64_t* d_out_ids, float* d_out_scores, int32_t* d_out_counts,
+                             void* stream);
+
 /* ---- by-products of the MaxSim kernel ("next" rows of SURVEY.md 8f-3) ---- */
 /* reconstruct_embeddings (rust/utils/embeddings.rs:12-69): decompressed, normalised
  * fp16 rows of the given local docs, concatenated.  d_out: f16 [sum(len), dim]. */
