@@ -224,6 +224,39 @@ extern "C" int fpb_search_exhaustive(const fpb_index* ix, const void* d_queries,
                      d_out_counts, st);
 }
 
+extern "C" int fpb_stage_group_rank(const fpb_index* ix, const float* d_scores, const int32_t* d_cand,
+                                    const int32_t* d_n, int64_t cols, int B, int top_k, void* d_gkeys,
+                                    size_t gkeys_bytes, int64_t* d_out_ids, float* d_out_scores,
+                                    int32_t* d_out_counts, void* stream) {
+  const char* who = "fpb_stage_group_rank";
+  if (!ix || !ix->doc_group) {
+    fpb_set_error("%s: needs an index handle with groups (fpb_index_with_groups_max)", who);
+    return FPB_ERR_INVALID;
+  }
+  FPB_TRY(fpb_refuse_shard_groups(who, ix));
+  if (!d_scores || !d_gkeys || !d_out_ids || !d_out_scores || !d_out_counts) {
+    fpb_set_error("%s: NULL score, key or output pointer", who);
+    return FPB_ERR_INVALID;
+  }
+  if (B < 1 || cols < 1) {
+    fpb_set_error("%s: B=%d and cols=%lld must be >= 1", who, B, (long long)cols);
+    return FPB_ERR_INVALID;
+  }
+  if (top_k < 1 || top_k > FPB_EX_MAX_TOP_K) {
+    fpb_set_error("%s: top_k=%d must be in [1, %d]", who, top_k, FPB_EX_MAX_TOP_K);
+    return FPB_ERR_INVALID;
+  }
+  const uint64_t row_keys = uint64_t(ix->max_per_group) * uint64_t(ix->n_groups);  // < 2^37: no overflow below
+  if (gkeys_bytes / 8 / uint64_t(B) < row_keys) {
+    fpb_set_error("%s: key scratch too small: need %d * %llu * 8 bytes, have %zu", who, B,
+                  (unsigned long long)row_keys, gkeys_bytes);
+    return FPB_ERR_WORKSPACE;
+  }
+  FPB_CUDA_CHECK(cudaSetDevice(ix->device));
+  return rank_groups(ix, d_scores, d_cand, d_n, cols, B, top_k, static_cast<uint64_t*>(d_gkeys), d_out_ids,
+                     d_out_scores, d_out_counts, static_cast<cudaStream_t>(stream));
+}
+
 extern "C" int fpb_shard_exhaustive_records(const fpb_index* ix, const void* d_queries, int B, int Q, int top_k,
                                             void* d_ws, size_t ws_bytes, fpb_record* d_records, void* stream) {
   FPB_TRY(fpb_refuse_unsharded_groups("fpb_shard_exhaustive_records", ix));

@@ -135,6 +135,7 @@ EXPORTED_SYMBOLS = [
     "fpb_stage_rank",
     "fpb_stage_keys",
     "fpb_stage_records",
+    "fpb_stage_group_rank",
     "fpb_search_shard",
     "fpb_merge_shards",
     "fpb_merge_shards_grouped",
@@ -265,6 +266,8 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_stage_keys.argtypes = [vp, i32, i32, ctypes.POINTER(FpbParams), vp, sz, vp, vp]
         lib.fpb_stage_records.restype = i32
         lib.fpb_stage_records.argtypes = [vp, i32, i32, ctypes.POINTER(FpbParams), vp, sz, vp, vp]
+        lib.fpb_stage_group_rank.restype = i32
+        lib.fpb_stage_group_rank.argtypes = [vp, vp, vp, vp, i64, i32, i32, vp, sz, vp, vp, vp, vp]
         lib.fpb_search_shard.restype = i32
         lib.fpb_search_shard.argtypes = [vp, vp, i32, i32, ctypes.POINTER(FpbParams), vp, sz, vp, vp]
         lib.fpb_shard_approx_keys.restype = i32

@@ -356,6 +356,14 @@ int fpb_stage_keys(const fpb_index*, int B, int Q, const fpb_params*, void* d_wo
                    uint64_t* d_keys, void* stream); /* sharded two-step mode: emit [B, R] approx keys */
 int fpb_stage_records(const fpb_index*, int B, int Q, const fpb_params*, void* d_workspace, size_t,
                       struct fpb_record* d_records, void* stream); /* sharded mode: emit [B, R] records */
+/* The exact grouped ranking of fpb_search_exhaustive over caller-given scores (tests): row b of d_scores [B, cols]
+ * holds d_n[b] scores (d_n NULL: cols); entry p scores local document d_cand[b * cols + p] (d_cand NULL: p), which
+ * must lie in [0, N).  d_gkeys: at least B * max_per_group * n_groups * 8 bytes of scratch.  A handle without groups
+ * or a shard-grouped one, NULL pointers, B or cols below 1, top_k outside [1, 4096] and too little scratch are
+ * refused before any CUDA call. */
+int fpb_stage_group_rank(const fpb_index* grouped, const float* d_scores, const int32_t* d_cand, const int32_t* d_n,
+                         int64_t cols, int B, int top_k, void* d_gkeys, size_t gkeys_bytes, int64_t* d_out_ids,
+                         float* d_out_scores, int32_t* d_out_counts, void* stream);
 
 /* ---- document-sharded search (new; the reference replicates the index and splits the
  * query list, fast_plaid.py:893-928).  Each rank runs fpb_search_shard on its shard and
