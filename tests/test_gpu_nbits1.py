@@ -16,6 +16,7 @@ import pytest
 import torch
 
 import test_gpu_build_kernels as bk
+import test_gpu_exact_kernels as xk
 import test_gpu_exhaustive as ex
 import test_gpu_kernels as gk
 from util import (build_oracle_index, fp16_ulp_diff, make_docs, make_queries, oracle_exact_scores,
@@ -75,24 +76,8 @@ def test_maxsim_dispatch_never_reaches_v4_or_v5(Q, cuda_device, monkeypatch):
 # ---- K7: exhaustive scores --------------------------------------------------------------------------------------------
 @gpu
 @pytest.mark.parametrize("Q", [1, 32, 100, 256])
-def test_exhaustive_scores_against_float64(Q, cuda_device):
-    """Every document of the boundary-length index: each score inside the bracket of the float64 reference's fp16
-    maxima (plus the fp32 rounding of their sum), and the exact sum of the kernel's own maxima."""
-    t, didx, ref = gk._index(DIM, NBITS)
-    q = gk._planted_queries(ref, 3, Q)
-    q16 = torch.from_numpy(q).half().to(cuda_device)
-    got = didx.exhaustive_scores(q16).cpu().numpy().astype(np.float64)
-    empty = ref.lens == 0
-    for b in range(q.shape[0]):
-        lo, hi, ms = ref.maxima(q[b])
-        slack = Q * 2.0 ** -24 * np.abs(ms[~empty]).sum(1)
-        s = got[b, ~empty]
-        assert (got[b, empty] == np.float32(Q * gk.SENTINEL)).all()
-        ok = (lo[~empty].sum(1) - slack <= s) & (s <= hi[~empty].sum(1) + slack)
-        assert ok.all(), f"query {b}: {int((~ok).sum())} scores outside their bracket"
-    B = q.shape[0]
-    maxima = didx.exhaustive_scores(q16.reshape(B * Q, 1, DIM)).cpu().view(B, Q, -1).transpose(1, 2)
-    assert np.array_equal(got.astype(np.float32), maxima.double().sum(-1).float().numpy())
+def test_exhaustive_scores_against_float64(Q, cuda_device, monkeypatch):
+    xk.test_exhaustive_scores_against_float64(DIM, NBITS, Q, dict(xk.K7_CELLS)[Q], cuda_device, monkeypatch)
 
 
 @gpu
