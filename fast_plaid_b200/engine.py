@@ -990,7 +990,7 @@ class DeviceIndex:
             finally:
                 self._handle = own
                 self._lib.fpb_index_destroy(handle)
-                self._groups_keepalive = (groups.ids, gl)  # until the stream has consumed them
+                self._groups_keepalive = self._stream_keep(groups.ids, gl)  # until the stream has consumed them
 
     # -- lifetime ------------------------------------------------------------------------
     def close(self) -> None:
@@ -1211,9 +1211,29 @@ class DeviceIndex:
         """The grow-only device buffer that `workspace` and the exhaustive search carve up (callers hold _exclusive)."""
         with self._lock:
             if self._buf is None or self._buf.numel() < nbytes:
+                self._drop(self._buf)
                 self._buf = None  # free the old buffer before allocating the larger one
                 self._buf = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
             return self._buf
+
+    def _drop(self, cached: torch.Tensor | None) -> None:
+        """Before a cached buffer is dropped: the caching allocator gives a freed block back to the stream it was
+        allocated on, at once, and that stream is not ordered after the calls that used it since.  Marking it used by
+        the current and the previous call's stream (each call waits for the one before, _exclusive) holds the block
+        back until they are done with it."""
+        if cached is not None:
+            for st in {torch.cuda.current_stream(self.device), self._last_stream} - {None}:
+                cached.record_stream(st)
+
+    def _stream_keep(self, *tensors: torch.Tensor | None) -> tuple:
+        """Tensors the caller owns that the call just queued reads: marked used by the current stream, so that the
+        allocator does not hand out their memory before the stream has read it when the caller frees them.  Returns
+        them, for the `_keepalive` attributes that hold them until the next call."""
+        st = torch.cuda.current_stream(self.device)
+        for t in tensors:
+            if t is not None:
+                t.record_stream(st)
+        return tensors
 
     def max_queries_per_call(self, Q: int, params: FpbParams, budget_bytes: int = 6 << 30) -> int:
         key = ("maxq", Q, params.n_ivf_probe, params.n_full_scores, params.top_k, params.flags, budget_bytes)
@@ -1274,7 +1294,8 @@ class DeviceIndex:
         filter: Filter | None = None, groups: Groups | None = None,
     ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries: fp16 [B, Q, D] on this device.  Returns device tensors
-        (ids int64 [B, top_k], scores f32 [B, top_k], counts int32 [B]).  Asynchronous.
+        (ids int64 [B, top_k], scores f32 [B, top_k], counts int32 [B]).  Asynchronous, except with `subset` lists,
+        whose copy from host memory (`_subset_csr`) waits for the stream.
         `subset`: per query a list of GLOBAL doc ids to restrict the search to
         (search.rs:494-517, :544-547).  `filter`: the same restriction in device form (fpb_search_batch_filter);
         for the same documents the result is the same bytes.  `groups`: at most groups.max_per_group documents per
@@ -1318,7 +1339,7 @@ class DeviceIndex:
                             self._stream(),
                         )
                     )
-                    self._keepalive = keep  # until the stream has consumed them
+                    self._keepalive = self._stream_keep(*keep)  # until the stream has consumed them
                 elif subset is None:
                     _check(
                         self._lib.fpb_search_batch(
@@ -1417,7 +1438,8 @@ class DeviceIndex:
                           groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Exact top_k over every document: (ids int64 [B, top_k] global, scores f32 [B, top_k], counts int32 [B]),
         the result contract of `search`.  The batch is split into calls whose workspace fits `budget_bytes`;
-        the result does not depend on the split.  Asynchronous.
+        the result does not depend on the split.  Asynchronous, except with `subset` lists (their copy from host
+        memory waits for the stream) and with `filter` (the workspace is sized by its largest filter, read back).
 
         `subset`: per query a list of GLOBAL doc ids (any order; duplicates and ids outside the index are ignored).
         Query b is then ranked among the documents of subset[b] only, with counts[b] = min(top_k, #documents), and
@@ -1555,7 +1577,7 @@ class DeviceIndex:
                         scores[s:e].data_ptr(), counts[s:e].data_ptr(), self._stream(),
                     )
                 )
-        self._keepalive = keep  # until the stream has consumed them
+            self._keepalive = self._stream_keep(*keep)  # until the stream has consumed them
 
     # -- document-sharded exhaustive search ------------------------------------------------------
     def shard_exhaustive_records(self, queries: torch.Tensor, top_k: int,
@@ -1619,15 +1641,14 @@ class DeviceIndex:
                 b_local = -(-(e - s) // max(G, 1))
                 buf = self._buffer(self.exhaustive_workspace_bytes(b_local, Q, k))
                 need = max(1, int(self._lib.fpb_sharded_scratch_bytes(b_local, k, comm.nranks)))
-                if getattr(self, "_scratch", None) is None or self._scratch.numel() < need:
-                    self._scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+                self._grow_scratch(need)
                 _check(self._lib.fpb_search_exhaustive_sharded(
                     self._handle, comm._handle, G, queries[s:e].data_ptr(), e - s, Q, k, buf.data_ptr(), buf.numel(),
                     self._scratch.data_ptr(), self._scratch.numel(), ids[s:e].data_ptr(), scores[s:e].data_ptr(),
                     counts[s:e].data_ptr(), self._stream()))
         return ids, scores, counts
 
-    def _host_io(self, B: int, Q: int, k: int) -> dict[str, torch.Tensor]:
+    def _host_io(self, B: int, Q: int, k: int) -> dict[str, Any]:
         """Cached pinned + device staging buffers of the host-buffer path."""
         key = (B, Q, k)
         with self._lock:
@@ -1645,12 +1666,16 @@ class DeviceIndex:
                     "h_ids": torch.empty((B, k), dtype=torch.int64).pin_memory(),
                     "h_scores": torch.empty((B, k), dtype=torch.float32).pin_memory(),
                     "h_counts": torch.empty((B,), dtype=torch.int32).pin_memory(),
+                    "staged": torch.cuda.Event(),  # the last stage_queries copy out of h_q
                 }
                 self._io[key] = io
         return io
 
-    def _cast_into_pinned(self, queries_host: torch.Tensor, h_q: torch.Tensor) -> None:
-        """fp32 -> fp16 on the host like the reference (fast_plaid.py:241), straight into pinned memory."""
+    def _cast_into_pinned(self, queries_host: torch.Tensor, io: dict[str, Any]) -> None:
+        """fp32 -> fp16 on the host like the reference (fast_plaid.py:241), straight into the pinned `h_q`, once the
+        copy a previous stage_queries queued out of it has run."""
+        io["staged"].synchronize()
+        h_q = io["h_q"]
         if queries_host.dtype == torch.float32 and queries_host.is_contiguous():
             # single-threaded F16C cast in the library: no dependence on ATen's intra-op pool (csrc/host_cast.cu)
             _check(self._lib.fpb_cast_f32_to_f16_host(queries_host.data_ptr(), h_q.data_ptr(), queries_host.numel()))
@@ -1661,8 +1686,9 @@ class DeviceIndex:
         """Host queries [B, Q, D] -> fp16 device tensor (cached buffer; asynchronous on the current stream)."""
         B, Q, _ = queries_host.shape
         io = self._host_io(B, Q, top_k)
-        self._cast_into_pinned(queries_host, io["h_q"])
+        self._cast_into_pinned(queries_host, io)
         io["d_q"].copy_(io["h_q"], non_blocking=True)
+        io["staged"].record()
         return io["d_q"]
 
     def search_host(
@@ -1683,7 +1709,7 @@ class DeviceIndex:
             params = self._approx_flags(params)
             step = self.max_queries_per_call(Q, params)
             io = self._host_io(B, Q, params.top_k)
-            self._cast_into_pinned(queries_host, io["h_q"])
+            self._cast_into_pinned(queries_host, io)
             queries_host = io["h_q"]
             for s in range(0, B, step):
                 e = min(B, s + step)
@@ -1707,9 +1733,9 @@ class DeviceIndex:
         global doc id i64) for this shard's n_full_scores/4 best candidates per query."""
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
-        buf, lay = self.workspace(B, Q, params)
-        rec = torch.empty((B, lay.R, 16), dtype=torch.uint8, device=self.device)
         with self._exclusive(), torch.cuda.device(self.device):
+            buf, lay = self.workspace(B, Q, params)
+            rec = torch.empty((B, lay.R, 16), dtype=torch.uint8, device=self.device)
             _check(
                 self._lib.fpb_search_shard(
                     self._handle, queries.data_ptr(), B, Q, ctypes.byref(params), buf.data_ptr(), buf.numel(),
@@ -1755,10 +1781,16 @@ class DeviceIndex:
     def _sharded_io(self, comm: ShardComm, n_query_groups: int, B: int, Q: int, params: FpbParams):
         b_local = -(-B // n_query_groups)
         buf, lay = self.workspace(b_local, Q, params)
-        need = int(self._lib.fpb_sharded_scratch_bytes(b_local, lay.R, comm.nranks))
-        if getattr(self, "_scratch", None) is None or self._scratch.numel() < need:
-            self._scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+        self._grow_scratch(int(self._lib.fpb_sharded_scratch_bytes(b_local, lay.R, comm.nranks)))
         return buf, self._scratch
+
+    def _grow_scratch(self, nbytes: int) -> None:
+        """The grow-only scratch of the sharded searches (callers hold _exclusive)."""
+        old = getattr(self, "_scratch", None)
+        if old is None or old.numel() < nbytes:
+            self._drop(old)
+            self._scratch = None
+            self._scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
 
     def search_sharded(self, comm: ShardComm, n_query_groups: int, queries: torch.Tensor, params: FpbParams,
                        groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -1792,7 +1824,7 @@ class DeviceIndex:
         B, Q, _ = self._check_queries(queries_host, host=True).shape
         with self._exclusive(), torch.cuda.device(self.device):
             io = self._host_io(B, Q, params.top_k)
-            self._cast_into_pinned(queries_host, io["h_q"])
+            self._cast_into_pinned(queries_host, io)
             buf, scratch = self._sharded_io(comm, n_query_groups, B, Q, params)
             _check(self._lib.fpb_search_batch_sharded_host(
                 self._handle, comm._handle, n_query_groups, io["h_q"].data_ptr(), B, Q, ctypes.byref(params),
@@ -1805,9 +1837,9 @@ class DeviceIndex:
     def shard_approx_keys(self, queries: torch.Tensor, params: FpbParams) -> torch.Tensor:
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
-        buf, lay = self.workspace(B, Q, params)
-        keys = torch.empty((B, lay.R), dtype=torch.int64, device=self.device)
         with self._exclusive(), torch.cuda.device(self.device):
+            buf, lay = self.workspace(B, Q, params)
+            keys = torch.empty((B, lay.R), dtype=torch.int64, device=self.device)
             _check(self._lib.fpb_shard_approx_keys(self._handle, queries.data_ptr(), B, Q, ctypes.byref(params),
                                                    buf.data_ptr(), buf.numel(), keys.data_ptr(), self._stream()))
         return keys
@@ -1820,19 +1852,22 @@ class DeviceIndex:
         ids, of which this shard reads its own range (fpb_shard_filter_begin)."""
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
-        buf, lay = self.workspace(B, Q, params)
-        cb = torch.empty((B, lay.cbitmap_words), dtype=torch.int32, device=self.device)
         if filter is not None:
             self._check_filter(filter, B)
             h_map = (ctypes.c_int32 * B)(*filter.query_filter)
             with self._exclusive(), torch.cuda.device(self.device):
+                buf, lay = self.workspace(B, Q, params)
+                cb = torch.empty((B, lay.cbitmap_words), dtype=torch.int32, device=self.device)
                 _check(self._lib.fpb_shard_filter_begin(self._handle, queries.data_ptr(), B, Q, ctypes.byref(params),
                                                         filter.bitmap.data_ptr(), filter.n_filters, filter.n_bits,
                                                         h_map, buf.data_ptr(), buf.numel(), cb.data_ptr(),
                                                         self._stream()))
+                self._stream_keep(filter.bitmap)  # the caller may free the filter before the stream reads it
             return cb
         sid, soff, smax = self._subset_csr(subset, 0, B)
         with self._exclusive(), torch.cuda.device(self.device):
+            buf, lay = self.workspace(B, Q, params)
+            cb = torch.empty((B, lay.cbitmap_words), dtype=torch.int32, device=self.device)
             _check(self._lib.fpb_shard_subset_begin(self._handle, queries.data_ptr(), B, Q, ctypes.byref(params),
                                                     sid.data_ptr(), soff.data_ptr(), smax, buf.data_ptr(),
                                                     buf.numel(), cb.data_ptr(), self._stream()))
@@ -1841,11 +1876,11 @@ class DeviceIndex:
 
     def shard_subset_keys(self, all_cbitmaps: torch.Tensor, Q: int, params: FpbParams) -> torch.Tensor:
         """Step 1b: all_cbitmaps int32 [n_shards, B, cbitmap_words] (all-gathered) -> int64 keys [B, R]."""
-        buf, lay = self.workspace(all_cbitmaps.shape[1], Q, params)
-        all_cbitmaps = self._check_gathered(all_cbitmaps, torch.int32, (lay.cbitmap_words,))
-        n_shards, B, _ = all_cbitmaps.shape
-        keys = torch.empty((B, lay.R), dtype=torch.int64, device=self.device)
         with self._exclusive(), torch.cuda.device(self.device):
+            buf, lay = self.workspace(all_cbitmaps.shape[1], Q, params)
+            all_cbitmaps = self._check_gathered(all_cbitmaps, torch.int32, (lay.cbitmap_words,))
+            n_shards, B, _ = all_cbitmaps.shape
+            keys = torch.empty((B, lay.R), dtype=torch.int64, device=self.device)
             _check(self._lib.fpb_shard_subset_keys(self._handle, B, Q, ctypes.byref(params), buf.data_ptr(),
                                                    buf.numel(), all_cbitmaps.data_ptr(), n_shards,
                                                    keys.data_ptr(), self._stream()))
@@ -1854,11 +1889,11 @@ class DeviceIndex:
     def shard_exact_records(self, all_keys: torch.Tensor, rank: int, Q: int, params: FpbParams) -> torch.Tensor:
         """all_keys: int64 [n_shards, B, R] (all-gathered).  Applies the global pruning threshold to
         this shard's list, exact-scores the survivors, returns uint8 [B, R, 16] records."""
-        buf, lay = self.workspace(all_keys.shape[1], Q, params)
-        all_keys = self._check_gathered(all_keys, torch.int64, (lay.R,))
-        n_shards, B, R = all_keys.shape
-        rec = torch.empty((B, R, 16), dtype=torch.uint8, device=self.device)
         with self._exclusive(), torch.cuda.device(self.device):
+            buf, lay = self.workspace(all_keys.shape[1], Q, params)
+            all_keys = self._check_gathered(all_keys, torch.int64, (lay.R,))
+            n_shards, B, R = all_keys.shape
+            rec = torch.empty((B, R, 16), dtype=torch.uint8, device=self.device)
             _check(self._lib.fpb_shard_apply_threshold(self._handle, all_keys.data_ptr(), n_shards, rank,
                                                        B, Q, ctypes.byref(params), buf.data_ptr(), buf.numel(),
                                                        self._stream()))
@@ -1888,7 +1923,7 @@ class DeviceIndex:
                     all_records.data_ptr(), n_shards, B, R, R if n_keep is None else int(n_keep), top_k,
                     gl.data_ptr(), gl.shape[0], groups.max_per_group, ids.data_ptr(), scores.data_ptr(),
                     counts.data_ptr(), self._stream()))
-                self._groups_keepalive = gl  # until the stream has consumed it
+                self._groups_keepalive = self._stream_keep(gl)  # until the stream has consumed it
                 return ids, scores, counts
             _check(
                 self._lib.fpb_merge_shards(
@@ -1909,11 +1944,11 @@ class DeviceIndex:
             order.insert(1, "subset" if filter is None else "filter")
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
-        buf, lay = self.workspace(B, Q, params)
-        st = self._stream()
         p = ctypes.byref(params)
-        out: dict[str, Any] = {"layout": lay, "workspace": buf}
         with self._exclusive(), torch.cuda.device(self.device):
+            buf, lay = self.workspace(B, Q, params)
+            st = self._stream()
+            out: dict[str, Any] = {"layout": lay, "workspace": buf}
             for name in order:
                 if name == "centroid_scores":
                     _check(self._lib.fpb_stage_centroid_scores(self._handle, queries.data_ptr(), B, Q, p,

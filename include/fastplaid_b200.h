@@ -13,8 +13,12 @@
  *     from fpb_last_error() (thread-local).  No exception crosses the boundary.  The
  *     reference's PyValueError / PyRuntimeError (rust/utils/errors.rs:5-7) are raised by
  *     the Python host from these codes;
- *   - all entry points are asynchronous w.r.t. the host on `stream` unless their name
- *     ends in `_host` (those synchronise the stream before returning);
+ *   - every entry point that takes a `stream` runs all its device work on it, and is
+ *     asynchronous w.r.t. the host unless its name ends in `_host` (those synchronise the
+ *     stream before returning) or its comment says "Synchronous on `stream`" (the index
+ *     maintenance calls that read a size back).  The small host tables a call builds
+ *     (the query map of a filtered or list-subset search) are copied from pageable memory
+ *     before the call returns, without waiting for the stream;
  *   - an fpb_index is immutable after creation and may be searched concurrently from
  *     several host threads on different streams with different workspaces, like the
  *     reference's `LoadedIndex` (`unsafe impl Send/Sync`, rust/search/load.rs:58-59).
