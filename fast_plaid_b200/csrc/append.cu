@@ -221,6 +221,7 @@ extern "C" int fpb_index_append(fpb_index** out, const fpb_index* ix, int64_t n_
   nx->max_per_group = 0;
   nx->global_group = nullptr;
   nx->n_total_docs = 0;
+  nx->doc_bias = nullptr;  // so does a bias
   int rc = launch_token_norms(nx, static_cast<__half*>(d_token_norms), ix->E, nullptr);
   if (rc == FPB_OK) rc = fpb_extend_walk_layout(nx, ix->N);  // synchronises the device
   if (rc != FPB_OK) {

@@ -83,7 +83,19 @@ struct fpb_index {
   // document-sharded index, [n_total_docs] by global id, for the merge across ranks; NULL / 0 otherwise
   const int32_t* global_group;
   int64_t n_total_docs;
+  // biased scores (fpb_index_with_bias): an fp32 bias per local document, [N] by local id, borrowed like doc_group.
+  // Every exact score is finished as __fadd_rn(score, doc_bias[d]) where it is stored (K5, K7's finalize), so that
+  // everything that selects on it sees the biased score; NULL on a handle without a bias
+  const float* doc_bias;
 };
+
+// The exact score of document d as every selection sees it: with a bias (BIAS, the template flag of the kernels that
+// finish exact scores), one fp32 addition rounded to nearest, never contracted into a neighbouring multiply
+template <bool BIAS>
+__device__ __forceinline__ float fpb_biased(float s, const float* __restrict__ bias, int64_t d) {
+  if constexpr (BIAS) return __fadd_rn(s, bias[d]);
+  return s;
+}
 
 void fpb_set_error(const char* fmt, ...);
 

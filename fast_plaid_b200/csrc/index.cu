@@ -216,6 +216,30 @@ extern "C" void fpb_index_destroy(fpb_index* index) {
   delete index;
 }
 
+// A handle that shares everything with `ix` (its groups too: derived handles compose in either order) and carries a
+// bias per local document, added to every exact score (K5, K7's finalize)
+extern "C" int fpb_index_with_bias(fpb_index** out, const fpb_index* ix, const float* d_doc_bias, int64_t n_docs) {
+  const char* who = "fpb_index_with_bias";
+  if (!out) {
+    fpb_set_error("%s: out is NULL", who);
+    return FPB_ERR_INVALID;
+  }
+  *out = nullptr;
+  if (!ix || !d_doc_bias) {
+    fpb_set_error("%s: NULL index or bias array", who);
+    return FPB_ERR_INVALID;
+  }
+  if (n_docs != ix->N) {
+    fpb_set_error("%s: the bias has %lld entries, the index %lld documents", who, (long long)n_docs, (long long)ix->N);
+    return FPB_ERR_INVALID;
+  }
+  fpb_index* bx = new fpb_index(*ix);
+  bx->doc_bias = d_doc_bias;
+  if (bx->walk) ++bx->walk->refs;
+  *out = bx;
+  return FPB_OK;
+}
+
 extern "C" int fpb_index_walk_group(const fpb_index* ix) { return ix ? ix->walk_group : -1; }
 
 extern "C" int fpb_index_walk_layout(const fpb_index* ix, int64_t* n_windows, int32_t* d_codes, int64_t* d_win) {

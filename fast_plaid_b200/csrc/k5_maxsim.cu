@@ -25,13 +25,14 @@ struct K5Smem {
   static constexpr int bytes = (K5_TILE * LDS + QP * LDS) * 2 + 4 * QP * 2 + 256 * 8;
 };
 
-template <int D, int NBITS, int QP>
+// BIAS: the score of document d is biased by bias[d] (fpb_index_with_bias); the <false> instances ignore `bias`
+template <int D, int NBITS, int QP, bool BIAS = false>
 __global__ void __launch_bounds__(K5_THREADS)
 k5_maxsim_kernel(const __half* __restrict__ C, const int64_t* __restrict__ doc_offsets,
                  const int32_t* __restrict__ codes, const uint8_t* __restrict__ residuals,
                  const __half* __restrict__ norms, WPerm wp,
                  const __half* __restrict__ Qpad, int Q, int B, int R, const int32_t* __restrict__ n_rerank,
-                 const int32_t* __restrict__ rerank, float* __restrict__ exact) {
+                 const int32_t* __restrict__ rerank, float* __restrict__ exact, const float* __restrict__ bias) {
   constexpr int LDS = K5Smem<D, QP>::LDS;
   constexpr int LPT = lanes_per_token<D, NBITS>();
   constexpr int KS = D / 16;
@@ -131,7 +132,7 @@ k5_maxsim_kernel(const __half* __restrict__ C, const int64_t* __restrict__ doc_o
       }
 #pragma unroll
       for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-      if (lane == 0) exact[int64_t(b) * R + r] = s;
+      if (lane == 0) exact[int64_t(b) * R + r] = fpb_biased<BIAS>(s, bias, d);
     }
   }
 }
@@ -230,14 +231,15 @@ k5_token_norms_kernel(const __half* __restrict__ C, const int32_t* __restrict__ 
 template <int D, int NBITS, int QP>
 int launch_k5_t(const fpb_index* ix, const Ws& ws, cudaStream_t st) {
   const fpb_layout& L = *ws.L;
-  auto kern = k5_maxsim_kernel<D, NBITS, QP>;
+  auto kern = ix->doc_bias ? k5_maxsim_kernel<D, NBITS, QP, true> : k5_maxsim_kernel<D, NBITS, QP>;
   constexpr int smem = K5Smem<D, QP>::bytes;
   // opt in on every launch: the attribute is per device and the call costs about a microsecond
   FPB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int64_t items = int64_t(L.B) * L.R;
   const int blocks = int(items < int64_t(ix->sm_count) * 8 ? items : int64_t(ix->sm_count) * 8);
   kern<<<blocks, K5_THREADS, smem, st>>>(ix->centroids, ix->doc_offsets, ix->doc_codes, ix->doc_residuals, ix->token_norms,
-                                         ix->w_perm, ws.queries(), L.Q, L.B, L.R, ws.n_rerank(), ws.rerank(), ws.exact());
+                                         ix->w_perm, ws.queries(), L.Q, L.B, L.R, ws.n_rerank(), ws.rerank(), ws.exact(),
+                                         ix->doc_bias);
   FPB_LAUNCH_CHECK("k5_maxsim");
   return FPB_OK;
 }

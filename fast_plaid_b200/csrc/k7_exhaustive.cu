@@ -431,21 +431,26 @@ __device__ __forceinline__ float k7_score(unsigned long long sum, bool empty, in
   return empty ? float(Q) * FPB_PAD_SENTINEL : __ll2float_rn(static_cast<long long>(sum)) * (1.0f / 16777216.0f);
 }
 
+// BIAS: the score of document d is biased by bias[d] (fpb_index_with_bias); the <false> instances ignore `bias`
+template <bool BIAS>
 __global__ void k7_finalize_kernel(const unsigned long long* __restrict__ acc, const int64_t* __restrict__ doc_offsets,
-                                   int64_t N, int64_t total, int Q, float* __restrict__ scores) {
+                                   int64_t N, int64_t total, int Q, float* __restrict__ scores,
+                                   const float* __restrict__ bias) {
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
     const int64_t d = i % N;
-    scores[i] = k7_score(acc[i], doc_offsets[d + 1] == doc_offsets[d], Q);
+    scores[i] = fpb_biased<BIAS>(k7_score(acc[i], doc_offsets[d + 1] == doc_offsets[d], Q), bias, d);
   }
 }
 
 // list walk: row b of the [B, cap] arrays k3b_select reads -- the scores of query b's list, its local document ids
 // (the candidates, ascending) and their number.  Positions past the end of the list are not written.
+template <bool BIAS>
 __global__ void k7_list_finalize_kernel(const unsigned long long* __restrict__ acc,
                                         const int64_t* __restrict__ doc_offsets, const int32_t* __restrict__ ids,
                                         const int32_t* __restrict__ count, const int32_t* __restrict__ qlist,
                                         int64_t cap, int64_t total, int Q, float* __restrict__ scores,
-                                        int32_t* __restrict__ cand, int32_t* __restrict__ n_cand) {
+                                        int32_t* __restrict__ cand, int32_t* __restrict__ n_cand,
+                                        const float* __restrict__ bias) {
   for (int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
     const int64_t b = i / cap, p = i % cap;
     const int l = qlist[b], n = count[l];
@@ -453,7 +458,7 @@ __global__ void k7_list_finalize_kernel(const unsigned long long* __restrict__ a
     if (p < n) {
       const int32_t d = ids[l * cap + p];
       cand[i] = d;
-      scores[i] = k7_score(acc[i], doc_offsets[d + 1] == doc_offsets[d], Q);
+      scores[i] = fpb_biased<BIAS>(k7_score(acc[i], doc_offsets[d + 1] == doc_offsets[d], Q), bias, d);
     }
   }
 }
@@ -560,8 +565,9 @@ int launch_exhaustive_scores(const fpb_index* ix, const ExLayout& X, char* ws, c
     return launch_k7_t<c.D, c.NBITS, K7_ALL>(ix, X, ws, dpc, st);
   }));
   const int64_t total = int64_t(X.B) * ix->N;
-  k7_finalize_kernel<<<finalize_blocks(ix, total), 256, 0, st>>>(
-      reinterpret_cast<const unsigned long long*>(ws + X.off_acc), ix->doc_offsets, ix->N, total, X.Q, d_scores);
+  (ix->doc_bias ? k7_finalize_kernel<true> : k7_finalize_kernel<false>)<<<finalize_blocks(ix, total), 256, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(ws + X.off_acc), ix->doc_offsets, ix->N, total, X.Q, d_scores,
+      ix->doc_bias);
   FPB_LAUNCH_CHECK("k7_finalize");
   return FPB_OK;
 }
@@ -598,10 +604,11 @@ int launch_exhaustive_list_scores(const fpb_index* ix, const ExLayout& X, char* 
                          [&](auto c) { return launch_k7_t<c.D, c.NBITS, K7_ALL, true>(ix, X, ws, dpc, st, lst); }));
   // 4. the [B, cap] scores, candidates and counts of the selection
   const int64_t total = int64_t(X.B) * X.cap;
-  k7_list_finalize_kernel<<<finalize_blocks(ix, total), 256, 0, st>>>(
+  (ix->doc_bias ? k7_list_finalize_kernel<true> : k7_list_finalize_kernel<false>)<<<finalize_blocks(ix, total), 256, 0,
+                                                                                      st>>>(
       reinterpret_cast<const unsigned long long*>(ws + X.off_acc), ix->doc_offsets, ids, count, t.qlist, X.cap, total,
       X.Q, reinterpret_cast<float*>(ws + X.off_scores), reinterpret_cast<int32_t*>(ws + X.off_cand),
-      reinterpret_cast<int32_t*>(ws + X.off_n_cand));
+      reinterpret_cast<int32_t*>(ws + X.off_n_cand), ix->doc_bias);
   FPB_LAUNCH_CHECK("k7_list_finalize");
   return FPB_OK;
 }

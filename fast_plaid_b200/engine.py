@@ -106,6 +106,7 @@ EXPORTED_SYMBOLS = [
     "fpb_index_with_groups",
     "fpb_index_with_groups_max",
     "fpb_index_with_shard_groups",
+    "fpb_index_with_bias",
     "fpb_ivf_append",
     "fpb_docs_compact",
     "fpb_ivf_delete",
@@ -206,6 +207,8 @@ def load_library() -> ctypes.CDLL:
         lib.fpb_index_with_groups_max.argtypes = [ctypes.POINTER(vp), vp, vp, i64, i32]
         lib.fpb_index_with_shard_groups.restype = i32
         lib.fpb_index_with_shard_groups.argtypes = [ctypes.POINTER(vp), vp, vp, i64, i32, vp, i64]
+        lib.fpb_index_with_bias.restype = i32
+        lib.fpb_index_with_bias.argtypes = [ctypes.POINTER(vp), vp, vp, i64]
         lib.fpb_ivf_append.restype = i32
         lib.fpb_ivf_append.argtypes = [i32, i64, vp, vp, i64, i64, vp, vp, vp, vp, i64, ctypes.POINTER(i64), vp]
         lib.fpb_docs_compact.restype = i32
@@ -488,6 +491,48 @@ class Groups:
                                    max_per_group)
         local.global_ids = torch.unique(whole, return_inverse=True)[1].to(torch.int32).contiguous()
         return local
+
+
+@dataclasses.dataclass
+class ScoreBias:
+    """A per-document score bias in its device form: `values` fp32 [num_documents], contiguous, on the index's device
+    (fpb_index_with_bias).  Every exact score of document d becomes fp32(score + values[d]), where the score is
+    produced, before anything selects on it."""
+    values: torch.Tensor
+
+    @staticmethod
+    def check(score_bias, num_documents: int | None) -> None:
+        """Refuses a bias that is not a 1-D floating-point tensor of `num_documents` finite values (num_documents=None:
+        any length)."""
+        if not isinstance(score_bias, torch.Tensor):
+            raise ValueError(f"score_bias must be a 1-D floating-point tensor, got {type(score_bias).__name__}")
+        if not score_bias.dtype.is_floating_point:  # bool, integer and complex dtypes are not
+            raise ValueError(f"score_bias must hold floating-point values, got {score_bias.dtype}")
+        if score_bias.dim() != 1:
+            raise ValueError(f"score_bias must be 1-D (one value per document), got shape {list(score_bias.shape)}")
+        if num_documents is not None and score_bias.shape[0] != num_documents:
+            raise ValueError(f"score_bias has {score_bias.shape[0]} entries, the index has {num_documents} documents")
+        if score_bias.numel() and not bool(torch.isfinite(score_bias.to(torch.float32)).all()):
+            raise ValueError("score_bias values must be finite (no NaN or infinity, also after the cast to fp32)")
+
+    @staticmethod
+    def from_tensor(score_bias: torch.Tensor, num_documents: int, device: torch.device | str) -> "ScoreBias":
+        """The device form of a user's bias: any floating-point dtype on any device, converted to fp32."""
+        ScoreBias.check(score_bias, num_documents)
+        return ScoreBias(score_bias.to(device=device, dtype=torch.float32).contiguous())
+
+    @staticmethod
+    def for_shard(score_bias: torch.Tensor, doc_id_base: int, num_documents: int,
+                  device: torch.device | str) -> "ScoreBias":
+        """The device form of a bias of the WHOLE document-sharded index for the shard holding global ids
+        [doc_id_base, doc_id_base + num_documents): its slice.  The whole tensor is checked first, so that every rank
+        passing the same tensor refuses it alike."""
+        if not isinstance(score_bias, torch.Tensor) or score_bias.dim() != 1 \
+                or score_bias.shape[0] < doc_id_base + num_documents:
+            raise ValueError(f"score_bias must cover the whole index, at least the shard's documents "
+                             f"[{doc_id_base}, {doc_id_base + num_documents})")
+        ScoreBias.check(score_bias, score_bias.shape[0])
+        return ScoreBias.from_tensor(score_bias[doc_id_base : doc_id_base + num_documents], num_documents, device)
 
 
 def _popcount(x: torch.Tensor) -> torch.Tensor:
@@ -992,6 +1037,38 @@ class DeviceIndex:
                 self._lib.fpb_index_destroy(handle)
                 self._groups_keepalive = self._stream_keep(groups.ids, gl)  # until the stream has consumed them
 
+    @contextlib.contextmanager
+    def _biased(self, bias: ScoreBias | None):
+        """Within the block every exact score of this index is biased by `bias`: the handle is swapped for one that
+        carries it (fpb_index_with_bias), under the search lock, and swapped back after.  Inside `_grouped` the
+        biased handle keeps the groups (and the other way round).  bias=None: the block runs on the current handle."""
+        if bias is None:
+            yield
+            return
+        v = bias.values
+        if (v.device != self.device or v.dtype != torch.float32 or v.dim() != 1 or v.shape[0] != self.num_documents
+                or not v.is_contiguous()):
+            raise ValueError(f"expected a contiguous score bias float32 [{self.num_documents}] on {self.device}, got "
+                             f"{v.dtype} {list(v.shape)} on {v.device}")
+        with self._search_lock:
+            if getattr(self, "_handle", None) is None or not self._handle.value:
+                raise RuntimeError("this DeviceIndex has been closed")
+            handle = ctypes.c_void_p()
+            _check(self._lib.fpb_index_with_bias(ctypes.byref(handle), self._handle, v.data_ptr(), v.shape[0]))
+            own, self._handle = self._handle, handle
+            try:
+                yield
+            finally:
+                self._handle = own
+                self._lib.fpb_index_destroy(handle)
+                self._bias_keepalive = self._stream_keep(v)  # until the stream has consumed it
+
+    @contextlib.contextmanager
+    def _ranked(self, groups: Groups | None, bias: ScoreBias | None):
+        """`_grouped` and `_biased` together: the block runs on a handle carrying both."""
+        with self._grouped(groups), self._biased(bias):
+            yield
+
     # -- lifetime ------------------------------------------------------------------------
     def close(self) -> None:
         lock = getattr(self, "_search_lock", None)
@@ -1291,7 +1368,7 @@ class DeviceIndex:
 
     def search(
         self, queries: torch.Tensor, params: FpbParams, subset: list[list[int]] | None = None,
-        filter: Filter | None = None, groups: Groups | None = None,
+        filter: Filter | None = None, groups: Groups | None = None, bias: ScoreBias | None = None,
     ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries: fp16 [B, Q, D] on this device.  Returns device tensors
         (ids int64 [B, top_k], scores f32 [B, top_k], counts int32 [B]).  Asynchronous, except with `subset` lists,
@@ -1299,9 +1376,10 @@ class DeviceIndex:
         `subset`: per query a list of GLOBAL doc ids to restrict the search to
         (search.rs:494-517, :544-547).  `filter`: the same restriction in device form (fpb_search_batch_filter);
         for the same documents the result is the same bytes.  `groups`: at most groups.max_per_group documents per
-        group among the n_full_scores / 4 re-ranked ones, each group's best ones (fpb_index_with_groups_max)."""
-        if groups is not None:
-            with self._grouped(groups):
+        group among the n_full_scores / 4 re-ranked ones, each group's best ones (fpb_index_with_groups_max).
+        `bias`: the re-ranked documents' exact scores biased before the ranking (fpb_index_with_bias)."""
+        if groups is not None or bias is not None:
+            with self._ranked(groups, bias):
                 return self.search(queries, params, subset, filter)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
@@ -1435,7 +1513,8 @@ class DeviceIndex:
 
     def search_exhaustive(self, queries: torch.Tensor, top_k: int, budget_bytes: int = 6 << 30,
                           subset: list[list[int]] | torch.Tensor | None = None, filter: Filter | None = None,
-                          groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                          groups: Groups | None = None,
+                          bias: ScoreBias | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Exact top_k over every document: (ids int64 [B, top_k] global, scores f32 [B, top_k], counts int32 [B]),
         the result contract of `search`.  The batch is split into calls whose workspace fits `budget_bytes`;
         the result does not depend on the split.  Asynchronous, except with `subset` lists (their copy from host
@@ -1449,9 +1528,10 @@ class DeviceIndex:
         (fpb_search_exhaustive_filter); for the same documents the result is the same bytes.
 
         `groups`: at most groups.max_per_group documents per group, the group's best ones: the exhaustive ranking
-        (restricted to the subset or filter) with each group's first max_per_group documents kept, cut to top_k."""
-        if groups is not None:
-            with self._grouped(groups):
+        (restricted to the subset or filter) with each group's first max_per_group documents kept, cut to top_k.
+        `bias`: every score biased before anything is selected, exactly (fpb_index_with_bias)."""
+        if groups is not None or bias is not None:
+            with self._ranked(groups, bias):
                 return self.search_exhaustive(queries, top_k, budget_bytes, subset, filter)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
@@ -1581,14 +1661,14 @@ class DeviceIndex:
 
     # -- document-sharded exhaustive search ------------------------------------------------------
     def shard_exhaustive_records(self, queries: torch.Tensor, top_k: int,
-                                 groups: Groups | None = None) -> torch.Tensor:
+                                 groups: Groups | None = None, bias: ScoreBias | None = None) -> torch.Tensor:
         """Step-wise sharded exhaustive search, local half: uint8 [B, top_k, 16] records (score f32 twice, global
         doc id i64) of this shard's top_k documents per query, padded with (-inf, -inf, -1).  The shards' records,
         all-gathered, go to `merge_records(all_records, top_k)`.  Asynchronous.  `groups` (Groups.for_shard): the
         shard's top_k under the group rule; the records then go to `merge_records(all_records, top_k, groups,
         n_keep=n_shards * top_k)`."""
-        if groups is not None:
-            with self._grouped(groups):
+        if groups is not None or bias is not None:
+            with self._ranked(groups, bias):
                 return self.shard_exhaustive_records(queries, top_k)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
@@ -1616,15 +1696,16 @@ class DeviceIndex:
 
     def search_exhaustive_sharded(self, comm: ShardComm, n_query_groups: int, queries: torch.Tensor, top_k: int,
                                   step: int | None = None,
-                                  groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                                  groups: Groups | None = None,
+                                  bias: ScoreBias | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Exhaustive search of a document-sharded index (fpb_search_exhaustive_sharded): queries fp16 [B, Q, D] on
         this device, the SAME batch on every rank of `comm` (collective call).  Returns device tensors (ids, scores,
         counts) for all B queries, the bytes `search_exhaustive` gives on one GPU holding the whole index.
         `step`: queries per collective call, the same on every rank (default: the whole batch in one call;
         `exhaustive_sharded_step` gives this rank's largest within a memory budget).  Asynchronous.  `groups`
         (Groups.for_shard): the grouped result of the whole index, exactly."""
-        if groups is not None:
-            with self._grouped(groups):
+        if groups is not None or bias is not None:
+            with self._ranked(groups, bias):
                 return self.search_exhaustive_sharded(comm, n_query_groups, queries, top_k, step)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
@@ -1693,12 +1774,13 @@ class DeviceIndex:
 
     def search_host(
         self, queries_host: torch.Tensor, params: FpbParams, groups: Groups | None = None,
+        bias: ScoreBias | None = None,
     ) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries_host: float [B, Q, D] in HOST memory.  The H2D copy, the search and the D2H copies of the
         results all happen inside the C-ABI call, which synchronises the stream.  Returns HOST tensors
         (ids, scores, counts).  `groups`: as in `search`."""
-        if groups is not None:
-            with self._grouped(groups):
+        if groups is not None or bias is not None:
+            with self._ranked(groups, bias):
                 return self.search_host(queries_host, params)
         B, Q, _ = self._check_queries(queries_host, host=True).shape
         if B == 0:
@@ -1793,12 +1875,13 @@ class DeviceIndex:
             self._scratch = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
 
     def search_sharded(self, comm: ShardComm, n_query_groups: int, queries: torch.Tensor, params: FpbParams,
-                       groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                       groups: Groups | None = None,
+                       bias: ScoreBias | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """queries: fp16 [B, Q, D] on this device, the SAME batch on every rank of `comm` (collective call).
         Returns device tensors (ids, scores, counts) for all B queries.  `groups` (Groups.for_shard): the merge keeps
         at most groups.max_per_group documents per group of the n_full_scores / 4 it re-ranks, as `search` does."""
-        if groups is not None:
-            with self._grouped(groups):
+        if groups is not None or bias is not None:
+            with self._ranked(groups, bias):
                 return self.search_sharded(comm, n_query_groups, queries, params)
         queries = self._check_queries(queries)
         B, Q, _ = queries.shape
@@ -1816,10 +1899,11 @@ class DeviceIndex:
 
     def search_sharded_host(self, comm: ShardComm, n_query_groups: int, queries_host: torch.Tensor,
                             params: FpbParams,
-                            groups: Groups | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                            groups: Groups | None = None,
+                            bias: ScoreBias | None = None) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Host-buffer form of `search_sharded`: fp32/fp16 queries in HOST memory in, host tensors out."""
-        if groups is not None:
-            with self._grouped(groups):
+        if groups is not None or bias is not None:
+            with self._ranked(groups, bias):
                 return self.search_sharded_host(comm, n_query_groups, queries_host, params)
         B, Q, _ = self._check_queries(queries_host, host=True).shape
         with self._exclusive(), torch.cuda.device(self.device):
@@ -1886,9 +1970,14 @@ class DeviceIndex:
                                                    keys.data_ptr(), self._stream()))
         return keys
 
-    def shard_exact_records(self, all_keys: torch.Tensor, rank: int, Q: int, params: FpbParams) -> torch.Tensor:
+    def shard_exact_records(self, all_keys: torch.Tensor, rank: int, Q: int, params: FpbParams,
+                            bias: ScoreBias | None = None) -> torch.Tensor:
         """all_keys: int64 [n_shards, B, R] (all-gathered).  Applies the global pruning threshold to
-        this shard's list, exact-scores the survivors, returns uint8 [B, R, 16] records."""
+        this shard's list, exact-scores the survivors, returns uint8 [B, R, 16] records.  `bias`
+        (ScoreBias.for_shard): the exact scores are biased."""
+        if bias is not None:
+            with self._biased(bias):
+                return self.shard_exact_records(all_keys, rank, Q, params)
         with self._exclusive(), torch.cuda.device(self.device):
             buf, lay = self.workspace(all_keys.shape[1], Q, params)
             all_keys = self._check_gathered(all_keys, torch.int64, (lay.R,))

@@ -588,6 +588,21 @@ class FastPlaid:
                 f"group_by= on a document-sharded index of {self.shard[1]} ranks needs an initialised "
                 "torch.distributed process group: FastPlaid exchanges the shards' results over no other channel")
 
+    def _check_score_bias(self, score_bias) -> None:
+        """The checks of `score_bias` that need no index: its type, dtype, shape and values (the length is checked
+        against the index once it is loaded).  On a document-sharded index of several ranks, the same need for an
+        initialised torch.distributed process group as `group_by`.  Before any index load or communicator exists."""
+        if score_bias is None:
+            return
+        _engine.ScoreBias.check(score_bias, None)
+        if self.shard is not None and self.shard[1] > 1:
+            import torch.distributed as dist
+
+            if not dist.is_initialized():
+                raise NotImplementedError(
+                    f"score_bias= on a document-sharded index of {self.shard[1]} ranks needs an initialised "
+                    "torch.distributed process group: FastPlaid exchanges the shards' results over no other channel")
+
     def _group_count(self, idx: DeviceIndex) -> int:
         """The length a group map must have: the whole index's document count on a document-sharded index (every rank
         passes the map of the whole index), the loaded index's elsewhere."""
@@ -627,30 +642,32 @@ class FastPlaid:
 
     def _search_device(self, idx: DeviceIndex, queries: torch.Tensor, params,
                        subset: list[list[int]] | None = None, group_by: torch.Tensor | None = None,
-                       max_per_group: int = 1) -> list[list[tuple[int, float]]]:
+                       max_per_group: int = 1,
+                       score_bias: torch.Tensor | None = None) -> list[list[tuple[int, float]]]:
         """search_on_device (fast_plaid.py:188-253) for the whole batch."""
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         if self.shard is not None:
-            return self._search_sharded(idx, queries, params, subset, group_by, max_per_group)
-        # the group map is remapped on every device that searches
+            return self._search_sharded(idx, queries, params, subset, group_by, max_per_group, score_bias)
+        # the group map is remapped, and the bias copied, on every device that searches
         groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device,
                                                                           max_per_group)
+        bias = None if score_bias is None else _engine.ScoreBias.from_tensor(score_bias, idx.num_documents, idx.device)
         if isinstance(subset, _SubsetTensor):
             q16 = queries.to(torch.float16).to(idx.device)
             filt = subset.to_filter(idx, q16.shape[0])
-            ids, scores, counts = idx.search(q16, params, filter=filt, groups=groups)
+            ids, scores, counts = idx.search(q16, params, filter=filt, groups=groups, bias=bias)
             return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         if subset is not None:
             q16 = queries.to(torch.float16).to(idx.device)
-            ids, scores, counts = idx.search(q16, params, subset=subset, groups=groups)
+            ids, scores, counts = idx.search(q16, params, subset=subset, groups=groups, bias=bias)
             return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         if queries.device.type == "cuda":
             q16 = queries.to(device=idx.device, dtype=torch.float16)  # fast_plaid.py:241
-            ids, scores, counts = idx.search(q16, params, groups=groups)
+            ids, scores, counts = idx.search(q16, params, groups=groups, bias=bias)
             return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         # fp16 cast on the host like the reference (fast_plaid.py:241), straight into pinned staging
-        ids, scores, counts = idx.search_host(queries, params, groups=groups)
+        ids, scores, counts = idx.search_host(queries, params, groups=groups, bias=bias)
         return _results_to_lists(ids, scores, counts)
 
     def _shard_comm(self, idx: DeviceIndex):
@@ -666,9 +683,11 @@ class FastPlaid:
 
     def _search_sharded(self, idx: DeviceIndex, queries: torch.Tensor, params,
                         subset: list[list[int]] | None = None, group_by: torch.Tensor | None = None,
-                        max_per_group: int = 1) -> list[list[tuple[int, float]]]:
+                        max_per_group: int = 1,
+                        score_bias: torch.Tensor | None = None) -> list[list[tuple[int, float]]]:
         """Document-sharded search: local records -> NCCL all-gather -> global prune + rank (by group with
-        `group_by`, the map of the whole index)."""
+        `group_by`, the map of the whole index; each shard's exact scores biased by its slice of `score_bias`, the
+        bias of the whole index)."""
         import torch.distributed as dist
 
         def all_gather(t: torch.Tensor) -> torch.Tensor:
@@ -684,13 +703,16 @@ class FastPlaid:
         _engine.check_merge_records(world // self.query_groups if subset is None else world, params.n_full_scores)
         groups = None if group_by is None else _engine.Groups.for_shard(group_by, idx.doc_id_base, idx.num_documents,
                                                                         idx.device, max_per_group)
+        bias = None if score_bias is None else _engine.ScoreBias.for_shard(score_bias, idx.doc_id_base,
+                                                                           idx.num_documents, idx.device)
         if subset is None:
             # the whole exchange below the C ABI: one call per batch, both all-gathers on the search stream
             comm = self._shard_comm(idx)
             if queries.device.type == "cpu" and queries.dtype.is_floating_point:
-                return _results_to_lists(*idx.search_sharded_host(comm, self.query_groups, queries, params, groups))
+                return _results_to_lists(*idx.search_sharded_host(comm, self.query_groups, queries, params, groups,
+                                                                  bias))
             q16 = queries.to(device=idx.device, dtype=torch.float16)
-            ids, scores, counts = idx.search_sharded(comm, self.query_groups, q16, params, groups)
+            ids, scores, counts = idx.search_sharded(comm, self.query_groups, q16, params, groups, bias)
             return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
         if self.query_groups != 1:
             raise NotImplementedError("subset= with query_groups > 1: use query_groups=1 (plain document sharding)")
@@ -709,7 +731,7 @@ class FastPlaid:
             cbitmap = idx.shard_subset_begin(q16, params, subset)
         all_keys = all_gather(idx.shard_subset_keys(all_gather(cbitmap), int(q16.shape[1]), params))
         # step 2: exact scores of the globally surviving documents only, all-gather of the records
-        rec = idx.shard_exact_records(all_keys, rank, int(q16.shape[1]), params)
+        rec = idx.shard_exact_records(all_keys, rank, int(q16.shape[1]), params, bias)
         ids, scores, counts = idx.merge_records(all_gather(rec), params.top_k, groups)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
@@ -726,6 +748,7 @@ class FastPlaid:
         n_processes: int | None = None,  # noqa: ARG002  (CPU-only knob in the reference)
         group_by: torch.Tensor | None = None,
         max_per_group: int = 1,
+        score_bias: torch.Tensor | None = None,
     ) -> list[list[tuple[int, float]]]:
         """Search the index (fast_plaid.py:930-983).  Returns, per query, up to ``top_k``
         ``(doc_id, score)`` pairs in rank order.
@@ -752,16 +775,29 @@ class FastPlaid:
         the ranking, a document is kept when fewer than ``max_per_group`` documents of its group were kept before
         it, and ``top_k`` counts documents.  So "the 10 best pages, at most 2 from any one PDF" is ``top_k=10,
         group_by=pdf_of_page, max_per_group=2``.  ``max_per_group=1`` is the one-per-group result, and one at least
-        as large as every group gives the ungrouped result.  Here too the rule applies to the re-ranked documents."""
+        as large as every group gives the ungrouped result.  Here too the rule applies to the re-ranked documents.
+
+        ``score_bias`` (a 1-D floating-point tensor of ``num_documents`` finite values, on any device, converted to
+        fp32) adds a prior per document, such as recency or source authority: document d is ranked and returned with
+        the score ``fp32(score_d + score_bias[d])``, one fp32 addition.  The bias applies where the exact scores are
+        computed, to the ``n_full_scores / 4`` documents the search re-ranks; the approximate candidate stage does not
+        see it.  So the result is the unbiased search with ``top_k = n_full_scores // 4``, each score biased, re-sorted
+        (score desc, then id asc), grouped by ``group_by`` if given, and cut to ``top_k``.  However large, a bias
+        cannot bring in a document the candidate stage did not re-rank: raise ``n_full_scores``, or use
+        ``search_exhaustive``, where the bias is exact.  On a document-sharded index every rank passes the bias of the
+        WHOLE index, as with ``group_by``."""
         _engine.Groups.check_max_per_group(max_per_group, group_by)
         self._check_group_by(group_by)
+        self._check_score_bias(score_bias)
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
         params = DeviceIndex.make_params(top_k, n_full_scores, n_ivf_probe, batch_size)
         if group_by is not None:
             _engine.Groups.check(group_by, self._group_count(search_indices[self.devices[0]]))
+        if score_bias is not None:
+            _engine.ScoreBias.check(score_bias, self._group_count(search_indices[self.devices[0]]))
         if len(self.devices) == 1:
             return self._search_device(search_indices[self.devices[0]], queries, params, subset, group_by,
-                                       max_per_group)
+                                       max_per_group, score_bias)
         # several devices in ONE process: replicated index, query list split across devices
         # (the reference's multi-GPU mode, fast_plaid.py:893-928)
         n = len(self.devices)
@@ -771,7 +807,7 @@ class FastPlaid:
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
                 ex.submit(self._search_device, search_indices[d], chunks[i], params, sub_chunks[i], group_by,
-                          max_per_group)
+                          max_per_group, score_bias)
                 for i, d in enumerate(self.devices)
                 if i < len(chunks)
             ]
@@ -782,20 +818,23 @@ class FastPlaid:
 
     def _search_exhaustive_device(self, idx: DeviceIndex, queries: torch.Tensor, top_k: int,
                                   subset: list[list[int]] | None = None, group_by: torch.Tensor | None = None,
-                                  max_per_group: int = 1) -> list[list[tuple[int, float]]]:
+                                  max_per_group: int = 1,
+                                  score_bias: torch.Tensor | None = None) -> list[list[tuple[int, float]]]:
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         groups = None if group_by is None else _engine.Groups.from_tensor(group_by, idx.num_documents, idx.device,
                                                                           max_per_group)
+        bias = None if score_bias is None else _engine.ScoreBias.from_tensor(score_bias, idx.num_documents, idx.device)
         q16 = queries.to(device=idx.device, dtype=torch.float16)  # the fp16 cast of `search` (fast_plaid.py:241)
         if isinstance(subset, _SubsetTensor) and subset.per_query and subset.data.dtype != torch.bool:
             # candidate rows to re-rank: each row is a list of the list walk as it stands
-            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset.data.to(idx.device), groups=groups)
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset.data.to(idx.device), groups=groups,
+                                                        bias=bias)
         elif isinstance(subset, _SubsetTensor):
             filt = subset.to_filter(idx, q16.shape[0])
-            ids, scores, counts = idx.search_exhaustive(q16, top_k, filter=filt, groups=groups)
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, filter=filt, groups=groups, bias=bias)
         else:
-            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset, groups=groups)
+            ids, scores, counts = idx.search_exhaustive(q16, top_k, subset=subset, groups=groups, bias=bias)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
     def _exhaustive_sharded_step(self, idx: DeviceIndex, B: int, Q: int, top_k: int, budget_bytes: int,
@@ -816,10 +855,12 @@ class FastPlaid:
 
     def _search_exhaustive_sharded(self, idx: DeviceIndex, queries: torch.Tensor, top_k: int,
                                    budget_bytes: int = 6 << 30, group_by: torch.Tensor | None = None,
-                                   max_per_group: int = 1) -> list[list[tuple[int, float]]]:
+                                   max_per_group: int = 1,
+                                   score_bias: torch.Tensor | None = None) -> list[list[tuple[int, float]]]:
         """Document-sharded exhaustive search: per-shard top_k records -> NCCL all-gather -> merge, in one C-ABI call
         per step of the batch (csrc/comm.cu).  `budget_bytes` bounds each rank's workspace.  `group_by`: the map of
-        the whole index; each shard's top_k under the group rule, merged under it."""
+        the whole index; each shard's top_k under the group rule, merged under it.  `score_bias`: the bias of the whole
+        index; each shard biases its own documents' scores before it selects."""
         if queries.dim() != 3:
             raise ValueError(f"Expected a 3D tensor for queries, but got shape {list(queries.shape)}")
         rank, world = self.shard
@@ -833,9 +874,11 @@ class FastPlaid:
             return []
         groups = None if group_by is None else _engine.Groups.for_shard(group_by, idx.doc_id_base, idx.num_documents,
                                                                         idx.device, max_per_group)
+        bias = None if score_bias is None else _engine.ScoreBias.for_shard(score_bias, idx.doc_id_base,
+                                                                           idx.num_documents, idx.device)
         step = self._exhaustive_sharded_step(idx, B, Q, int(top_k), budget_bytes, groups)
         ids, scores, counts = idx.search_exhaustive_sharded(comm, self.query_groups, q16, top_k, step=step,
-                                                            groups=groups)
+                                                            groups=groups, bias=bias)
         return _results_to_lists(ids.cpu(), scores.cpu(), counts.cpu())
 
     @torch.inference_mode()
@@ -846,6 +889,7 @@ class FastPlaid:
         subset: list[list[int]] | list[int] | None = None,
         group_by: torch.Tensor | None = None,
         max_per_group: int = 1,
+        score_bias: torch.Tensor | None = None,
     ) -> list[list[tuple[int, float]]]:
         """Exact search: score EVERY document with the exact MaxSim formula of the re-rank stage and return,
         per query, the ``top_k`` best ``(doc_id, score)`` pairs in rank order (score desc, then id asc).
@@ -878,9 +922,14 @@ class FastPlaid:
         ``shard=`` too, where every rank passes the map of the whole index and the result is exact as well: each
         rank selects its own ``top_k`` under the rule, and the merge applies it again.  ``max_per_group`` (as in
         ``search``) keeps each group's first ``max_per_group`` documents of that ranking, exactly; ``top_k`` then
-        counts documents."""
+        counts documents.
+
+        ``score_bias`` (as in ``search``) ranks by ``fp32(score_d + score_bias[d])`` and returns that score, exactly:
+        every document (of ``subset``) is biased before the ``top_k`` are selected, and ``group_by`` walks the biased
+        ranking.  With ``shard=`` too, where the result is the same bytes as on one GPU holding the whole index."""
         _engine.Groups.check_max_per_group(max_per_group, group_by)
         self._check_group_by(group_by)
+        self._check_score_bias(score_bias)
         if self.shard is not None and not (subset is None or (isinstance(subset, list) and not subset)):
             raise NotImplementedError(
                 "search_exhaustive with subset= on a document-sharded index is not implemented: each rank would "
@@ -899,12 +948,15 @@ class FastPlaid:
         search_indices, queries, subset = self._prepare_search(queries_embeddings, subset)
         if group_by is not None:
             _engine.Groups.check(group_by, self._group_count(search_indices[self.devices[0]]))
+        if score_bias is not None:
+            _engine.ScoreBias.check(score_bias, self._group_count(search_indices[self.devices[0]]))
         if self.shard is not None:
             return self._search_exhaustive_sharded(search_indices[self.devices[0]], queries, top_k,
-                                                   group_by=group_by, max_per_group=max_per_group)
+                                                   group_by=group_by, max_per_group=max_per_group,
+                                                   score_bias=score_bias)
         if len(self.devices) == 1:
             return self._search_exhaustive_device(search_indices[self.devices[0]], queries, top_k, subset, group_by,
-                                                  max_per_group)
+                                                  max_per_group, score_bias)
         # several devices in ONE process hold replicas: the query list is split across them, like `search`
         n = len(self.devices)
         chunk = math.ceil(queries.shape[0] / n)
@@ -913,7 +965,7 @@ class FastPlaid:
         with ThreadPoolExecutor(max_workers=n) as ex:
             futs = [
                 ex.submit(self._search_exhaustive_device, search_indices[d], chunks[i], top_k, sub_chunks[i],
-                          group_by, max_per_group)
+                          group_by, max_per_group, score_bias)
                 for i, d in enumerate(self.devices)
                 if i < len(chunks)
             ]
@@ -935,12 +987,14 @@ class FastPlaid:
         n_processes: int | None = None,
         group_by: torch.Tensor | None = None,
         max_per_group: int = 1,
+        score_bias: torch.Tensor | None = None,
     ) -> list[list[tuple[int, float, torch.Tensor]]]:
         """``search`` plus, per result, the ``[query_tokens, doc_tokens]`` fp16 similarity
-        matrix (fast_plaid.py:985-1043, search.rs:668-686).  ``group_by`` and ``max_per_group``: as in ``search``."""
+        matrix (fast_plaid.py:985-1043, search.rs:668-686).  ``group_by``, ``max_per_group`` and ``score_bias``: as in
+        ``search``; the scores and the order are the biased ones, the matrices stay the raw similarities."""
         _engine.Groups.check_max_per_group(max_per_group, group_by)
         base = self.search(queries_embeddings, top_k, batch_size, n_full_scores, n_ivf_probe, show_progress,
-                           subset, n_processes, group_by, max_per_group)
+                           subset, n_processes, group_by, max_per_group, score_bias)
         search_indices, queries, _ = self._prepare_search(queries_embeddings, None)
         # several devices in one process hold replicas: any of them can produce every matrix
         idx = search_indices[self.devices[0]]

@@ -159,6 +159,27 @@ int fpb_index_with_groups_max(fpb_index** out, const fpb_index* index, const int
                               int max_per_group);
 
 /*
+ * fpb_index_with_bias -- biased scores: a new handle over every array of `index` (shared, like fpb_index_with_groups'
+ * handles) that also carries d_doc_bias (f32 [n_docs], borrowed: the caller keeps it alive until the handle's last
+ * search has run), a finite bias per local document.  Every exact score the handle produces is then
+ * s'_d = s_d + d_doc_bias[d], one fp32 addition rounded to nearest, and everything that ranks or selects on exact scores
+ * sees s'_d:
+ *   - fpb_exhaustive_scores returns the biased table, and fpb_search_exhaustive, _subset and _filter rank every
+ *     (listed) document by s'_d, exactly, with or without groups;
+ *   - fpb_search_batch, _subset, _filter, _host and fpb_stage_maxsim bias the n_full_scores / 4 documents they re-rank:
+ *     the candidate stage is unchanged, so the result is the unbiased search with top_k = n_full_scores / 4, biased,
+ *     re-sorted by (score desc, id asc), grouped if the handle has groups, cut to top_k;
+ *   - the sharded entry points and their records carry s'_d (each rank passes its slice of the whole index's bias).
+ * The derived handles compose in either order: fpb_index_with_groups(_max) and fpb_index_with_shard_groups on a biased
+ * handle keep the bias, and fpb_index_with_bias on a grouped handle keeps its groups.  A bias of +-inf or NaN is not
+ * checked here (the caller refuses it: a NaN would break the selections' order); a finite sum that overflows is
+ * +-inf, which ranks like any other value.  NULL pointers and n_docs != the index's document count are refused before
+ * any CUDA call.  Destroy the handle with fpb_index_destroy; `index` stays valid.  fpb_index_append on it returns a
+ * handle without a bias.
+ */
+int fpb_index_with_bias(fpb_index** out, const fpb_index* index, const float* d_doc_bias, int64_t n_docs);
+
+/*
  * fpb_ivf_append -- the inverted file of an index of n_old_docs documents grown by n_new_docs documents (ids
  * n_old_docs ..): for every one of the n_cells cells, its old list (d_ivf_offsets i64 [n_cells + 1] into d_ivf_pids)
  * followed by the ascending ids of the new documents with a token in that cell.  The new documents' codes are
