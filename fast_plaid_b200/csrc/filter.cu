@@ -111,62 +111,6 @@ filter_centroids_kernel(const uint32_t* __restrict__ sbitmap, int words, const i
   }
 }
 
-// One CTA per list l: the ids of the set bits of row l of `bitmap` in index order into out[l][0, cap), and their
-// number, at most cap, into n_out[l].  The ordered compaction of k2_compact with its writes bounded by cap: the bits
-// past the cap-th are dropped, so an understated bound cuts a list short instead of writing past it.
-__global__ void __launch_bounds__(1024)
-filter_compact_kernel(const uint32_t* __restrict__ bitmap, int words, int32_t* __restrict__ out, int cap,
-                      int32_t* __restrict__ n_out) {
-  __shared__ int warp_sums[32];
-  __shared__ int s_base;
-  const uint32_t* bm = bitmap + int64_t(blockIdx.x) * words;
-  int32_t* o = out + int64_t(blockIdx.x) * cap;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_base = 0;
-  __syncthreads();
-  for (int w0 = 0; w0 < words && s_base < cap; w0 += 4096) {  // s_base is uniform: read after a barrier
-    const int wi = w0 + tid * 4;  // 4 consecutive words per thread keeps the output ordered
-    uint32_t w[4];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) w[u] = (wi + u < words) ? bm[wi + u] : 0u;
-    const int c = __popc(w[0]) + __popc(w[1]) + __popc(w[2]) + __popc(w[3]);
-    int incl = c;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, incl, off);
-      if (lane >= off) incl += v;
-    }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      const int ws = warp_sums[lane];
-      int wincl = ws;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, wincl, off);
-        if (lane >= off) wincl += v;
-      }
-      warp_sums[lane] = wincl - ws;  // exclusive
-    }
-    __syncthreads();
-    const int base = s_base;
-    int pos = base + warp_sums[warp] + incl - c;
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      uint32_t x = w[u];
-      while (x && pos < cap) {
-        const int bit = __ffs(x) - 1;
-        x &= x - 1;
-        o[pos++] = (wi + u) * 32 + bit;
-      }
-    }
-    __syncthreads();
-    if (tid == 1023) s_base = base + warp_sums[31] + incl;  // total of this round
-    __syncthreads();
-  }
-  if (tid == 0) n_out[blockIdx.x] = s_base < cap ? s_base : cap;
-}
-
 // row b of rows ([B, words]) = row src[b], for every b with src[b] != b
 __global__ void __launch_bounds__(256)
 filter_broadcast_kernel(const int32_t* __restrict__ src, uint32_t* __restrict__ rows, int words) {
@@ -258,9 +202,7 @@ int launch_filter_lists(const fpb_index* ix, const uint32_t* d_filters, int64_t 
         d_filters, filter_words(n_bits), ix->doc_id_base, ix->N, nullptr, nullptr, bitmap, words);
     FPB_LAUNCH_CHECK("filter_expand");
   }
-  filter_compact_kernel<<<n_lists, 1024, 0, st>>>(bitmap, words, ids, cap, count);
-  FPB_LAUNCH_CHECK("filter_compact");
-  return FPB_OK;
+  return launch_compact(bitmap, nullptr, words, ids, cap, count, n_lists, st);
 }
 
 int check_filter_args(const char* who, const uint32_t* d_filters, int n_filters, int64_t n_bits,

@@ -17,38 +17,12 @@
 
 namespace {
 
-// Exclusive prefix of the threads' counts c over a 1024-thread block; *total gets the sum.  warp_sums: 32 ints of
-// shared memory.  Contains two __syncthreads().
-__device__ __forceinline__ int block_exclusive_scan(int c, int* warp_sums, int* total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int incl = c;
-#pragma unroll
-  for (int off = 1; off < 32; off <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, off);
-    if (lane >= off) incl += v;
-  }
-  if (lane == 31) warp_sums[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    const int ws = warp_sums[lane];
-    int wincl = ws;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, wincl, off);
-      if (lane >= off) wincl += v;
-    }
-    warp_sums[lane] = wincl - ws;
-    if (lane == 31) *total = wincl;
-  }
-  __syncthreads();
-  return warp_sums[warp] + incl - c;
-}
-
 __device__ __forceinline__ bool group_ok(int32_t g, int64_t n_groups) { return g >= 0 && int64_t(g) < n_groups; }
 
 // Grouped K6, one CTA per query: row b of exact / rerank (stride R) holds the scores and local ids of n_rerank[b]
 // documents, of which the first m of each group in the canonical order are kept (ONE: the instance for m = 1, which
-// ignores m).  Shared memory: the canonical keys [Rp2], then (group, rank position) keys [Rp2].
+// ignores m).  Shared memory: the canonical keys [Rp2], then gkeys [Rp2], the group rule's (group, rank position)
+// keys and then the kept keys in rank order.
 template <bool ONE>
 __global__ void __launch_bounds__(1024)
 k6_rank_grouped_kernel(const float* __restrict__ exact, const int32_t* __restrict__ rerank,
@@ -58,60 +32,24 @@ k6_rank_grouped_kernel(const float* __restrict__ exact, const int32_t* __restric
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);
   uint64_t* gkeys = keys + Rp2;
-  __shared__ unsigned char first[FPB_EX_MAX_TOP_K];  // first[i]: rank position i is among its group's m best
-  __shared__ int warp_sums[32];
-  __shared__ int s_total;
-  const int b = blockIdx.x, tid = threadIdx.x;
+  __shared__ unsigned char kept[FPB_EX_MAX_TOP_K];  // kept[i]: rank position i is among its group's m best
+  const int b = blockIdx.x;
   const int n = n_rerank[b];
-  // 1. the canonical order of the re-ranked documents (a document of no valid group is left out)
-  for (int i = tid; i < Rp2; i += 1024) {
+  // the canonical order of the re-ranked documents (a document of no valid group is left out)
+  for (int i = threadIdx.x; i < Rp2; i += 1024) {
     uint64_t k = 0;
     if (i < n) {
       const int32_t d = rerank[int64_t(b) * R + i];
       if (group_ok(doc_group[d], n_groups)) k = rank_key_f32(exact[int64_t(b) * R + i], uint32_t(d));
     }
     keys[i] = k;
-    first[i] = 0;
   }
   __syncthreads();
   block_sort_desc(keys, Rp2);
-  // 2. (group, rank position) keys: sorted descending, a group's entries are adjacent and its best position first,
-  // so entry j is among its group's m best when the entry m places before it belongs to another group
-  for (int i = tid; i < Rp2; i += 1024) {
-    uint64_t g = 0;
-    if (keys[i]) g = (uint64_t(uint32_t(doc_group[rank_key_id(keys[i])])) << 32) | (0xffffffffu - uint32_t(i));
-    gkeys[i] = g;
-  }
-  __syncthreads();
-  block_sort_desc(gkeys, Rp2);
-  for (int j = tid; j < Rp2; j += 1024) {
-    const uint64_t g = gkeys[j];
-    if (g && (ONE ? j == 0 || (gkeys[j - 1] >> 32) != (g >> 32) : j < m || (gkeys[j - m] >> 32) != (g >> 32)))
-      first[0xffffffffu - uint32_t(g)] = 1;
-  }
-  __syncthreads();
-  // 3. ordered compaction of the kept positions: thread t owns positions [t * per, (t + 1) * per)
-  const int per = Rp2 > 1024 ? Rp2 / 1024 : 1;
-  const int i0 = tid * per;
-  int c = 0;
-  for (int u = 0; u < per; ++u) c += (i0 + u < Rp2 && first[i0 + u]) ? 1 : 0;
-  int pos = block_exclusive_scan(c, warp_sums, &s_total);
-  for (int u = 0; u < per; ++u) {
-    const int i = i0 + u;
-    if (i < Rp2 && first[i]) {
-      if (pos < top_k) {
-        out_ids[int64_t(b) * top_k + pos] = doc_id_base + int64_t(rank_key_id(keys[i]));
-        out_scores[int64_t(b) * top_k + pos] = rank_key_f32_value(keys[i]);
-      }
-      ++pos;
-    }
-  }
-  const int cnt = min(top_k, s_total);
-  for (int i = cnt + tid; i < top_k; i += 1024) {
-    out_ids[int64_t(b) * top_k + i] = -1;
-    out_scores[int64_t(b) * top_k + i] = -INFINITY;
-  }
-  if (tid == 0) out_counts[b] = cnt;
+  const int cnt = block_group_rule(
+      keys, Rp2, ONE ? 1 : m, [&](int i) { return doc_group[rank_key_id(keys[i])]; }, [&](int i) { return keys[i]; },
+      gkeys, kept);
+  block_write_ranking(gkeys, cnt, top_k, doc_id_base, out_ids, out_scores, out_counts, b);
 }
 
 // The group maximum of exact search.  Row b of `scores` (stride cols) holds n[b] scores (n == NULL: all cols), entry p
@@ -189,159 +127,29 @@ group_round_max_kernel(const float* __restrict__ scores, const int32_t* __restri
   group_max(scores, cand, n, cols, B, doc_group, n_groups, row_stride, bound, gkeys);
 }
 
-// Digits of the 64-bit key for the radix passes, most significant first (K3b's)
-__constant__ int GS_LO[6] = {53, 42, 32, 21, 10, 0};
-__constant__ int GS_W[6] = {11, 11, 10, 11, 11, 10};
-constexpr int GS_BCAP = 2048;  // capacity of the threshold bucket on the fast path
+// group_select's entries: the keys of a gkeys row, 0 for an empty one
+struct RowKeys {
+  static constexpr bool dense = false;
+  const unsigned long long* row;
+  __device__ static uint64_t empty() { return 0; }
+  __device__ uint64_t load(int64_t i) const { return row[i]; }
+  __device__ bool present(uint64_t k) const { return k != 0; }
+  __device__ float value(uint64_t k) const { return rank_key_f32_value(k); }
+  __device__ uint64_t key(uint64_t k, int64_t) const { return k; }
+};
 
 // One CTA per query: the top_k largest non-empty keys of row b of gkeys [B, n_groups], in descending order, written
 // as K6 writes its ranking.  The keys are distinct (each names its own document), so the top_k are the keys at or
-// above the top_k-th.  The steps are K3b's: linear value buckets over the [min, max] score range, and only the
-// threshold bucket ordered by the whole key; radix passes over the key when that bucket is too large.
+// above the top_k-th.
 __global__ void __launch_bounds__(1024)
 group_select_kernel(const unsigned long long* __restrict__ gkeys, int64_t n_groups, int top_k, int Rp2,
                     int64_t doc_id_base, int64_t* __restrict__ out_ids, float* __restrict__ out_scores,
                     int32_t* __restrict__ out_counts) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);  // [Rp2]
-  __shared__ int hist[SEL_BINS];
-  __shared__ int s_need, s_hd, s_cnt, s_cnt2, s_fast, s_nz;
-  __shared__ uint64_t s_prefix, s_mask;
-  __shared__ uint64_t bkeys[GS_BCAP];
-  __shared__ float s_red[64];
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
-  const unsigned long long* row = gkeys + int64_t(b) * n_groups;
-  float mn = INFINITY, mx = -INFINITY;
-  int nz = 0;
-  for (int64_t i = tid; i < n_groups; i += 1024) {
-    const uint64_t k = row[i];
-    if (k) {
-      const float v = rank_key_f32_value(k);
-      mn = fminf(mn, v);
-      mx = fmaxf(mx, v);
-      ++nz;
-    }
-  }
-  for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
-  if (tid == 0) {
-    s_cnt = 0;
-    s_cnt2 = 0;
-    s_fast = 0;
-    s_nz = 0;
-  }
-  block_min_max(mn, mx, s_red);
-  if (nz) atomicAdd(&s_nz, nz);
-  __syncthreads();
-  const int64_t n_nz = s_nz;
-  if (n_nz <= top_k) {  // every non-empty group is selected
-    for (int64_t i = tid; i < n_groups; i += 1024) {
-      const uint64_t k = row[i];
-      if (k) keys[atomicAdd(&s_cnt, 1)] = k;
-    }
-    __syncthreads();
-  } else {
-    const float range = mx - mn;
-    const bool usable = range > 0.f && range < 3.0e38f;
-    const float scale = usable ? float(SEL_BINS - 1) / range : 0.f;
-    if (usable) {
-      for (int64_t i = tid; i < n_groups; i += 1024) {
-        const uint64_t k = row[i];
-        if (k) atomicAdd(&hist[value_bucket(rank_key_f32_value(k), mn, scale)], 1);
-      }
-      __syncthreads();
-      int hd, rest;
-      if (tid < 32 && warp_find_bucket(hist, SEL_BINS, top_k, &hd, &rest)) {
-        s_need = rest;
-        s_hd = hd;
-        s_fast = hist[hd] <= GS_BCAP ? 1 : 0;
-      }
-      __syncthreads();
-      if (s_fast) {
-        const int t = s_hd;
-        for (int64_t i = tid; i < n_groups; i += 1024) {
-          const uint64_t k = row[i];
-          if (k) {
-            const int bk = value_bucket(rank_key_f32_value(k), mn, scale);
-            if (bk > t) {
-              keys[atomicAdd(&s_cnt, 1)] = k;  // fewer than top_k of these
-            } else if (bk == t) {
-              bkeys[atomicAdd(&s_cnt2, 1)] = k;  // at most GS_BCAP of these
-            }
-          }
-        }
-        __syncthreads();
-        const int c2 = s_cnt2, need2 = s_need;
-        for (int i = c2 + tid; i < GS_BCAP; i += 1024) bkeys[i] = 0ull;
-        __syncthreads();
-        block_sort_desc(bkeys, GS_BCAP);
-        const int c1 = s_cnt;
-        for (int i = tid; i < need2; i += 1024) keys[c1 + i] = bkeys[i];
-        __syncthreads();
-        if (tid == 0) s_cnt = c1 + need2;  // == top_k
-        __syncthreads();
-      }
-    }
-    if (!s_fast) {  // radix passes over the 64-bit key: the threshold key T, then every key >= T
-      if (tid == 0) {
-        s_need = top_k;
-        s_prefix = 0;
-        s_mask = 0;
-        s_cnt = 0;
-      }
-      for (int pass = 0; pass < 6; ++pass) {
-        const int lo = GS_LO[pass], width = GS_W[pass];
-        const uint64_t dmask = (1ull << width) - 1ull;
-        for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
-        __syncthreads();
-        const uint64_t prefix = s_prefix, mask = s_mask;
-        const int64_t n_up = (n_groups + 1023) / 1024 * 1024;
-        for (int64_t i = tid; i < n_up; i += 1024) {
-          const uint64_t k = i < n_groups ? row[i] : 0ull;
-          const bool in = k != 0 && (k & mask) == prefix;
-          const unsigned act = __ballot_sync(0xffffffffu, in);
-          if (in) {
-            const int bin = int((k >> lo) & dmask);
-            const unsigned peers = __match_any_sync(act, bin);
-            if (lane == __ffs(peers) - 1) atomicAdd(&hist[bin], __popc(peers));
-          }
-        }
-        __syncthreads();
-        int d, rest;
-        if (tid < 32 && warp_find_bucket(hist, 1 << width, s_need, &d, &rest)) {
-          s_need = rest;
-          s_hd = hist[d];
-          s_prefix = prefix | (uint64_t(d) << lo);
-          s_mask = mask | (dmask << lo);
-        }
-        __syncthreads();
-        if (s_hd == s_need) break;  // the whole bucket is selected
-      }
-      const uint64_t T = s_prefix;  // unprocessed low bits are zero
-      for (int64_t i = tid; i < n_groups; i += 1024) {
-        const uint64_t k = row[i];
-        if (k && k >= T) {
-          const int pos = atomicAdd(&s_cnt, 1);
-          if (pos < Rp2) keys[pos] = k;
-        }
-      }
-      __syncthreads();
-    }
-  }
-  const int cnt = min(s_cnt, top_k);
-  for (int i = cnt + tid; i < Rp2; i += 1024) keys[i] = 0ull;
-  __syncthreads();
-  block_sort_desc(keys, Rp2);
-  for (int i = tid; i < top_k; i += 1024) {
-    int64_t id = -1;
-    float sc = -INFINITY;
-    if (i < cnt) {
-      id = doc_id_base + int64_t(rank_key_id(keys[i]));
-      sc = rank_key_f32_value(keys[i]);
-    }
-    out_ids[int64_t(b) * top_k + i] = id;
-    out_scores[int64_t(b) * top_k + i] = sc;
-  }
-  if (tid == 0) out_counts[b] = cnt;
+  const int b = blockIdx.x;
+  const int cnt = block_select_keys(RowKeys{gkeys + int64_t(b) * n_groups}, n_groups, top_k, keys, Rp2);
+  block_write_ranking(keys, cnt, top_k, doc_id_base, out_ids, out_scores, out_counts, b);
 }
 
 // The grouped shard merge, one CTA per query, over the gathered records in k6_merge_kernel's layout
@@ -351,8 +159,9 @@ group_select_kernel(const unsigned long long* __restrict__ gkeys, int64_t n_grou
 //   3. keep sorted position i when fewer than m documents of its group come before it (global_group by global id);
 //   4. write the first top_k kept ones.
 // Shared memory, 11 bytes per record slot (180 KB at the merge limit): keys [P] (the approximate keys, then the exact
-// keys of the Kp2 = next_pow2(min(n_keep, total)) first slots, then the (group, position) keys), pay [P] (the record
-// index of each slot, carried through both sorts) and kept [P].  Ids and scores are read back from the records.
+// keys of the Kp2 = next_pow2(min(n_keep, total)) first slots, then the (group, position) keys, then the kept keys),
+// pay [P] (the record index of each slot, carried through both sorts) and kept [P].  The kept keys are rebuilt from
+// the records.
 __global__ void __launch_bounds__(1024)
 k6_merge_grouped_kernel(const fpb_record* __restrict__ all_groups, int n_shards, int B, int R, int P, int Kp2,
                         int n_keep, int top_k, const int32_t* __restrict__ global_group, int64_t n_total_docs, int m,
@@ -362,41 +171,15 @@ k6_merge_grouped_kernel(const fpb_record* __restrict__ all_groups, int n_shards,
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);  // [P]
   uint16_t* pay = reinterpret_cast<uint16_t*>(keys + P);    // [P] record index (P <= 2^14)
   unsigned char* kept = reinterpret_cast<unsigned char*>(pay + P);  // [P]
-  __shared__ int warp_sums[32];
-  __shared__ int s_valid, s_total;
-  const int b = blockIdx.x % B, tid = threadIdx.x;
+  const int b = blockIdx.x % B;
   const fpb_record* all = all_groups + int64_t(blockIdx.x / B) * n_shards * B * R;
-  out_ids += int64_t(blockIdx.x - b) * top_k;
-  out_scores += int64_t(blockIdx.x - b) * top_k;
-  out_counts += blockIdx.x - b;
   const int total = n_shards * R;
-  auto record = [&](int j) -> const fpb_record& { return all[(int64_t(j / R) * B + b) * R + j % R]; };
+  auto record = [&](int j) -> const fpb_record& { return merge_record(all, B, R, b, j); };
   // 1. the global pruning rule, as k6_merge_kernel applies it
   const bool prune = n_keep < total;
-  int cand = total;  // slots [0, cand) hold the candidate records
-  if (prune) {
-    if (tid == 0) s_valid = 0;
-    __syncthreads();
-    int local_valid = 0;
-    for (int i = tid; i < P; i += 1024) {
-      uint64_t k = 0;
-      if (i < total) {
-        const fpb_record rec = record(i);
-        if (rec.doc_id >= 0) {
-          k = rank_key_f32(rec.approx, uint32_t(rec.doc_id));
-          ++local_valid;
-        }
-      }
-      keys[i] = k;
-      pay[i] = uint16_t(i);
-    }
-    if (local_valid) atomicAdd(&s_valid, local_valid);
-    __syncthreads();
-    block_sort_desc(keys, P, pay);
-    cand = min(s_valid, n_keep);
-  }
+  const int cand = prune ? block_merge_prune(all, B, R, b, total, P, n_keep, keys, pay) : total;  // slots [0, cand)
   // 2. the canonical order of the candidates; a padding record, or one of no valid group, is left out
-  for (int i = tid; i < Kp2; i += 1024) {
+  for (int i = threadIdx.x; i < Kp2; i += 1024) {
     uint64_t k = 0;
     if (i < cand) {
       const int j = prune ? int(pay[i]) : i;
@@ -406,48 +189,18 @@ k6_merge_grouped_kernel(const fpb_record* __restrict__ all_groups, int n_shards,
       pay[i] = uint16_t(j);
     }
     keys[i] = k;
-    kept[i] = 0;
   }
   __syncthreads();
   block_sort_desc(keys, Kp2, pay);
-  // 3. (group, rank position) keys in place of the exact keys: sorted descending, a group's entries are adjacent and
-  // its best position first, so entry j is among its group's m best when the entry m places before it is of another
-  for (int i = tid; i < Kp2; i += 1024) {
-    uint64_t g = 0;
-    if (keys[i]) g = (uint64_t(uint32_t(global_group[record(pay[i]).doc_id])) << 32) | (0xffffffffu - uint32_t(i));
-    keys[i] = g;
-  }
-  __syncthreads();
-  block_sort_desc(keys, Kp2);
-  for (int j = tid; j < Kp2; j += 1024) {
-    const uint64_t g = keys[j];
-    if (g && (j < m || (keys[j - m] >> 32) != (g >> 32))) kept[0xffffffffu - uint32_t(g)] = 1;
-  }
-  __syncthreads();
-  // 4. ordered compaction of the kept positions: thread t owns positions [t * per, (t + 1) * per)
-  const int per = Kp2 > 1024 ? Kp2 / 1024 : 1;
-  const int i0 = tid * per;
-  int c = 0;
-  for (int u = 0; u < per; ++u) c += (i0 + u < Kp2 && kept[i0 + u]) ? 1 : 0;
-  int pos = block_exclusive_scan(c, warp_sums, &s_total);
-  for (int u = 0; u < per; ++u) {
-    const int i = i0 + u;
-    if (i < Kp2 && kept[i]) {
-      if (pos < top_k) {
+  // 3. the group rule, its (group, position) keys in place of the exact keys, which are read back from the records
+  const int cnt = block_group_rule(
+      keys, Kp2, m, [&](int i) { return global_group[record(pay[i]).doc_id]; },
+      [&](int i) {
         const fpb_record rec = record(pay[i]);
-        const uint64_t k = rank_key_f32(rec.exact, uint32_t(rec.doc_id));  // the value K6 writes (-0 as +0)
-        out_ids[int64_t(b) * top_k + pos] = int64_t(rank_key_id(k));
-        out_scores[int64_t(b) * top_k + pos] = rank_key_f32_value(k);
-      }
-      ++pos;
-    }
-  }
-  const int cnt = min(top_k, s_total);
-  for (int i = cnt + tid; i < top_k; i += 1024) {
-    out_ids[int64_t(b) * top_k + i] = -1;
-    out_scores[int64_t(b) * top_k + i] = -INFINITY;
-  }
-  if (tid == 0) out_counts[b] = cnt;
+        return rank_key_f32(rec.exact, uint32_t(rec.doc_id));  // the value K6 writes (-0 as +0)
+      },
+      keys, kept);
+  block_write_ranking(keys, cnt, top_k, 0, out_ids, out_scores, out_counts, blockIdx.x);
 }
 
 __global__ void results_to_records_kernel(const int64_t* __restrict__ ids, const float* __restrict__ scores, int64_t n,

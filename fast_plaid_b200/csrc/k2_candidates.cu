@@ -5,6 +5,7 @@
 // Here every probed list is OR-ed into a per-query bitmap over the local doc ids and the
 // bitmap is compacted in index order, which yields the sorted-unique id list directly.
 #include "kernels.h"
+#include "select.cuh"
 
 namespace {
 
@@ -53,20 +54,20 @@ k2_mark_wide_kernel(const int32_t* __restrict__ cells, int slots, const int64_t*
   }
 }
 
-// one CTA per query: ordered compaction of the bitmap into cand[b][0..n_cand[b])
+// One CTA per row b: the ids of the set bits of row b of `bitmap` (ANDed with row b of `mask`, when given) in index
+// order into out[b][0, cap), and their number, at most cap, into n_out[b].  The bits past the cap-th are dropped, so an
+// understated cap cuts a list short instead of writing past it.
 __global__ void __launch_bounds__(1024)
 k2_compact_kernel(const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ mask, int bitmap_words,
-                  int32_t* __restrict__ cand, int cand_cap, int32_t* __restrict__ n_cand) {
+                  int32_t* __restrict__ out, int cap, int32_t* __restrict__ n_out) {
   __shared__ int warp_sums[32];
-  __shared__ int s_base;
-  const int b = blockIdx.x;
+  __shared__ int s_total;
+  const int b = blockIdx.x, tid = threadIdx.x;
   const uint32_t* bm = bitmap + int64_t(b) * bitmap_words;
   const uint32_t* mk = mask ? mask + int64_t(b) * bitmap_words : nullptr;  // subset intersection (search.rs:544-547)
-  int32_t* out = cand + int64_t(b) * cand_cap;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_base = 0;
-  __syncthreads();
-  for (int w0 = 0; w0 < bitmap_words; w0 += 4096) {
+  int32_t* o = out + int64_t(b) * cap;
+  int base = 0;  // set bits of the rounds before, the same in every thread
+  for (int w0 = 0; w0 < bitmap_words && base < cap; w0 += 4096) {
     const int wi = w0 + tid * 4;  // 4 consecutive words per thread keeps the output ordered
     uint32_t w[4];
 #pragma unroll
@@ -74,42 +75,21 @@ k2_compact_kernel(const uint32_t* __restrict__ bitmap, const uint32_t* __restric
       w[u] = (wi + u < bitmap_words) ? bm[wi + u] : 0u;
       if (mk && wi + u < bitmap_words) w[u] &= mk[wi + u];
     }
-    const int c = __popc(w[0]) + __popc(w[1]) + __popc(w[2]) + __popc(w[3]);
-    int incl = c;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, incl, off);
-      if (lane >= off) incl += v;
-    }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      int ws = warp_sums[lane];
-      int wincl = ws;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, wincl, off);
-        if (lane >= off) wincl += v;
-      }
-      warp_sums[lane] = wincl - ws;  // exclusive
-    }
-    __syncthreads();
-    const int base = s_base;
-    int pos = base + warp_sums[warp] + incl - c;
+    int pos = base + block_exclusive_scan(__popc(w[0]) + __popc(w[1]) + __popc(w[2]) + __popc(w[3]), warp_sums,
+                                          &s_total);
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       uint32_t x = w[u];
-      while (x) {
+      while (x && pos < cap) {
         const int bit = __ffs(x) - 1;
         x &= x - 1;
-        out[pos++] = (wi + u) * 32 + bit;
+        o[pos++] = (wi + u) * 32 + bit;
       }
     }
-    __syncthreads();
-    if (tid == 1023) s_base = base + warp_sums[31] + incl;  // total of this round
-    __syncthreads();
+    base += s_total;
+    __syncthreads();  // the next round's scan rewrites warp_sums and s_total
   }
-  if (tid == 0) n_cand[b] = s_base;
+  if (tid == 0) n_out[b] = min(base, cap);
 }
 
 // The subset's documents as a bitmap and the centroids occurring in them as a second bitmap

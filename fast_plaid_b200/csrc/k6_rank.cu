@@ -15,28 +15,27 @@ namespace {
 // the reference's topk(n_full) followed by topk(n_full/4) up to tie order.
 // ---------------------------------------------------------------------------------------
 
-// Digits of the 64-bit key, most significant first: 11+11+10 bits cover the score, the rest
-// only matters when scores tie at the threshold.
-__constant__ int K3B_LO[6] = {53, 42, 32, 21, 10, 0};
-__constant__ int K3B_W[6] = {11, 11, 10, 11, 11, 10};
-constexpr int K3B_VPT = 4;  // independent loads in flight per thread
-constexpr int K3B_BCAP = 2048;  // capacity of the threshold bucket on the fast path
+// K3b's entries: candidate i of a row and its score
+struct CandidateScores {
+  static constexpr bool dense = true;
+  const float* scores;
+  __device__ static float empty() { return NAN; }
+  __device__ float load(int i) const { return scores[i]; }
+  __device__ bool present(float) const { return true; }
+  __device__ float value(float v) const { return v; }
+  __device__ uint64_t key(float v, int i) const { return rank_key_f32(v, uint32_t(i)); }
+};
 
 // Row b of `approx` (stride cand_cap) holds the scores of n_cand[b] candidates, candidate i being document
-// cand[b, i].  cand == NULL: all cand_cap entries of the row are candidates, candidate i being document i.
-__global__ void __launch_bounds__(1024)
+// cand[b, i].  cand == NULL: all cand_cap entries of the row are candidates, candidate i being document i.  Two CTAs
+// per SM: 32 registers, which the selection fits without spilling.
+__global__ void __launch_bounds__(1024, 2)
 k3b_select_kernel(const float* __restrict__ approx, const int32_t* __restrict__ cand, int cand_cap,
                   const int32_t* __restrict__ n_cand, int n_dec, int Rp2, int32_t* __restrict__ rerank,
                   float* __restrict__ rerank_approx, int32_t* __restrict__ n_rerank) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);
-  __shared__ int hist[SEL_BINS];
-  __shared__ int s_need, s_hd, s_cnt;
-  __shared__ uint64_t s_prefix, s_mask;
-  __shared__ uint64_t bkeys[K3B_BCAP];  // fast path: keys of the threshold bucket
-  __shared__ float s_red[64];
-  __shared__ int s_cnt2, s_fast;
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+  const int b = blockIdx.x, tid = threadIdx.x;
   const int n = cand ? n_cand[b] : cand_cap;
   const float* ab = approx + int64_t(b) * cand_cap;
   const int32_t* cb = cand ? cand + int64_t(b) * cand_cap : nullptr;
@@ -50,160 +49,7 @@ k3b_select_kernel(const float* __restrict__ approx, const int32_t* __restrict__ 
     if (tid == 0) n_rerank[b] = n;
     return;
   }
-  // ---- fast path: 2048 buckets over the VALUE range [min, max] of this query's scores ----
-  // The radix passes below start from the top bits of the float key, where the scores of one query share
-  // sign, exponent and the leading mantissa bits: a handful of hot bins, so every element pays a ballot +
-  // match_any + contended shared atomic, three passes long (0.49 ms on cfg-3).  A linear bucketisation of the
-  // actual value range spreads the scores, one histogram pass isolates the threshold bucket, and only that
-  // bucket (typically n / 2048 elements) is ordered by the exact 64-bit key.  value_bucket() is monotone, so
-  // every element of a higher bucket is strictly larger: the selection is exactly the same.
-  {
-    constexpr int FV = 8;  // independent loads in flight per thread
-    float mn = INFINITY, mx = -INFINITY;
-    for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
-      float v[FV];
-#pragma unroll
-      for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : NAN;  // fmin/fmax skip NaN
-#pragma unroll
-      for (int u = 0; u < FV; ++u) {
-        mn = fminf(mn, v[u]);
-        mx = fmaxf(mx, v[u]);
-      }
-    }
-    for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
-    if (tid == 0) {
-      s_cnt = 0;
-      s_cnt2 = 0;
-      s_fast = 0;
-    }
-    block_min_max(mn, mx, s_red);
-    const float range = mx - mn;
-    // finite, non-degenerate range (NaN / inf scores or all-equal scores take the radix path)
-    const bool usable = range > 0.f && range < 3.0e38f;
-    const float scale = usable ? float(SEL_BINS - 1) / range : 0.f;
-    if (usable) {
-      for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
-        float v[FV];
-#pragma unroll
-        for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : 0.f;
-#pragma unroll
-        for (int u = 0; u < FV; ++u)
-          if (i0 + u * 1024 < n) atomicAdd(&hist[value_bucket(v[u], mn, scale)], 1);
-      }
-      __syncthreads();
-      int hd, rest;
-      if (tid < 32 && warp_find_bucket(hist, SEL_BINS, n_dec, &hd, &rest)) {
-        s_need = rest;
-        s_hd = hd;
-        s_fast = hist[hd] <= K3B_BCAP ? 1 : 0;
-      }
-      __syncthreads();
-      if (s_fast) {
-        const int t = s_hd;
-        for (int i0 = tid; i0 < n; i0 += 1024 * FV) {
-          float v[FV];
-#pragma unroll
-          for (int u = 0; u < FV; ++u) v[u] = (i0 + u * 1024 < n) ? ab[i0 + u * 1024] : 0.f;
-#pragma unroll
-          for (int u = 0; u < FV; ++u) {
-            const int i = i0 + u * 1024;
-            if (i < n) {
-              const int bk = value_bucket(v[u], mn, scale);
-              if (bk > t) {
-                keys[atomicAdd(&s_cnt, 1)] = rank_key_f32(v[u], uint32_t(i));    // fewer than n_dec of these
-              } else if (bk == t) {
-                bkeys[atomicAdd(&s_cnt2, 1)] = rank_key_f32(v[u], uint32_t(i));  // at most K3B_BCAP of these
-              }
-            }
-          }
-        }
-        __syncthreads();
-        const int c2 = s_cnt2, need2 = s_need;
-        for (int i = c2 + tid; i < K3B_BCAP; i += 1024) bkeys[i] = 0ull;
-        __syncthreads();
-        block_sort_desc(bkeys, K3B_BCAP);
-        const int c1 = s_cnt;
-        for (int i = tid; i < need2; i += 1024) keys[c1 + i] = bkeys[i];
-        __syncthreads();
-        if (tid == 0) s_cnt = c1 + need2;  // == n_dec
-        __syncthreads();
-      }
-    }
-  }
-  if (!s_fast) {  // ---- radix passes over the 64-bit key: the threshold key T, then every key >= T ----
-    if (tid == 0) {
-      s_need = n_dec;
-      s_prefix = 0;
-      s_mask = 0;
-    }
-    const int stride = 1024 * K3B_VPT;
-    const int n_up = (n + stride - 1) / stride * stride;
-    for (int pass = 0; pass < 6; ++pass) {
-      const int lo = K3B_LO[pass], width = K3B_W[pass];
-      const uint64_t dmask = (1ull << width) - 1ull;
-      for (int i = tid; i < SEL_BINS; i += 1024) hist[i] = 0;
-      __syncthreads();
-      const uint64_t prefix = s_prefix, mask = s_mask;
-      for (int i0 = tid; i0 < n_up; i0 += stride) {
-        float v[K3B_VPT];
-#pragma unroll
-        for (int u = 0; u < K3B_VPT; ++u) {
-          const int i = i0 + u * 1024;
-          v[u] = (i < n) ? ab[i] : 0.f;
-        }
-#pragma unroll
-        for (int u = 0; u < K3B_VPT; ++u) {
-          const int i = i0 + u * 1024;
-          const bool valid = i < n;
-          const uint64_t key = valid ? rank_key_f32(v[u], uint32_t(i)) : 0ull;
-          const bool in = valid && ((key & mask) == prefix);
-          const unsigned act = __ballot_sync(0xffffffffu, in);
-          if (in) {
-            const int bin = int((key >> lo) & dmask);
-            const unsigned peers = __match_any_sync(act, bin);
-            if (lane == __ffs(peers) - 1) atomicAdd(&hist[bin], __popc(peers));
-          }
-        }
-      }
-      __syncthreads();
-      int d, rest;
-      if (tid < 32 && warp_find_bucket(hist, 1 << width, s_need, &d, &rest)) {
-        s_need = rest;
-        s_hd = hist[d];
-        s_prefix = prefix | (uint64_t(d) << lo);
-        s_mask = mask | (dmask << lo);
-      }
-      __syncthreads();
-      if (s_hd == s_need) break;  // the whole bucket is selected
-    }
-    const uint64_t T = s_prefix;  // unprocessed low bits are zero
-    if (tid == 0) s_cnt = 0;
-    __syncthreads();
-    for (int i0 = tid; i0 < n_up; i0 += stride) {
-      float v[K3B_VPT];
-#pragma unroll
-      for (int u = 0; u < K3B_VPT; ++u) {
-        const int i = i0 + u * 1024;
-        v[u] = (i < n) ? ab[i] : 0.f;
-      }
-#pragma unroll
-      for (int u = 0; u < K3B_VPT; ++u) {
-        const int i = i0 + u * 1024;
-        if (i < n) {
-          const uint64_t key = rank_key_f32(v[u], uint32_t(i));
-          if (key >= T) {
-            const int pos = atomicAdd(&s_cnt, 1);
-            if (pos < Rp2) keys[pos] = key;
-          }
-        }
-      }
-    }
-  }
-  __syncthreads();
-  const int cnt = min(s_cnt, Rp2);
-  for (int i = cnt + tid; i < Rp2; i += 1024) keys[i] = 0ull;
-  __syncthreads();
-  block_sort_desc(keys, Rp2);
+  block_select_keys(CandidateScores{ab}, n, n_dec, keys, Rp2);
   for (int r = tid; r < n_dec; r += 1024) {
     const uint32_t idx = rank_key_id(keys[r]);
     rr[r] = cb ? cb[idx] : int32_t(idx);
@@ -228,18 +74,7 @@ k6_rank_kernel(const float* __restrict__ exact, const int32_t* __restrict__ rera
   }
   __syncthreads();
   block_sort_desc(keys, Rp2);
-  const int cnt = min(top_k, n);
-  for (int i = tid; i < top_k; i += 1024) {
-    int64_t id = -1;
-    float sc = -INFINITY;
-    if (i < cnt) {
-      id = doc_id_base + int64_t(rank_key_id(keys[i]));
-      sc = rank_key_f32_value(keys[i]);
-    }
-    out_ids[int64_t(b) * top_k + i] = id;
-    out_scores[int64_t(b) * top_k + i] = sc;
-  }
-  if (tid == 0) out_counts[b] = cnt;
+  block_write_ranking(keys, n, top_k, doc_id_base, out_ids, out_scores, out_counts, b);
 }
 
 __global__ void emit_records_kernel(const float* __restrict__ exact, const float* __restrict__ rerank_approx,
@@ -271,59 +106,22 @@ k6_merge_kernel(const fpb_record* __restrict__ all_groups, int n_shards, int B, 
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);  // [P]
   uint64_t* keys2 = keys + P;                               // [Rp2]
   uint16_t* pay = reinterpret_cast<uint16_t*>(keys2 + Rp2);  // [P] record index carried through the sort (P <= 2^14)
-  __shared__ int s_valid;
   // query blockIdx.x of the whole batch = query `b` of query group blockIdx.x / B, whose records are the
   // [n_shards, B, R] block of that group (one group: the block index is the query)
-  const int b = blockIdx.x % B, tid = threadIdx.x;
+  const int b = blockIdx.x % B;
   const fpb_record* all = all_groups + int64_t(blockIdx.x / B) * n_shards * B * R;
-  out_ids += int64_t(blockIdx.x - b) * top_k;
-  out_scores += int64_t(blockIdx.x - b) * top_k;
-  out_counts += blockIdx.x - b;
-  const int total = n_shards * R;
-  if (tid == 0) s_valid = 0;
-  __syncthreads();
-  int local_valid = 0;
-  for (int i = tid; i < P; i += 1024) {
-    uint64_t k = 0;
-    if (i < total) {
-      const int s = i / R, r = i % R;
-      const fpb_record rec = all[(int64_t(s) * B + b) * R + r];
-      if (rec.doc_id >= 0) {
-        k = rank_key_f32(rec.approx, uint32_t(rec.doc_id));
-        ++local_valid;
-      }
-    }
-    keys[i] = k;
-    pay[i] = uint16_t(i);
-  }
-  if (local_valid) atomicAdd(&s_valid, local_valid);
-  __syncthreads();
-  block_sort_desc(keys, P, pay);
-  const int keep = min(s_valid, R);
-  for (int i = tid; i < Rp2; i += 1024) {
+  const int keep = block_merge_prune(all, B, R, b, n_shards * R, P, R, keys, pay);
+  for (int i = threadIdx.x; i < Rp2; i += 1024) {
     uint64_t k2 = 0;
     if (i < keep) {
-      const int j = int(pay[i]);
-      const int s = j / R, r = j % R;
-      const fpb_record rec = all[(int64_t(s) * B + b) * R + r];
+      const fpb_record rec = merge_record(all, B, R, b, pay[i]);
       k2 = rank_key_f32(rec.exact, uint32_t(rec.doc_id));
     }
     keys2[i] = k2;
   }
   __syncthreads();
   block_sort_desc(keys2, Rp2);
-  const int cnt = min(top_k, keep);
-  for (int i = tid; i < top_k; i += 1024) {
-    int64_t id = -1;
-    float sc = -INFINITY;
-    if (i < cnt) {
-      id = int64_t(rank_key_id(keys2[i]));
-      sc = rank_key_f32_value(keys2[i]);
-    }
-    out_ids[int64_t(b) * top_k + i] = id;
-    out_scores[int64_t(b) * top_k + i] = sc;
-  }
-  if (tid == 0) out_counts[b] = cnt;
+  block_write_ranking(keys2, keep, top_k, 0, out_ids, out_scores, out_counts, blockIdx.x);
 }
 
 // two-step sharded search, step 1: 64-bit keys of the local pruned list
@@ -348,7 +146,7 @@ apply_threshold_kernel(const uint64_t* __restrict__ all, int n_shards, int rank,
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw);
   __shared__ int warp_sums[32];
   __shared__ int s_base;
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int b = blockIdx.x, tid = threadIdx.x;
   const int total = n_shards * R;
   for (int i = tid; i < P; i += 1024) {
     uint64_t k = 0;
@@ -383,27 +181,8 @@ apply_threshold_kernel(const uint64_t* __restrict__ all, int n_shards, int rank,
     }
     c += keep[u] ? 1 : 0;
   }
-  int incl = c;
-#pragma unroll
-  for (int off = 1; off < 32; off <<= 1) {
-    const int v = __shfl_up_sync(0xffffffffu, incl, off);
-    if (lane >= off) incl += v;
-  }
-  if (lane == 31) warp_sums[warp] = incl;
-  __syncthreads();  // also: everybody has read T / keys[] before tmp_* overwrites the buffer
-  if (warp == 0) {
-    const int ws = warp_sums[lane];
-    int wincl = ws;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, wincl, off);
-      if (lane >= off) wincl += v;
-    }
-    warp_sums[lane] = wincl - ws;
-    if (lane == 31) s_base = wincl;
-  }
-  __syncthreads();
-  int pos = warp_sums[warp] + incl - c;
+  // the scan's first barrier also orders every read of T / keys[] before tmp_* overwrites the buffer
+  int pos = block_exclusive_scan(c, warp_sums, &s_base);
 #pragma unroll
   for (int u = 0; u < PER; ++u) {
     if (keep[u]) {
